@@ -62,13 +62,26 @@ Info bfsFused(Vector<float>* v, const Matrix<a>* A, Index s, Descriptor* desc, i
 
   const size_t nwords = (static_cast<size_t>(n) + 31)/32;
   const size_t words_bytes = ((nwords*sizeof(unsigned int) + 255)/256)*256;
+  const size_t nchunks = (nwords + 31)/32;
+  const size_t counters_bytes = GB_BFS_NCOUNTERS*sizeof(unsigned long long);
+  const size_t heavy_bytes = GB_BFS_HEAVY_CAP*sizeof(Index);
+  const size_t walk_bytes = nchunks*GB_BFS_CHUNK*sizeof(Index);
   unsigned char* base = reinterpret_cast<unsigned char*>(desc->scratch(GB_SCRATCH_BFS,
-      4*words_bytes + 256 + GB_BFS_HEAVY_CAP*sizeof(Index)));
+      4*words_bytes + counters_bytes + heavy_bytes + walk_bytes +
+      nchunks*(sizeof(int) + sizeof(Index))));
   BfsFusedArgs args;
   args.push_ptr = S->d_csrRowPtr_;  args.push_ind = S->d_csrColInd_;
   args.pull_ptr = S->d_cscColPtr_;  args.pull_ind = S->d_cscRowInd_;
   args.pull_first = first;
+  // Rows without in-neighbours may count as visited from the start only when they
+  // have no out-neighbours either: a visited row is taken to have been expanded, so
+  // in a directed graph one that points somewhere would let the pull discover what
+  // it points at.  When the pulled structure is the pushed one, that is the same
+  // bitmap; otherwise the pushed structure's empty rows are ANDed in.
+  const bool same_structure = S->symmetric_ || S->d_cscColPtr_ == S->d_csrRowPtr_;
   args.pull_empty = pullEmptyRowBits(first, n);
+  args.push_empty = same_structure ? NULL : pullEmptyRowBits(
+      pullFirstNeighbours(S, 0, S->d_csrRowPtr_, S->d_csrColInd_, n), n);
   args.n = n;
   args.source = s;
   args.max_levels = desc->max_niter_;
@@ -82,22 +95,35 @@ Info bfsFused(Vector<float>* v, const Matrix<a>* A, Index s, Descriptor* desc, i
   args.frontier   = reinterpret_cast<unsigned int*>(base + 2*words_bytes);
   args.next       = reinterpret_cast<unsigned int*>(base + 3*words_bytes);
   args.counters   = reinterpret_cast<unsigned long long*>(base + 4*words_bytes);
-  args.heavy      = reinterpret_cast<Index*>(base + 4*words_bytes + 256);
+  args.heavy      = reinterpret_cast<Index*>(base + 4*words_bytes + counters_bytes);
+  args.walk       = reinterpret_cast<Index*>(base + 4*words_bytes + counters_bytes +
+                                             heavy_bytes);
+  args.walk_count = reinterpret_cast<int*>(base + 4*words_bytes + counters_bytes +
+                                           heavy_bytes + walk_bytes);
+  args.walk_chunks = reinterpret_cast<Index*>(args.walk_count + nchunks);
 
-  static const int minb = getEnv("GB200_BFS_MINB", 2);
-  static int resident = 0;               // CTAs that fit at once (cooperative launch)
-  void (*kernel)(BfsFusedArgs) = (minb >= 2) ? bfsFusedKernel<GB_BFS_MINB> : bfsFusedKernel<1>;
+  static const int trace = getEnv("GB200_BFS_TRACE", 0);
+  args.trace = trace;
+
+  // push-only traversals run the instantiation without the pull level, with more
+  // warps per SM
+  const bool push_only = (args.mode == 1);
+  void (*kernel)(BfsFusedArgs) =
+      push_only ? bfsFusedKernel<GB_BFS_PUSH_NT, GB_BFS_PUSH_MINB, false>
+                : bfsFusedKernel<GB_BFS_NT, GB_BFS_MINB, true>;
+  const int nt = push_only ? GB_BFS_PUSH_NT : GB_BFS_NT;
+  static int resident_of[2] = {0, 0};    // CTAs that fit at once (cooperative launch)
+  int& resident = resident_of[push_only ? 1 : 0];
   if (resident == 0) {
     int per_sm = 0;
-    CUDA_CALL(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel,
-        GB_BFS_NT, 0));
+    CUDA_CALL(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, nt, 0));
     resident = per_sm*runtime().sm_count;
     if (resident < 1) return GrB_PANIC;
   }
   void* params[] = { &args };
   profiler().begin(GB_PROF_PULL_BOOL, stream);
   CUDA_CALL(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kernel),
-      dim3(resident), dim3(GB_BFS_NT), params, 0, stream));
+      dim3(resident), dim3(nt), params, 0, stream));
   GB_KERNEL_CHECK();
   profiler().end(GB_PROF_PULL_BOOL, stream, 0.0);
   if (profiler().enabled) {
@@ -110,21 +136,25 @@ Info bfsFused(Vector<float>* v, const Matrix<a>* A, Index s, Descriptor* desc, i
     GB_KERNEL_CHECK();
   }
   v->dense_.touched();
-  static const int trace = getEnv("GB200_BFS_TRACE", 0);
   if (trace) {                           // per-level times of this traversal
-    unsigned long long cells[32];
+    unsigned long long cells[GB_BFS_NCOUNTERS];
     CUDA_CALL(cudaMemcpyAsync(cells, args.counters, sizeof(cells), cudaMemcpyDeviceToHost,
         stream));
     runtime().sync();
     const int levels = static_cast<int>(cells[6] < 15 ? cells[6] : 15);
     fprintf(stderr, "bfs trace: set-up %.1fus",
             1e-3*static_cast<double>((cells[12] >> 1) - cells[28]));
-    for (int l = 1; l <= levels; ++l)
-      fprintf(stderr, " L%d %s %.1fus", l, (cells[12 + l] & 1ull) ? "pull" : "push",
-              1e-3*static_cast<double>((cells[12 + l] >> 1) - (cells[12 + l - 1] >> 1)));
-    fprintf(stderr, " | L2 CTA0: scan %.1fus walk %.1fus parked %llu\n",
-            1e-3*static_cast<double>(cells[29] - (cells[13] >> 1)),
-            1e-3*static_cast<double>(cells[30] - cells[29]), cells[31]);
+    for (int l = 1; l <= levels; ++l) {
+      const unsigned long long start = cells[12 + l - 1] >> 1, end = cells[12 + l] >> 1;
+      if (cells[12 + l] & 1ull)          // pull: scan, walk, rows walked
+        fprintf(stderr, " L%d pull %.1fus (scan %.1f walk %.1f, %llu walked)", l,
+                1e-3*static_cast<double>(end - start),
+                1e-3*static_cast<double>(cells[44 + l] - start),
+                1e-3*static_cast<double>(end - cells[44 + l]), cells[60 + l]);
+      else
+        fprintf(stderr, " L%d push %.1fus", l, 1e-3*static_cast<double>(end - start));
+    }
+    fprintf(stderr, "\n");
   }
   if (depth != NULL) {
     const unsigned long long levels = runtime().fetch(args.counters + 6);

@@ -19,12 +19,27 @@
 //     barrier (an R-MAT source has 10^5..10^6 neighbours).  Discoveries set the
 //     visited bit with atomicOr immediately (same level either way), the winner
 //     writes v and the N bit.
-//   pull level (frontier large): the fused Boolean pull of kernels/spmv_pull.cuh —
-//     a warp owns 4 words of the bitmap per iteration, the first-neighbour summary
-//     decides most rows, the rest walk their list with early exit, probing the
-//     visited bitmap AS OF THE LEVEL'S START (operand reuse, reference
-//     kernels/spmv.hpp:35-41) — and the owner of a word writes N, the merged
-//     visited word of the other copy, v for the discovered rows and clears F.
+//   pull level (frontier large): the fused Boolean pull of kernels/spmv_pull.cuh,
+//     probing the visited bitmap AS OF THE LEVEL'S START (operand reuse, reference
+//     kernels/spmv.hpp:35-41), in two phases separated by a grid barrier:
+//     scan  — warps take chunks of 32 bitmap words (1024 rows) round-robin; a
+//             lane per word, fully visited words only move their bitmap words on;
+//             the open words go through the first-neighbour summary GB_BFS_BATCH
+//             at a time (all their summary loads, then all their probes, in
+//             flight together); rows whose first neighbour is not visited and
+//             that have more are written to the chunk's slice of the walk list,
+//             and a chunk with any to a list of such chunks.
+//             The owner of a word writes N, the merged visited word of the other
+//             copy, v for the discovered rows and clears F.
+//     walk  — warps claim listed chunks from a counter; a lane walks its row's
+//             list GB_BFS_WALK_STEP entries per step, a list still longer than
+//             GB_BFS_WALK_WARP after the first step is walked by the whole warp,
+//             32 entries and one ballot per step.  Discoveries are ORed into N and
+//             the other visited copy.
+//   v is written once per row: the source at set-up, a discovered row when it is
+//   discovered, and after the last level 0 for every row never reached (and, when
+//   max_levels cuts the traversal off, for the rows found at the last level: only
+//   levels 1..max_levels are assigned, as in the operation-by-operation loop).
 // Direction: the reference's ratio rule with hysteresis (vector.hpp:318-342):
 // sparse -> dense when |f|/n > switchpoint and growing, dense -> sparse when
 // <= switchpoint and shrinking; results do not depend on it.
@@ -38,18 +53,34 @@
 namespace graphblas {
 namespace backend {
 
-// CTA shape, measured on RMAT-24: 768 x 2 per SM 0.275 ms, 512 x 3 0.281, 1024 x 2
-// 0.305 (32 registers: the pull loop spills), 1024 x 1 0.297 (no spills, half the
-// warps: the first pull level is latency-bound and takes 40 % longer).
+// CTA shape and register bound, chosen on an H100 (DESIGN.md §4.5, §9)
+// Traversals that may pull: 512 x 2 per SM, the most warps the pull runs at without
+// spilling (64 registers).  Push-only traversals (mode 1) compile the pull out and
+// keep the 768 x 2 shape: the push levels are latency-bound and want the warps.
 #ifndef GB_BFS_NT
-#define GB_BFS_NT     768
+#define GB_BFS_NT     512
 #endif
 #ifndef GB_BFS_MINB
 #define GB_BFS_MINB   2               // resident CTAs per SM the register budget allows
 #endif
+#ifndef GB_BFS_PUSH_NT
+#define GB_BFS_PUSH_NT   768
+#endif
+#ifndef GB_BFS_PUSH_MINB
+#define GB_BFS_PUSH_MINB 2
+#endif
+#ifndef GB_BFS_BATCH
+#define GB_BFS_BATCH  4               // open words whose summaries a warp loads together
+#endif
+#ifndef GB_BFS_WALK_STEP
+#define GB_BFS_WALK_STEP 4            // entries a lane requests at once walking a list
+#endif
+#ifndef GB_BFS_WALK_WARP
+#define GB_BFS_WALK_WARP 32           // list remainder longer than this: walked by a warp
+#endif
 #define GB_BFS_HEAVY  2048            // adjacency longer than this: grid-wide expansion
 #define GB_BFS_HEAVY_CAP 4096         // heavy vertices per level kept in the list
-#define GB_BFS_PARK   4096            // rows a CTA parks for its walking phase per pull level
+#define GB_BFS_CHUNK  1024            // rows of a pull chunk (32 bitmap words)
 
 struct BfsFusedArgs {
   // structure: rows to expand when pushing, rows to inspect when pulling
@@ -57,6 +88,9 @@ struct BfsFusedArgs {
   const Index* pull_ptr;   const Index* pull_ind;     // in-neighbours of a vertex
   const Index* pull_first;                            // first-neighbour summary of pull_*
   const unsigned int* pull_empty;                     // bitmap of rows without in-neighbours
+  const unsigned int* push_empty;                     // ... without out-neighbours; NULL
+                                                      // when the structure is symmetric
+  int   trace;               // count the rows walked per level (GB200_BFS_TRACE)
   Index n;
   Index source;
   int   max_levels;
@@ -75,9 +109,19 @@ struct BfsFusedArgs {
                                   // be reading the cell of L-1),
                                   // [6] levels executed, [7..11] work counters (out),
                                   // [12..27] time at the end of the set-up and of every
-                                  // level (ns << 1 | pulled), for GB200_BFS_TRACE
+                                  // level (ns << 1 | pulled), [28] time at the start,
+                                  // [35..37] walk-chunk claim counters of the pull
+                                  // levels, [38..40] chunks listed in walk_chunks
+                                  // (both rotating like [0..2]),
+                                  // [44..59] time at the scan barrier of every pull
+                                  // level, [60..75] rows it left to walk; [12..] and
+                                  // [44..] for GB200_BFS_TRACE (GB_BFS_NCOUNTERS cells)
   Index*        heavy;            // [GB_BFS_HEAVY_CAP]
+  Index*        walk;             // [nchunks * GB_BFS_CHUNK] rows to walk, by chunk
+  int*          walk_count;       // [nchunks] rows to walk per chunk
+  Index*        walk_chunks;      // [nchunks] the chunks with rows to walk, listed
 };
+#define GB_BFS_NCOUNTERS 128
 
 __device__ __forceinline__ unsigned long long bfsClockNs() {
   unsigned long long t;
@@ -92,17 +136,45 @@ __device__ __forceinline__ bool bfsClaim(unsigned int* visited, Index vtx) {
   return (atomicOr(word, bit) & bit) == 0;
 }
 
-// MINB: CTAs per SM the register allocation must allow (the pull levels are
-// latency-bound: occupancy matters more than a few spilled pointers).
-template <int MINB>
-__global__ void __launch_bounds__(GB_BFS_NT, MINB)
+// The next chunk for this warp from a claim counter (warp-uniform result).
+__device__ __forceinline__ Index bfsClaimChunk(unsigned long long* cell, int lane) {
+  unsigned long long c = 0ull;
+  if (lane == 0) c = atomicAdd(cell, 1ull);
+  return static_cast<Index>(__shfl_sync(GB_FULL_MASK, c, 0));
+}
+
+// The bitmap copies in use: visited[vsel] is the visited set as of the level's
+// start, fsel says whether frontier/next have swapped roles.  Two bits instead of
+// four live pointers (registers are what bounds the CTAs per SM); the pointers are
+// re-read from the kernel parameters.
+__device__ __forceinline__ unsigned int* bfsVis(const BfsFusedArgs& a, int vsel) {
+  return vsel ? a.visited[1] : a.visited[0];
+}
+__device__ __forceinline__ unsigned int* bfsVisOther(const BfsFusedArgs& a, int vsel) {
+  return vsel ? a.visited[0] : a.visited[1];
+}
+__device__ __forceinline__ unsigned int* bfsF(const BfsFusedArgs& a, int fsel) {
+  return fsel ? a.next : a.frontier;
+}
+__device__ __forceinline__ unsigned int* bfsN(const BfsFusedArgs& a, int fsel) {
+  return fsel ? a.frontier : a.next;
+}
+
+// Rows of word w no level can discover and nothing can be discovered from: no
+// in-neighbours, and (in a directed structure) no out-neighbours either.  They count
+// as visited from the start and are unreached unless one is the source.
+__device__ __forceinline__ unsigned int bfsIsolated(const BfsFusedArgs& a, Index w) {
+  return a.pull_empty[w] & (a.push_empty != NULL ? a.push_empty[w] : 0xffffffffu);
+}
+
+// NT x MINB: the CTA shape; PULL = false compiles the pull level out (push-only
+// traversals, a.mode == 1).
+template <int NT, int MINB, bool PULL>
+__global__ void __launch_bounds__(NT, MINB)
 bfsFusedKernel(BfsFusedArgs a) {
   namespace cg = cooperative_groups;
   cg::grid_group grid = cg::this_grid();
-  __shared__ int s_red[GB_BFS_NT/32];
-  __shared__ int s_parked;                 // rows waiting in s_park (pull levels)
-  __shared__ Index s_park[GB_BFS_PARK];
-  if (threadIdx.x == 0) s_parked = 0;
+  __shared__ int s_red[NT/32];
 
   const Index n = a.n;
   const Index nwords = (n + 31) >> 5;
@@ -111,39 +183,40 @@ bfsFusedKernel(BfsFusedArgs a) {
   const Index gthreads = gridDim.x*blockDim.x;
   const Index gwarp = gtid >> 5;
   const Index gwarps = gthreads >> 5;
+  const Index nchunks = (nwords + 31) >> 5;               // pull chunks of 32 words
 
   if (gtid == 0) a.counters[28] = bfsClockNs();
-  // ---- level 0: clear the state, seed the source ---------------------------------
-  for (Index i = gtid; i < n; i += gthreads)
-    a.levels[i] = (i == a.source) ? 1.f : 0.f;
+  // ---- level 0: clear the bitmaps, seed the source (v is written once per row: the
+  // rows never reached get their 0 after the last level) ----------------------------
+  if (gtid == 0) a.levels[a.source] = 1.f;
   for (Index w = gtid; w < nwords; w += gthreads) {
     const unsigned int seed = (w == (a.source >> 5)) ? (1u << (a.source & 31)) : 0u;
     // rows nothing points at count as visited from the start: no level can discover
     // them, and the pull levels would look at them every time
-    a.visited[0][w] = seed | a.pull_empty[w];
+    a.visited[0][w] = seed | bfsIsolated(a, w);
     a.visited[1][w] = 0u; a.frontier[w] = seed; a.next[w] = 0u;
   }
   if (gtid < 12) a.counters[gtid] = 0ull;
+  if (gtid >= 35 && gtid < 41) a.counters[gtid] = 0ull;
+  if (gtid >= 60 && gtid < 76) a.counters[gtid] = 0ull;
   grid.sync();
   if (gtid == 0) a.counters[12] = bfsClockNs() << 1;          // [12..27]: level clock
 
-  unsigned int* vis = a.visited[0];       // visited as of the level's start
-  unsigned int* vis_other = a.visited[1];
-  unsigned int* F = a.frontier;
-  unsigned int* N = a.next;
-  unsigned long long fcount = 1ull;
-  bool dense = (a.mode == 2);             // direction state (storage of the frontier)
+  int vsel = 0;                           // bfsVis / bfsVisOther
+  int fsel = 0;                           // bfsF / bfsN
+  unsigned int fcount = 1u;               // frontier size (<= n)
+  bool dense = PULL && (a.mode == 2);             // direction state (storage of the frontier)
   float prev_ratio = 0.f;
   int inspected = 0;                      // colind entries looked at by this thread
   int pushed_vertices = 0;                // frontier entries expanded (lane 0 counts)
-  long long pushed_edges = 0;             // their adjacency lengths
-  int discovered_pushing = 0;
+  unsigned int pushed_edges = 0u;         // their adjacency lengths (a vertex is pushed
+                                          // once: at most nnz < 2^31 per thread)
   int pull_levels = 0;
   int level = 1;
 
-  for (; level <= a.max_levels && fcount > 0ull; ++level) {
+  for (; level <= a.max_levels && fcount > 0u; ++level) {
     // direction for this level (reference Vector::convert)
-    if (a.mode == 0) {
+    if (PULL && a.mode == 0) {
       const float ratio = static_cast<float>(fcount)/static_cast<float>(n);
       if (!dense) {
         if (ratio > a.switchpoint && ratio > prev_ratio) dense = true; else prev_ratio = ratio;
@@ -156,6 +229,8 @@ bfsFusedKernel(BfsFusedArgs a) {
     if (gtid == 0) {                        // next level's cells
       a.counters[(level + 1) % 3] = 0ull;
       a.counters[3 + (level + 1) % 3] = 0ull;
+      a.counters[35 + (level + 1) % 3] = 0ull;
+      a.counters[38 + (level + 1) % 3] = 0ull;
     }
     const float next_level = static_cast<float>(level + 1);
     int found_here = 0;
@@ -167,8 +242,8 @@ bfsFusedKernel(BfsFusedArgs a) {
       // then walks the non-empty ones.
       for (Index w0 = gwarp*32; w0 < nwords; w0 += gwarps*32) {
         const Index mine = w0 + lane;
-        unsigned int my_bits = (mine < nwords) ? F[mine] : 0u;
-        if (my_bits != 0u) F[mine] = 0u;          // this buffer is the next level's N
+        unsigned int my_bits = (mine < nwords) ? bfsF(a, fsel)[mine] : 0u;
+        if (my_bits != 0u) bfsF(a, fsel)[mine] = 0u;   // this buffer is the next level's N
         unsigned int pending = __ballot_sync(GB_FULL_MASK, my_bits != 0u);
         while (pending != 0u) {
           const int src_lane = __ffs(pending) - 1;
@@ -195,9 +270,9 @@ bfsFusedKernel(BfsFusedArgs a) {
             }
             for (Index k = lane; k < deg; k += 32) {
               const Index nbr = __ldg(a.push_ind + beg + k);
-              if (bfsClaim(vis, nbr)) {
+              if (bfsClaim(bfsVis(a, vsel), nbr)) {
                 a.levels[nbr] = next_level;
-                atomicOr(N + (nbr >> 5), 1u << (nbr & 31));
+                atomicOr(bfsN(a, fsel) + (nbr >> 5), 1u << (nbr & 31));
                 ++found_here;
               }
             }
@@ -205,159 +280,226 @@ bfsFusedKernel(BfsFusedArgs a) {
         }
       }
       grid.sync();
-      unsigned long long nheavy = *reinterpret_cast<volatile unsigned long long*>(heavy_cell);
-      if (nheavy > GB_BFS_HEAVY_CAP) nheavy = GB_BFS_HEAVY_CAP;
-      if (nheavy > 0ull) {
-        for (unsigned long long h = 0; h < nheavy; ++h) {
+      const unsigned long long listed =
+          *reinterpret_cast<volatile unsigned long long*>(heavy_cell);
+      const int nheavy = (listed > GB_BFS_HEAVY_CAP) ? GB_BFS_HEAVY_CAP
+                                                     : static_cast<int>(listed);
+      if (nheavy > 0) {
+        for (int h = 0; h < nheavy; ++h) {
           const Index u = a.heavy[h];
           const Index beg = __ldg(a.push_ptr + u);
           const Index deg = __ldg(a.push_ptr + u + 1) - beg;
           for (Index k = gtid; k < deg; k += gthreads) {
             const Index nbr = __ldg(a.push_ind + beg + k);
-            if (bfsClaim(vis, nbr)) {
+            if (bfsClaim(bfsVis(a, vsel), nbr)) {
               a.levels[nbr] = next_level;
-              atomicOr(N + (nbr >> 5), 1u << (nbr & 31));
+              atomicOr(bfsN(a, fsel) + (nbr >> 5), 1u << (nbr & 31));
               ++found_here;
             }
           }
         }
       }
-      discovered_pushing += found_here;
-    } else {
+    } else if (PULL) {
       ++pull_levels;
       // ---------------- pull: every unvisited row looks for a visited neighbour ----
-      const Index ngroups = (nwords + 3) >> 2;
-      for (Index g = gwarp; g < ngroups; g += gwarps) {
-        unsigned int mword[4];
-        Index f[4];
-        unsigned int pword[4];
+      unsigned long long* const walk_cell = a.counters + 35 + (level % 3);
+      unsigned long long* const list_cell = a.counters + 38 + (level % 3);
+      // scan: a lane per bitmap word of the chunk, chunks dealt round-robin (the
+      // grid has ~4 chunks per warp at RMAT-24 and they cost about the same); the
+      // next chunk's words are requested before this one is worked on
+      Index c = gwarp;
+      unsigned int next_vis = (c < nchunks && c*32 + lane < nwords)
+                              ? bfsVis(a, vsel)[c*32 + lane] : 0xffffffffu;
+      while (c < nchunks) {
+        const Index word = c*32 + lane;
+        const unsigned int my_vis = next_vis;
+        const Index c_next = c + gwarps;
+        next_vis = (c_next < nchunks && c_next*32 + lane < nwords)
+                   ? bfsVis(a, vsel)[c_next*32 + lane] : 0xffffffffu;
+        Index* const walk = a.walk + c*GB_BFS_CHUNK;
+        int nwalk = 0;                        // rows of this chunk left to walk
+        unsigned int my_out = 0u;             // discoveries in this lane's word
+        unsigned int open = __ballot_sync(GB_FULL_MASK, my_vis != 0xffffffffu);
+        while (open != 0u) {
+          // up to GB_BFS_BATCH open words: all first-neighbour loads, then all
+          // probes, then the decisions
+          const unsigned int batch = open;
+          Index f[GB_BFS_BATCH];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const Index word = g*4 + j;
-          mword[j] = (word < nwords) ? vis[word] : 0xffffffffu;
-        }
-        if ((mword[0] & mword[1] & mword[2] & mword[3]) == 0xffffffffu) {
-          // nothing left to discover in these 128 rows (the common case after the
-          // first pull level): only the bitmaps move on
-          if (lane < 4 && g*4 + lane < nwords) {
-            N[g*4 + lane] = 0u;
-            vis_other[g*4 + lane] = 0xffffffffu;
-            F[g*4 + lane] = 0u;
+          for (int j = 0; j < GB_BFS_BATCH; ++j) {
+            const int wl = __ffs(open) - 1;   // -1 when none is left
+            open &= open - 1u;
+            f[j] = static_cast<Index>(-1);
+            if (wl >= 0) {
+              const unsigned int m = __shfl_sync(GB_FULL_MASK, my_vis, wl);
+              const Index row = c*GB_BFS_CHUNK + wl*32 + lane;
+              if (row < n && !((m >> lane) & 1u)) f[j] = __ldg(a.pull_first + row);
+            }
           }
-          continue;
-        }
+          unsigned int pword[GB_BFS_BATCH];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const Index row = (g*4 + j)*32 + lane;
-          const bool open = (row < n) && !((mword[j] >> lane) & 1u);
-          f[j] = open ? __ldg(a.pull_first + row) : static_cast<Index>(-1);
-          if (open) ++inspected;
-        }
+          for (int j = 0; j < GB_BFS_BATCH; ++j)
+            pword[j] = (f[j] != static_cast<Index>(-1))
+                       ? bfsVis(a, vsel)[(f[j] & 0x7fffffff) >> 5] : 0u;
+          unsigned int hit = 0u, more = 0u;   // bit j: row of batch word j
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          pword[j] = 0u;
-          if (f[j] != static_cast<Index>(-1)) pword[j] = vis[(f[j] & 0x7fffffff) >> 5];
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const Index word = g*4 + j;
-          const Index row = word*32 + lane;
-          bool found = (pword[j] >> (f[j] & 31)) & 1u;
-          // more entries and the first one not visited: the row has to be walked.
-          // Few lanes of a warp are in that position and a walk is a chain of
-          // dependent loads, so the rows are parked in a CTA-wide list and walked by
-          // all threads after the scan (inline only when the list is full).
-          bool walk = (f[j] >= 0 && !found);
-          const unsigned int walkers = __ballot_sync(GB_FULL_MASK, walk);
-          if (walkers != 0u) {
-            int base = 0;
-            if (lane == 0) base = atomicAdd(&s_parked, __popc(walkers));
-            base = __shfl_sync(GB_FULL_MASK, base, 0);
-            const int slot = base + __popc(walkers & ((1u << lane) - 1u));
-            if (walk && slot < GB_BFS_PARK) { s_park[slot] = row; walk = false; }
+          for (int j = 0; j < GB_BFS_BATCH; ++j) {
+            const bool found = (pword[j] >> (f[j] & 31)) & 1u;
+            // the first entry is looked at (-1: not open, or a row without entries)
+            inspected += (f[j] != static_cast<Index>(-1)) ? 1 : 0;
+            hit |= static_cast<unsigned int>(found) << j;
+            // more entries and the first one not visited: the row is walked after
+            // the scan, by whichever warp claims this chunk's slice of the list
+            more |= static_cast<unsigned int>(f[j] >= 0 && !found) << j;
           }
-          if (walk) {
-            Index k = __ldg(a.pull_ptr + row) + 1;
-            const Index end = __ldg(a.pull_ptr + row + 1);
-            for (; k < end; ++k) {
-              const Index col = __ldg(a.pull_ind + k);
+          unsigned int rest = batch;
+#pragma unroll
+          for (int j = 0; j < GB_BFS_BATCH && rest != 0u; ++j) {
+            const int wl = __ffs(rest) - 1;
+            rest &= rest - 1u;
+            const Index row = c*GB_BFS_CHUNK + wl*32 + lane;
+            const bool found = (hit >> j) & 1u, walk_row = (more >> j) & 1u;
+            const unsigned int walkers = __ballot_sync(GB_FULL_MASK, walk_row);
+            if (walk_row) walk[nwalk + __popc(walkers & ((1u << lane) - 1u))] = row;
+            nwalk += __popc(walkers);
+            const unsigned int out = __ballot_sync(GB_FULL_MASK, found);
+            if (found) { a.levels[row] = next_level; ++found_here; }
+            if (lane == wl) my_out = out;
+          }
+        }
+        if (word < nwords) {
+          bfsN(a, fsel)[word] = my_out;
+          bfsVisOther(a, vsel)[word] = my_vis | my_out;
+          bfsF(a, fsel)[word] = 0u;
+        }
+        if (lane == 0 && nwalk > 0) {
+          a.walk_count[c] = nwalk;
+          a.walk_chunks[atomicAdd(list_cell, 1ull)] = c;
+          if (a.trace && level < 16)
+            atomicAdd(a.counters + 60 + level, static_cast<unsigned long long>(nwalk));
+        }
+        c = c_next;
+      }
+      grid.sync();
+      if (gtid == 0 && level < 16) a.counters[44 + level] = bfsClockNs();
+      // walk: the chunks with rows to walk, claimed from a counter, a lane per row;
+      // a list with more than GB_BFS_WALK_WARP entries left after the lane has
+      // looked at GB_BFS_WALK_STEP of them is walked by the whole warp
+      const Index nlisted = static_cast<Index>(
+          *reinterpret_cast<volatile unsigned long long*>(list_cell));
+      for (Index i = gwarp; i < nlisted; ) {
+        const Index i_next = gwarps + bfsClaimChunk(walk_cell, lane);
+        const Index c = a.walk_chunks[i];
+        const int nwalk = a.walk_count[c];
+        for (int i0 = 0; i0 < nwalk; i0 += 32) {
+          Index row = 0, k = 0, end = 0;
+          if (i0 + lane < nwalk) {
+            row = a.walk[c*GB_BFS_CHUNK + i0 + lane];
+            k = __ldg(a.pull_ptr + row) + 1;
+            end = __ldg(a.pull_ptr + row + 1);
+          }
+          // most walks end after a few entries: every lane starts on its own list
+          const Index stop = (end - k > GB_BFS_WALK_WARP + GB_BFS_WALK_STEP)
+                             ? k + GB_BFS_WALK_STEP : end;
+          bool found = false;
+          // GB_BFS_WALK_STEP entries per step: their bitmap words are fetched
+          // together, then examined in list order (the count stops at the first
+          // visited one)
+          while (k < stop && !found) {
+            Index col[GB_BFS_WALK_STEP];
+            unsigned int wv[GB_BFS_WALK_STEP];
+#pragma unroll
+            for (int u = 0; u < GB_BFS_WALK_STEP; ++u)
+              col[u] = (k + u < stop) ? __ldg(a.pull_ind + k + u) : static_cast<Index>(-1);
+#pragma unroll
+            for (int u = 0; u < GB_BFS_WALK_STEP; ++u)
+              wv[u] = (col[u] >= 0) ? bfsVis(a, vsel)[col[u] >> 5] : 0u;
+#pragma unroll
+            for (int u = 0; u < GB_BFS_WALK_STEP; ++u) {
+              if (found || col[u] < 0) continue;
               ++inspected;
-              if ((vis[col >> 5] >> (col & 31)) & 1u) { found = true; break; }
+              found = (wv[u] >> (col[u] & 31)) & 1u;
             }
+            k += GB_BFS_WALK_STEP;
           }
-          const unsigned int out = __ballot_sync(GB_FULL_MASK, found);
-          if (word < nwords) {
-            if (found) a.levels[row] = next_level;
-            if (lane == 0) {
-              N[word] = out;
-              vis_other[word] = mword[j] | out;
-              F[word] = 0u;
+          unsigned int longs = __ballot_sync(GB_FULL_MASK, !found && k < end);
+          while (longs != 0u) {
+            const int src = __ffs(longs) - 1;
+            longs &= longs - 1u;
+            const Index lend = __shfl_sync(GB_FULL_MASK, end, src);
+            bool hit = false;
+            for (Index lk = __shfl_sync(GB_FULL_MASK, k, src); lk < lend && !hit; lk += 32) {
+              bool v = false;
+              if (lk + lane < lend) {
+                const Index col = __ldg(a.pull_ind + lk + lane);
+                v = (bfsVis(a, vsel)[col >> 5] >> (col & 31)) & 1u;
+              }
+              const unsigned int b = __ballot_sync(GB_FULL_MASK, v);
+              hit = (b != 0u);
+              if (lane == 0)
+                inspected += hit ? __ffs(b) : (lend - lk < 32 ? lend - lk : 32);
             }
+            if (lane == src) found = hit;
           }
-          found_here += found ? 1 : 0;
-        }
-      }
-      // the parked rows, one per thread at a time
-      __syncthreads();
-      if (gtid == 0 && level == 2) { a.counters[29] = bfsClockNs(); a.counters[31] = s_parked; }
-      const int parked = (s_parked < GB_BFS_PARK) ? s_parked : GB_BFS_PARK;
-      for (int i = threadIdx.x; i < parked; i += GB_BFS_NT) {
-        const Index row = s_park[i];
-        Index k = __ldg(a.pull_ptr + row) + 1;
-        const Index end = __ldg(a.pull_ptr + row + 1);
-        bool found = false;
-        // four entries per step: their bitmap words are fetched together, then
-        // examined in list order (the count stops at the first visited one)
-        while (k < end && !found) {
-          Index col[4];
-          unsigned int word[4];
-#pragma unroll
-          for (int u = 0; u < 4; ++u)
-            col[u] = (k + u < end) ? __ldg(a.pull_ind + k + u) : static_cast<Index>(-1);
-#pragma unroll
-          for (int u = 0; u < 4; ++u)
-            word[u] = (col[u] >= 0) ? vis[col[u] >> 5] : 0u;
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            if (found || col[u] < 0) continue;
-            ++inspected;
-            found = (word[u] >> (col[u] & 31)) & 1u;
+          if (found) {
+            const unsigned int bit = 1u << (row & 31);
+            atomicOr(bfsN(a, fsel) + (row >> 5), bit);
+            atomicOr(bfsVisOther(a, vsel) + (row >> 5), bit);
+            a.levels[row] = next_level;
+            ++found_here;
           }
-          k += 4;
         }
-        if (found) {
-          const unsigned int bit = 1u << (row & 31);
-          atomicOr(N + (row >> 5), bit);
-          atomicOr(vis_other + (row >> 5), bit);
-          a.levels[row] = next_level;
-          ++found_here;
-        }
+        i = i_next;
       }
-      __syncthreads();
-      if (gtid == 0 && level == 2) a.counters[30] = bfsClockNs();
-      if (threadIdx.x == 0) s_parked = 0;
     }
     // ---- frontier size of the next level ------------------------------------------
-    const int block_found = blockSum<GB_BFS_NT>(found_here, s_red);
-    if (threadIdx.x == 0 && block_found)
+    const int block_found = blockSum<NT>(found_here, s_red);
+    if (threadIdx.x == 0 && block_found) {
       atomicAdd(count_cell, static_cast<unsigned long long>(block_found));
+      if (!dense)                           // [11] vertices discovered pushing
+        atomicAdd(a.counters + 11, static_cast<unsigned long long>(block_found));
+    }
     grid.sync();
     if (gtid == 0 && level < 16)
       a.counters[12 + level] = (bfsClockNs() << 1) | (dense ? 1ull : 0ull);
-    fcount = *reinterpret_cast<volatile unsigned long long*>(count_cell);
-    if (dense) { unsigned int* t = vis; vis = vis_other; vis_other = t; }
-    { unsigned int* t = F; F = N; N = t; }
+    fcount = static_cast<unsigned int>(
+        *reinterpret_cast<volatile unsigned long long*>(count_cell));
+    if (dense) vsel ^= 1;
+    fsel ^= 1;
+  }
+  // ---- v of the rows never reached: visited now only because nothing points at
+  // them (the source aside) or not visited at all -------------------------------------
+  // A traversal cut off after max_levels (the frontier is not empty): the rows found
+  // at the last level, now the frontier, get no level either, as in the
+  // operation-by-operation loop, which assigns levels 1..max_niter.
+  const unsigned int* const cut_rows = (fcount > 0u) ? bfsF(a, fsel) : NULL;
+  // A warp takes 32 words, one per lane, then writes the rows of each word that
+  // has any, a lane per row.
+  for (Index w0 = gwarp*32; w0 < nwords; w0 += gwarps*32) {
+    const Index w = w0 + lane;
+    unsigned int unreached = 0u;
+    if (w < nwords) {
+      unreached = ~(bfsVis(a, vsel)[w] & ~bfsIsolated(a, w)) |
+                  (cut_rows != NULL ? cut_rows[w] : 0u);
+      if (w == (a.source >> 5)) unreached &= ~(1u << (a.source & 31));
+      if (w == nwords - 1 && (n & 31)) unreached &= (1u << (n & 31)) - 1u;
+    }
+    unsigned int pending = __ballot_sync(GB_FULL_MASK, unreached != 0u);
+    while (pending != 0u) {
+      const int src = __ffs(pending) - 1;
+      pending &= pending - 1u;
+      const unsigned int bits = __shfl_sync(GB_FULL_MASK, unreached, src);
+      if ((bits >> lane) & 1u) a.levels[(w0 + src)*32 + lane] = 0.f;
+    }
   }
   // ---- results -----------------------------------------------------------------
   // [7] entries inspected pulling, [8] pull levels, [9] vertices pushed, [10] edges
   // pushed, [11] vertices discovered pushing — the algorithmic bytes of SURVEY.md §8d
-  const int block_insp = blockSum<GB_BFS_NT>(inspected, s_red);
-  const int block_pv = blockSum<GB_BFS_NT>(pushed_vertices, s_red);
-  const int block_dp = blockSum<GB_BFS_NT>(discovered_pushing, s_red);
+  const int block_insp = blockSum<NT>(inspected, s_red);
+  const int block_pv = blockSum<NT>(pushed_vertices, s_red);
   if (threadIdx.x == 0) {
     if (block_insp) atomicAdd(a.counters + 7, static_cast<unsigned long long>(block_insp));
     if (block_pv)   atomicAdd(a.counters + 9, static_cast<unsigned long long>(block_pv));
-    if (block_dp)   atomicAdd(a.counters + 11, static_cast<unsigned long long>(block_dp));
   }
   if (pushed_edges) atomicAdd(a.counters + 10, static_cast<unsigned long long>(pushed_edges));
   if (gtid == 0) {
