@@ -66,9 +66,11 @@ Info bfsFused(Vector<float>* v, const Matrix<a>* A, Index s, Descriptor* desc, i
   const size_t counters_bytes = GB_BFS_NCOUNTERS*sizeof(unsigned long long);
   const size_t heavy_bytes = GB_BFS_HEAVY_CAP*sizeof(Index);
   const size_t walk_bytes = nchunks*GB_BFS_CHUNK*sizeof(Index);
+  const size_t lists_bytes = ((nchunks*(sizeof(int) + sizeof(Index)) + 255)/256)*256;
+  const size_t level8_bytes = ((static_cast<size_t>(n) + 255)/256)*256;
   unsigned char* base = reinterpret_cast<unsigned char*>(desc->scratch(GB_SCRATCH_BFS,
-      4*words_bytes + counters_bytes + heavy_bytes + walk_bytes +
-      nchunks*(sizeof(int) + sizeof(Index))));
+      4*words_bytes + counters_bytes + heavy_bytes + walk_bytes + lists_bytes +
+      level8_bytes));
   BfsFusedArgs args;
   args.push_ptr = S->d_csrRowPtr_;  args.push_ind = S->d_csrColInd_;
   args.pull_ptr = S->d_cscColPtr_;  args.pull_ind = S->d_cscRowInd_;
@@ -101,6 +103,9 @@ Info bfsFused(Vector<float>* v, const Matrix<a>* A, Index s, Descriptor* desc, i
   args.walk_count = reinterpret_cast<int*>(base + 4*words_bytes + counters_bytes +
                                            heavy_bytes + walk_bytes);
   args.walk_chunks = reinterpret_cast<Index*>(args.walk_count + nchunks);
+  // no fill: the kernel reads the byte of a row only when it wrote it in this traversal
+  args.level8     = base + 4*words_bytes + counters_bytes + heavy_bytes + walk_bytes +
+                    lists_bytes;
 
   static const int trace = getEnv("GB200_BFS_TRACE", 0);
   args.trace = trace;
@@ -154,7 +159,7 @@ Info bfsFused(Vector<float>* v, const Matrix<a>* A, Index s, Descriptor* desc, i
       else
         fprintf(stderr, " L%d push %.1fus", l, 1e-3*static_cast<double>(end - start));
     }
-    fprintf(stderr, "\n");
+    fprintf(stderr, " end-pass %.1fus\n", 1e-3*static_cast<double>(cells[29] - cells[30]));
   }
   if (depth != NULL) {
     const unsigned long long levels = runtime().fetch(args.counters + 6);

@@ -12,7 +12,8 @@
 // the whole traversal).
 //
 // State: visited bitmap (two copies, ping-pong on pull levels), frontier bitmap F,
-// next-frontier bitmap N, float levels v (the result, 1-based, 0 = unreached).
+// next-frontier bitmap N, a byte per row holding its level while the traversal runs,
+// float levels v (the result, 1-based, 0 = unreached).
 //   push level (frontier small): warps scan F; a vertex of moderate degree is
 //     expanded by its warp, lanes striding the adjacency; vertices with more than
 //     GB_BFS_HEAVY neighbours go to a list that the WHOLE grid expands after a
@@ -30,16 +31,17 @@
 //             that have more are written to the chunk's slice of the walk list,
 //             and a chunk with any to a list of such chunks.
 //             The owner of a word writes N, the merged visited word of the other
-//             copy, v for the discovered rows and clears F.
+//             copy, the level bytes of the discovered rows and clears F.
 //     walk  — warps claim listed chunks from a counter; a lane walks its row's
 //             list GB_BFS_WALK_STEP entries per step, a list still longer than
 //             GB_BFS_WALK_WARP after the first step is walked by the whole warp,
 //             32 entries and one ballot per step.  Discoveries are ORed into N and
 //             the other visited copy.
-//   v is written once per row: the source at set-up, a discovered row when it is
-//   discovered, and after the last level 0 for every row never reached (and, when
+//   v is written once per row, after the last level, in one pass of full-line
+//   stores: the level byte of every reached row, 0 for the others (and, when
 //   max_levels cuts the traversal off, for the rows found at the last level: only
-//   levels 1..max_levels are assigned, as in the operation-by-operation loop).
+//   levels 1..max_levels are assigned, as in the operation-by-operation loop).  A
+//   row reached at level 255 or deeper keeps byte 255 and gets v when discovered.
 // Direction: the reference's ratio rule with hysteresis (vector.hpp:318-342):
 // sparse -> dense when |f|/n > switchpoint and growing, dense -> sparse when
 // <= switchpoint and shrinking; results do not depend on it.
@@ -98,6 +100,7 @@ struct BfsFusedArgs {
   int   mode;                // 0 push-pull, 1 push only, 2 pull only (reference --mxvmode)
   // state (device memory, sized for n)
   float*        levels;      // result
+  unsigned char* level8;     // [n] level of each row reached so far, 255: level >= 255
   unsigned int* visited[2];
   unsigned int* frontier;    // F
   unsigned int* next;        // N
@@ -110,6 +113,8 @@ struct BfsFusedArgs {
                                   // [6] levels executed, [7..11] work counters (out),
                                   // [12..27] time at the end of the set-up and of every
                                   // level (ns << 1 | pulled), [28] time at the start,
+                                  // [29] at the end of the pass that writes v, [30]
+                                  // at the end of the last level,
                                   // [35..37] walk-chunk claim counters of the pull
                                   // levels, [38..40] chunks listed in walk_chunks
                                   // (both rotating like [0..2]),
@@ -134,6 +139,19 @@ __device__ __forceinline__ bool bfsClaim(unsigned int* visited, Index vtx) {
   unsigned int* word = visited + (vtx >> 5);
   if (*reinterpret_cast<volatile unsigned int*>(word) & bit) return false;
   return (atomicOr(word, bit) & bit) == 0;
+}
+
+// Row `row` is reached at level lv.  Levels are kept as one byte per row during the
+// traversal (16.8 MB at RMAT-24: it stays in L2 beside the bitmaps) and v is written
+// after the last level, in full lines.  From level 255 on the byte is 255 and v is
+// written here; the pass at the end leaves those rows alone.
+__device__ __forceinline__ void bfsSetLevel(const BfsFusedArgs& a, Index row, int lv) {
+  if (lv < 255) {
+    a.level8[row] = static_cast<unsigned char>(lv);
+  } else {
+    a.level8[row] = 255;
+    a.levels[row] = static_cast<float>(lv);
+  }
 }
 
 // The next chunk for this warp from a claim counter (warp-uniform result).
@@ -179,16 +197,20 @@ bfsFusedKernel(BfsFusedArgs a) {
   const Index n = a.n;
   const Index nwords = (n + 31) >> 5;
   const int lane = threadIdx.x & 31;
-  const Index gtid = blockIdx.x*blockDim.x + threadIdx.x;        // grid << 2^31 threads
-  const Index gthreads = gridDim.x*blockDim.x;
+  // The kernel is launched with NT threads per CTA.  The constant instead of
+  // blockDim.x lets the compiler rebuild gthreads from gridDim.x where it needs it
+  // instead of keeping it in a register: at 768 x 2 (40 registers) that is what keeps
+  // spill reloads out of the push expansion loops.
+  const Index gtid = blockIdx.x*NT + threadIdx.x;                 // grid << 2^31 threads
+  const Index gthreads = gridDim.x*NT;
   const Index gwarp = gtid >> 5;
   const Index gwarps = gthreads >> 5;
   const Index nchunks = (nwords + 31) >> 5;               // pull chunks of 32 words
 
   if (gtid == 0) a.counters[28] = bfsClockNs();
-  // ---- level 0: clear the bitmaps, seed the source (v is written once per row: the
-  // rows never reached get their 0 after the last level) ----------------------------
-  if (gtid == 0) a.levels[a.source] = 1.f;
+  // ---- level 0: clear the bitmaps, seed the source (v is written once per row, after
+  // the last level) ---------------------------------------------------------------------
+  if (gtid == 0) a.level8[a.source] = 1;
   for (Index w = gtid; w < nwords; w += gthreads) {
     const unsigned int seed = (w == (a.source >> 5)) ? (1u << (a.source & 31)) : 0u;
     // rows nothing points at count as visited from the start: no level can discover
@@ -232,7 +254,6 @@ bfsFusedKernel(BfsFusedArgs a) {
       a.counters[35 + (level + 1) % 3] = 0ull;
       a.counters[38 + (level + 1) % 3] = 0ull;
     }
-    const float next_level = static_cast<float>(level + 1);
     int found_here = 0;
 
     if (!dense) {
@@ -271,7 +292,7 @@ bfsFusedKernel(BfsFusedArgs a) {
             for (Index k = lane; k < deg; k += 32) {
               const Index nbr = __ldg(a.push_ind + beg + k);
               if (bfsClaim(bfsVis(a, vsel), nbr)) {
-                a.levels[nbr] = next_level;
+                bfsSetLevel(a, nbr, level + 1);
                 atomicOr(bfsN(a, fsel) + (nbr >> 5), 1u << (nbr & 31));
                 ++found_here;
               }
@@ -292,7 +313,7 @@ bfsFusedKernel(BfsFusedArgs a) {
           for (Index k = gtid; k < deg; k += gthreads) {
             const Index nbr = __ldg(a.push_ind + beg + k);
             if (bfsClaim(bfsVis(a, vsel), nbr)) {
-              a.levels[nbr] = next_level;
+              bfsSetLevel(a, nbr, level + 1);
               atomicOr(bfsN(a, fsel) + (nbr >> 5), 1u << (nbr & 31));
               ++found_here;
             }
@@ -363,7 +384,7 @@ bfsFusedKernel(BfsFusedArgs a) {
             if (walk_row) walk[nwalk + __popc(walkers & ((1u << lane) - 1u))] = row;
             nwalk += __popc(walkers);
             const unsigned int out = __ballot_sync(GB_FULL_MASK, found);
-            if (found) { a.levels[row] = next_level; ++found_here; }
+            if (found) { bfsSetLevel(a, row, level + 1); ++found_here; }
             if (lane == wl) my_out = out;
           }
         }
@@ -445,7 +466,7 @@ bfsFusedKernel(BfsFusedArgs a) {
             const unsigned int bit = 1u << (row & 31);
             atomicOr(bfsN(a, fsel) + (row >> 5), bit);
             atomicOr(bfsVisOther(a, vsel) + (row >> 5), bit);
-            a.levels[row] = next_level;
+            bfsSetLevel(a, row, level + 1);
             ++found_here;
           }
         }
@@ -467,30 +488,69 @@ bfsFusedKernel(BfsFusedArgs a) {
     if (dense) vsel ^= 1;
     fsel ^= 1;
   }
-  // ---- v of the rows never reached: visited now only because nothing points at
-  // them (the source aside) or not visited at all -------------------------------------
-  // A traversal cut off after max_levels (the frontier is not empty): the rows found
-  // at the last level, now the frontier, get no level either, as in the
-  // operation-by-operation loop, which assigns levels 1..max_niter.
+  if (gtid == 0) a.counters[30] = bfsClockNs();   // [30]: the end of the last level
+  // ---- v, every row once, in full lines ----------------------------------------
+  // A row is reached when it is visited now and not only because nothing points at
+  // it (the source is reached).  A traversal cut off after max_levels (the frontier
+  // is not empty): the rows found at the last level, now the frontier, get no level
+  // either, as in the operation-by-operation loop, which assigns levels 1..max_niter.
+  // Reached rows get their byte, the others 0; a byte is only read for a row reached
+  // in this traversal, which wrote it.
   const unsigned int* const cut_rows = (fcount > 0u) ? bfsF(a, fsel) : NULL;
-  // A warp takes 32 words, one per lane, then writes the rows of each word that
-  // has any, a lane per row.
-  for (Index w0 = gwarp*32; w0 < nwords; w0 += gwarps*32) {
-    const Index w = w0 + lane;
-    unsigned int unreached = 0u;
-    if (w < nwords) {
-      unreached = ~(bfsVis(a, vsel)[w] & ~bfsIsolated(a, w)) |
-                  (cut_rows != NULL ? cut_rows[w] : 0u);
-      if (w == (a.source >> 5)) unreached &= ~(1u << (a.source & 31));
-      if (w == nwords - 1 && (n & 31)) unreached &= (1u << (n & 31)) - 1u;
+  // An adopted array need not be 16-byte aligned: then every row is stored alone.
+  const bool lines = (reinterpret_cast<uintptr_t>(a.levels) & 15u) == 0u;
+  // A warp takes 512 rows (16 bitmap words, 512 bytes): lanes 0..15 build the reach
+  // masks, then each lane writes 4 rows per step, a warp 512 contiguous bytes per
+  // 16-byte store.  4 rows holding a level of 255 or more, or past n, or not aligned,
+  // are written row by row.  The loop counts blocks of 16 words, not rows, so that
+  // stepping past the last block cannot overflow (rows stay below n + 512, as the
+  // pull scan's stay below n + 1024).  The 4-byte load also takes the bytes of rows
+  // not reached, which this traversal never wrote; their values are not used.
+  const Index nblocks = (nwords + 15) >> 4;
+  for (Index blk = gwarp; blk < nblocks; blk += gwarps) {
+    const Index r0 = blk*512;
+    const Index w = blk*16 + (lane & 15);
+    unsigned int reached = 0u;
+    if (lane < 16 && w < nwords) {
+      reached = bfsVis(a, vsel)[w] & ~bfsIsolated(a, w);
+      if (cut_rows != NULL) reached &= ~cut_rows[w];
+      if (w == (a.source >> 5)) reached |= 1u << (a.source & 31);
     }
-    unsigned int pending = __ballot_sync(GB_FULL_MASK, unreached != 0u);
-    while (pending != 0u) {
-      const int src = __ffs(pending) - 1;
-      pending &= pending - 1u;
-      const unsigned int bits = __shfl_sync(GB_FULL_MASK, unreached, src);
-      if ((bits >> lane) & 1u) a.levels[(w0 + src)*32 + lane] = 0.f;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const unsigned int bits =
+          (__shfl_sync(GB_FULL_MASK, reached, 4*j + (lane >> 3)) >> (4*(lane & 7))) & 0xfu;
+      const Index row = r0 + 128*j + 4*lane;
+      if (row >= n) continue;
+      if (lines && row + 4 <= n) {
+        const unsigned int b = *reinterpret_cast<const unsigned int*>(a.level8 + row);
+        float f[4];
+        bool escape = false;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const unsigned int byte = (b >> (8*k)) & 0xffu;
+          const bool r = (bits >> k) & 1u;
+          escape |= r && byte == 255u;
+          f[k] = r ? static_cast<float>(byte) : 0.f;
+        }
+        if (!escape) {
+          *reinterpret_cast<float4*>(a.levels + row) = make_float4(f[0], f[1], f[2], f[3]);
+          continue;
+        }
+      }
+      for (int k = 0; k < 4 && row + k < n; ++k) {
+        if (!((bits >> k) & 1u)) {
+          a.levels[row + k] = 0.f;
+        } else {
+          const unsigned int byte = a.level8[row + k];
+          if (byte != 255u) a.levels[row + k] = static_cast<float>(byte);
+        }
+      }
     }
+  }
+  if (a.trace) {                          // [29]: the end of the pass above
+    grid.sync();
+    if (gtid == 0) a.counters[29] = bfsClockNs();
   }
   // ---- results -----------------------------------------------------------------
   // [7] entries inspected pulling, [8] pull levels, [9] vertices pushed, [10] edges
