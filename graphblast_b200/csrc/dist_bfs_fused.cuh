@@ -85,8 +85,7 @@ __device__ __forceinline__ unsigned long long distNow() {
   if (gtid == 0 && level < 12) a.cells[16 + 8*level + (slot)] = distNow();    \
 } while (0)
 
-template <int MINB>
-__global__ void __launch_bounds__(GBX_BFS_NT, MINB)
+__global__ void __launch_bounds__(GBX_BFS_NT, 2)
 bfsFusedDistKernel(BfsDistArgs a) {
   namespace cg = cooperative_groups;
   cg::grid_group grid = cg::this_grid();
@@ -404,9 +403,7 @@ int gb200_dist_bfs_fused(gb200_xchg_t x, gb200_vector_t v, gb200_matrix_t M,
   a.epoch0 = x->epoch;
   a.timeout_cycles = 20000000000ll;
 
-  static const int minb = getEnv("GB200_BFS_MINB", 2);
-  void (*kernel)(gbx::BfsDistArgs) = (minb >= 2) ? gbx::bfsFusedDistKernel<2>
-                                                 : gbx::bfsFusedDistKernel<1>;
+  void (*kernel)(gbx::BfsDistArgs) = gbx::bfsFusedDistKernel;
   static int resident = 0;
   if (resident == 0) {
     int per_sm = 0;

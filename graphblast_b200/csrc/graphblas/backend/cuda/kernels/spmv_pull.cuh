@@ -2,7 +2,7 @@
 //
 //  * spmvMergeKernel      : generic-semiring CSR SpMV, merge-path load balanced
 //                           (rows + nonzeros split evenly across CTAs and threads),
-//                           256-bit streaming loads of colind/val, gathers of the
+//                           streaming loads of colind/val, gathers of the
 //                           dense vector served from L2 (evict-last), shuffle-based
 //                           segmented scan for rows that straddle threads, per-CTA
 //                           carry-out fixed up by spmvCarryFixupKernel.
@@ -82,8 +82,10 @@ __global__ void spmvMergePartitionKernel(Index* __restrict__ tile_rows,
 // free, and the sequential readers pay one XOR.
 __device__ __forceinline__ int prodSlot(int p) { return p ^ ((p >> 3) & 4); }
 
-// Gather: 0 = no gather (lab only), 1 = gather u[col].
-template <int NT, int IPT, bool Vec256, int Gather, bool LaneMajor,
+// LaneMajor: lanes of a warp take consecutive nonzeros with 32-bit loads (any
+// alignment).  Otherwise every thread takes 8 consecutive nonzeros, read as two
+// 128-bit loads per array (colind and val must be 32-byte aligned).
+template <int NT, int IPT, bool LaneMajor,
           typename W, typename a, typename U,
           typename MulOp, typename AddOp>
 __global__ void __launch_bounds__(NT, GB_SPMV_MINB(NT))
@@ -171,14 +173,12 @@ spmvMergeKernelT(W* __restrict__           w,
   for (int c = t; c < nchunks; c += NT) {
     const Index kb = k0a + (c << 3);
     W prods[8];
-    if (Vec256 && kb + 8 <= nnz) {
+    if (kb + 8 <= nnz) {
       const Word8 cw = ldStream256(colind + kb);
       const Word8 vw = ldStream256(val + kb);
       U uv[8];
 #pragma unroll
-      for (int j = 0; j < 8; ++j)
-        uv[j] = Gather ? ldGather(u + cw.w[j], pol)
-                       : static_cast<U>(cw.w[j] & 1);
+      for (int j = 0; j < 8; ++j) uv[j] = ldGather(u + cw.w[j], pol);
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         a av;
@@ -198,17 +198,12 @@ spmvMergeKernelT(W* __restrict__           w,
         }
       }
     }
-    if (sizeof(W) == 4) {
-      float4 lo4, hi4;
-      memcpy(&lo4, &prods[0], 16);
-      memcpy(&hi4, &prods[4], 16);
-      const int swap = c & 4;          // == prodSlot(8c) - 8c
-      *reinterpret_cast<float4*>(&s_prod[(c << 3) + swap])       = lo4;
-      *reinterpret_cast<float4*>(&s_prod[(c << 3) + (4 - swap)]) = hi4;
-    } else {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) s_prod[prodSlot((c << 3) + j)] = prods[j];
-    }
+    float4 lo4, hi4;
+    memcpy(&lo4, &prods[0], 16);
+    memcpy(&hi4, &prods[4], 16);
+    const int swap = c & 4;            // == prodSlot(8c) - 8c
+    *reinterpret_cast<float4*>(&s_prod[(c << 3) + swap])       = lo4;
+    *reinterpret_cast<float4*>(&s_prod[(c << 3) + (4 - swap)]) = hi4;
   }
 
   // ---- phase 1b: row-end offsets for rows r0 .. r1 (last = still-open row) ----
@@ -390,8 +385,8 @@ spmvMaskedOrPullKernel(W* __restrict__           w,
 // test of a row is a broadcast word load and the neighbour test is a gather into
 // an n/8-byte array (2 MB at RMAT-24) that lives in L1/L2 instead of a 4n-byte
 // float array.  A warp owns 32 consecutive rows = one output word: the new
-// frontier is written both as 0/1 floats (the vector's storage) and, through one
-// ballot, as its bitmap shadow.
+// frontier is written, through one ballot, as the bitmap shadow only; the caller
+// holds the 0/1 values lazily (DenseVector::materialize).
 // ---------------------------------------------------------------------------
 // first[i] = -1 (empty row) | colind[rowptr[i]] | that value with bit 31 set when
 // it is the row's only entry.  Computed once per matrix structure.
@@ -429,10 +424,9 @@ __global__ void pullEmptyRowBitsKernel(unsigned int* __restrict__ bits,
   }
 }
 
-template <bool UseScmp, bool UseEarlyExit, bool UseOpReuse, typename W>
+template <bool UseScmp, bool UseEarlyExit, bool UseOpReuse>
 __global__ void __launch_bounds__(GB_PULL_NT)
-spmvMaskedOrPullBitsKernel(W* __restrict__                  w,
-                           unsigned int* __restrict__       w_bits,
+spmvMaskedOrPullBitsKernel(unsigned int* __restrict__       w_bits,
                            const unsigned int* __restrict__ mask_bits,
                            const unsigned int* __restrict__ u_bits,
                            Index                            nrows,
@@ -508,12 +502,7 @@ spmvMaskedOrPullBitsKernel(W* __restrict__                  w,
         }
       }
       const unsigned int out = __ballot_sync(GB_FULL_MASK, found);
-      if (word < nwords) {
-        if (lane == 0) w_bits[word] = out;
-        // w == NULL: the caller holds the values lazily (bitmap only)
-        if (w != NULL && row < nrows)
-          w[row] = found ? static_cast<W>(1) : static_cast<W>(0);
-      }
+      if (lane == 0 && word < nwords) w_bits[word] = out;
       found_total += found ? 1 : 0;
     }
   }
@@ -525,7 +514,7 @@ spmvMaskedOrPullBitsKernel(W* __restrict__                  w,
     atomicAdd(inspected_bytes, 4ull*static_cast<unsigned long long>(insp));
   // The CTA that finishes last posts the discovered count to the host mailbox
   // (util.hpp): the level loop reads it without a stream synchronisation.
-  if (threadIdx.x == 0 && mail != NULL) {
+  if (threadIdx.x == 0) {
     __threadfence();
     if (atomicAdd(done, 1ull) == gridDim.x - 1) {
       const unsigned long long count =

@@ -5,15 +5,11 @@ Operand values are small nonzero integers (-3..7), so a value read from the
 wrong array or the wrong position changes the result; C is compared in full:
 its pattern must be the mask's and every value must be bit-exact.
 
-Routes of backend/cuda/spgemm.hpp (spgemmMasked):
-  * hash kernels (kernels/spgemm_hash.cuh): the default when the mask has a CSC
-    side ("hash" cases below);
+Routes of backend/cuda/spgemm.hpp (spgemmMasked), both run by every GPU test:
+  * hash kernels (kernels/spgemm_hash.cuh): a mask with a CSC side ("hash"
+    cases below);
   * search kernels spgemmMaskedEdgeKernel + spgemmMaskedHeavyKernel
-    (kernels/spgemm_masked.cuh): a mask without a CSC side ("search" cases), or
-    every mask with GB200_SPGEMM_HASH=0;
-  * warp-per-row spgemmMaskedKernel: GB200_SPGEMM_ROWS=1.
-Both switches are read once per process, so test_other_routes_in_a_subprocess
-re-runs this module under each of them.
+    (kernels/spgemm_masked.cuh): a mask without a CSC side ("search" cases).
 
 The designed operands put list lengths and partner counts at, below and one past
 every boundary of the hash kernels.  The boundaries (kernels/spgemm_hash.cuh,
@@ -33,8 +29,6 @@ kernels/spgemm_masked.cuh; test_kernel_constants_match_the_table checks them):
 import collections
 import os
 import re
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -208,6 +202,14 @@ def oracle(p):
                           p.M.ptr, p.M.ind, p.M.val)
 
 
+def tc_lower(scale=14):
+    """L = tril of an R-MAT: operand, mask and output pattern of the triangle count
+    (L * L^T) .* L."""
+    rp, ci = orc.rmat_csr(scale)
+    lr, lc = orc.tril(rp, ci)
+    return Csr(len(lr) - 1, len(lr) - 1, lr, lc, np.ones(len(lc), np.int32))
+
+
 def routes(p):
     """Where the hash kernels take every mask entry: a per-entry table."""
     i, j = p.M.rows(), p.M.ind
@@ -313,11 +315,18 @@ def test_designed_operands_reach_every_class_pass_and_split():
     assert ((np.diff(p.M.ptr) == 0) & (np.diff(p.A.ptr) > 0)).any()
     col_cnt = np.bincount(p.M.ind, minlength=p.M.ncols)
     assert ((col_cnt == 0) & (np.diff(p.Bt.ptr) > 0)).any()
-    # search route: entries for the thread-per-entry and for the heavy kernel
+    # search route: entries for the thread-per-entry and for the heavy kernel, at
+    # the threshold and one past it
     shorter = np.minimum(r["a_len"], r["b_len"])
-    assert (shorter > HEAVY).any() and (shorter <= HEAVY).any()
+    assert {HEAVY, HEAVY + 1} <= set(shorter.tolist())
     assert (shorter > HEAVY).sum() > 100
     assert np.count_nonzero(want) > len(want) // 2
+    # the triangle count's entry (i, j) meets rows i and j of L: on the search
+    # route too it reaches both kernels
+    L = tc_lower()
+    deg = np.diff(L.ptr)
+    shorter = np.minimum(deg[L.rows()], deg[L.ind])
+    assert (shorter > HEAVY).any() and (shorter <= HEAVY).any()
 
 
 # ---------------------------------------------------------------------------
@@ -427,38 +436,17 @@ def tc_per_entry(rp, ci):
 @pytest.mark.gpu
 def test_triangle_count_twice_on_the_same_output(gb):
     """algorithm.tc twice into one B, per entry both times (B keeps its buffers
-    between the calls)."""
+    between the calls), on both routes: L is the mask, so L with a CSC side takes
+    the hash kernels and L without one the search kernels."""
     from graphblast_b200 import algorithm
-    rp, ci = orc.rmat_csr(14)
-    lr, lc = orc.tril(rp, ci)
-    L = Csr(len(lr) - 1, len(lr) - 1, lr, lc, np.ones(len(lc), np.int32))
-    dL = device_matrix(gb, L)
-    B = gb.Matrix(L.nrows, L.nrows, dtype=gb.api.INT32)
-    want = tc_per_entry(lr, lc)
+    L = tc_lower()
+    want = tc_per_entry(L.ptr, L.ind)
     desc = gb.Descriptor(mxvmode=0)
-    for _ in range(2):
-        ntris, _ = algorithm.tc(dL, B, desc)
-        assert ntris == int(want.sum()) == orc.tc(lr, lc)
-        check_entries(B, L, want)
+    for route in ROUTES:
+        dL = device_matrix(gb, L, with_csc=(route == "hash"))
+        B = gb.Matrix(L.nrows, L.nrows, dtype=gb.api.INT32)
+        for _ in range(2):
+            ntris, _ = algorithm.tc(dL, B, desc)
+            assert ntris == int(want.sum()) == orc.tc(L.ptr, L.ind), route
+            check_entries(B, L, want)
 
-
-ROUTE_ENVS = {"rows": {"GB200_SPGEMM_ROWS": "1"}, "search": {"GB200_SPGEMM_HASH": "0"}}
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("name", sorted(ROUTE_ENVS))
-def test_other_routes_in_a_subprocess(name):
-    """This module's GPU tests again with the warp-per-row kernel
-    (GB200_SPGEMM_ROWS=1) and with the search kernels for every mask
-    (GB200_SPGEMM_HASH=0): all routes agree with the oracle, hence with each
-    other."""
-    if any(os.environ.get(k) for env in ROUTE_ENVS.values() for k in env):
-        pytest.skip("already running under a route switch")
-    env = dict(os.environ)
-    env.update(ROUTE_ENVS[name])
-    cmd = [sys.executable, "-m", "pytest", "-x", "-q", "-p", "no:cacheprovider",
-           "-m", "gpu", os.path.abspath(__file__), "-k", "not other_routes"]
-    r = subprocess.run(cmd, env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT,
-                       text=True, timeout=1500)
-    assert r.returncode == 0, r.stdout[-4000:]
-    assert " passed" in r.stdout and " failed" not in r.stdout

@@ -84,34 +84,28 @@ def test_edge_share_check_does_not_change_results(gb):
 
 
 @pytest.mark.parametrize("name", ["PlusMultiplies", "MinimumPlus"])
-def test_column_relabelling_is_bit_identical(gb, name):
-    """GB200_SPMV_RELABEL=1 (experimental, off by default): the generic pull SpMV
-    gathers through relabelled column indices from a permuted copy of u; products
-    and their order are unchanged, so the result must not differ in a single bit
-    (random float values on purpose)."""
-    import os
+def test_repeated_generic_pulls_are_bit_identical(gb, name):
+    """The generic pull SpMV with random float values, twice on each of three
+    freshly built matrices: the first pull computes the matrix's tile partition,
+    the second reuses it.  Every result must equal every other in every bit."""
     rp, ci = orc.rmat_csr(12)
     n = len(rp) - 1
     rng = np.random.RandomState(9)
     val = rng.rand(len(ci)).astype(np.float32) + 0.5
     u_h = rng.rand(n).astype(np.float32) + 0.5
     sem = getattr(gb.Semiring, name)
-    out = {}
-    for flag in ("0", "1", "1"):                   # second "1" reuses the cached copy
-        os.environ["GB200_SPMV_RELABEL"] = flag
-        try:
-            A = make_matrix(gb, rp, ci, val, symmetric=False)
-            desc = gb.Descriptor(mxvmode=2)
-            u = gb.Vector(n)
-            u.build(u_h)
-            w = gb.Vector(n)
+    out = []
+    for _ in range(3):
+        A = make_matrix(gb, rp, ci, val, symmetric=False)
+        desc = gb.Descriptor(mxvmode=2)
+        u = gb.Vector(n)
+        u.build(u_h)
+        w = gb.Vector(n)
+        for _ in range(2):
             gb.vxm(w, None, None, sem, u, A, desc)
-            gb.vxm(w, None, None, sem, u, A, desc)
-            out.setdefault(flag, []).append(w.extractTuples().copy())
-        finally:
-            os.environ["GB200_SPMV_RELABEL"] = "0"
-    assert np.array_equal(out["0"][0].view(np.uint32), out["1"][0].view(np.uint32))
-    assert np.array_equal(out["0"][0].view(np.uint32), out["1"][1].view(np.uint32))
+            out.append(w.extractTuples().view(np.uint32).copy())
+    for got in out[1:]:
+        assert np.array_equal(out[0], got)
 
 
 @pytest.mark.parametrize("n", [11, 33, 64, 1000])

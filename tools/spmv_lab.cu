@@ -125,7 +125,7 @@ streamGatherWindowKernel(float* out, const int* colind, const float* val,
 
 // Ceiling of the hub design: stream + (hub from shared memory | cold gather), no
 // row reduction.  One persistent CTA per SM, K hub slots in dynamic shared memory.
-template <int NT, bool ColdNoAlloc>
+template <int NT>
 __global__ void __launch_bounds__(NT, 1)
 streamGatherHubKernel(float* out, const int* enc, const float* val, const float* u,
                       const float* hub_vals, int K, long long nnz) {
@@ -143,7 +143,7 @@ streamGatherHubKernel(float* out, const int* enc, const float* val, const float*
 #pragma unroll
     for (int j = 0; j < 8; ++j)
       if (cw.w[j] >= 0)
-        uv[j] = ColdNoAlloc ? ldGatherCold(u + cw.w[j], pol) : ldGather(u + cw.w[j], pol);
+        uv[j] = ldGather(u + cw.w[j], pol);
 #pragma unroll
     for (int j = 0; j < 8; ++j)
       if (cw.w[j] < 0) uv[j] = s_hubv[cw.w[j] & 0x7fffffff];
@@ -179,7 +179,7 @@ float runHub(float* w, const HubIndex& h, const int* rowptr, const float* val,
   return best;
 }
 
-template <int NT, int IPT, bool Gather, bool LaneMajor>
+template <int NT, int IPT, bool LaneMajor>
 float runMerge(float* w, const int* rowptr, const int* colind, const float* val,
                const float* u, int n, int nnz, int reps, int carveout) {
   SR op;
@@ -190,7 +190,7 @@ float runMerge(float* w, const int* rowptr, const int* colind, const float* val,
   thrust::device_vector<float> cval(nctas);
   spmvMergePartitionKernel<<<(nctas + 256)/256, 256>>>(
       thrust::raw_pointer_cast(tiles.data()), rowptr, n, nnz, nctas, tile);
-  auto kern = spmvMergeKernelT<NT, IPT, !LaneMajor, (Gather ? 1 : 0), LaneMajor, float, float, float,
+  auto kern = spmvMergeKernelT<NT, IPT, LaneMajor, float, float, float,
       decltype(graphblas::extractMul(op)), decltype(graphblas::extractAdd(op))>;
   if (carveout >= 0)
     cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout,
@@ -287,27 +287,26 @@ int main(int argc, char** argv) {
   }
   report("stream + gather (one chunk per thread)", best);
 
-#define LAB(NT, IPT, G, LM, CARVE)                                           \
+#define LAB(NT, IPT, LM, CARVE)                                              \
   { char name[96];                                                           \
     snprintf(name, sizeof(name),                                             \
-             "merge NT=%d IPT=%d gather=%d lanemajor=%d carveout=%d",        \
-             NT, IPT, (int)G, (int)LM, CARVE);                               \
-    report(name, runMerge<NT, IPT, G, LM>(wp, rp, ci, va, up, (int)n,        \
-                                          (int)nnz, reps, CARVE)); }
+             "merge NT=%d IPT=%d lanemajor=%d carveout=%d",                  \
+             NT, IPT, (int)LM, CARVE);                                       \
+    report(name, runMerge<NT, IPT, LM>(wp, rp, ci, va, up, (int)n,           \
+                                       (int)nnz, reps, CARVE)); }
   if (getenv("LAB_FULL")) {
-  LAB(128, 7, true, false, 25)
-  LAB(128, 9, true, false, 25)
-  LAB(128, 11, true, false, 25)
-  LAB(128, 15, true, false, 25)
-  LAB(128, 15, true, false, 33)
-  LAB(64, 11, true, false, 25)
-  LAB(64, 15, true, false, 25)
-  LAB(64, 19, true, false, 25)
-  LAB(256, 7, true, false, 25)
-  LAB(256, 9, true, false, 33)
-  LAB(128, 9, true, true, 25)
-  LAB(128, 9, false, false, 25)
-  } else { LAB(128, 9, true, false, 25) }
+  LAB(128, 7, false, 25)
+  LAB(128, 9, false, 25)
+  LAB(128, 11, false, 25)
+  LAB(128, 15, false, 25)
+  LAB(128, 15, false, 33)
+  LAB(64, 11, false, 25)
+  LAB(64, 15, false, 25)
+  LAB(64, 19, false, 25)
+  LAB(256, 7, false, 25)
+  LAB(256, 9, false, 33)
+  LAB(128, 9, true, 25)
+  } else { LAB(128, 9, false, 25) }
 
   // wavefront vs sector: gathers folded into 4 KB / 64 KB / 1 MB windows
   for (int mask : {1023, 16383, 262143}) {
@@ -330,14 +329,8 @@ int main(int argc, char** argv) {
     if (K == 0) cudaMemcpy(h.enc_ci, ci, nnz*sizeof(int), cudaMemcpyDeviceToDevice);
     hubPrepassKernel<<<(K + 255)/256 + 1, 256>>>((float*)h.hub_vals, up, h.hub_ids,
         K > 0 ? h.count : 0, K > 0 ? K : 4, 0.f, wp, (const Index*)NULL, 0, 0.f);
-    for (int variant = 0; variant < 4; ++variant) {
-      const int nt = (variant & 1) ? 512 : 1024;
-      const bool cold = (variant & 2) != 0;
-      auto k1024a = streamGatherHubKernel<1024, false>;
-      auto k1024c = streamGatherHubKernel<1024, true>;
-      auto k512a = streamGatherHubKernel<512, false>;
-      auto k512c = streamGatherHubKernel<512, true>;
-      auto kern = nt == 1024 ? (cold ? k1024c : k1024a) : (cold ? k512c : k512a);
+    for (int nt : {1024, 512}) {
+      auto kern = nt == 1024 ? streamGatherHubKernel<1024> : streamGatherHubKernel<512>;
       cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200*1024);
       best = 1e30f;
       for (int r = 0; r < reps + 1; ++r) {
@@ -347,8 +340,8 @@ int main(int argc, char** argv) {
         if (r > 0 && ms < best) best = ms;
       }
       char name[96];
-      snprintf(name, sizeof(name), "ceiling K=%d cover=%.3f NT=%d cold_noalloc=%d", K,
-               K > 0 ? h.coverage : 0.0, nt, (int)cold);
+      snprintf(name, sizeof(name), "ceiling K=%d cover=%.3f NT=%d", K,
+               K > 0 ? h.coverage : 0.0, nt);
       report(name, best);
     }
     h.release();
@@ -357,7 +350,7 @@ int main(int argc, char** argv) {
 
   // ---- hub kernel -------------------------------------------------------------
   // reference result: the merge kernel
-  runMerge<128, 9, true, false>(wp, rp, ci, va, up, (int)n, (int)nnz, 1, 25);
+  runMerge<128, 9, false>(wp, rp, ci, va, up, (int)n, (int)nnz, 1, 25);
   std::vector<float> want(n), got(n);
   std::vector<int> h_rp(n + 1);
   cudaMemcpy(h_rp.data(), rp, (n + 1)*sizeof(int), cudaMemcpyDeviceToHost);
