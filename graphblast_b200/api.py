@@ -1,4 +1,9 @@
-"""Host-side mirror of the reference interface for the mxv/vxm + masked-mxm path.
+"""Host-side mirror of the reference interface for the mxv/vxm + mxm path.
+
+mxm with a mask is the int plus-times product of triangle counting (C takes the
+mask's pattern); mxm(C, None, None, op, A, B, desc) is the unmasked sparse
+product C = A (+.x) B for FP32 matrices over any order-independent semiring and
+for INT32 matrices over PlusMultiplies.
 
 Classes and functions keep the reference's names, argument meaning and error
 behaviour (every call returns/raises a graphblas::Info code):

@@ -794,6 +794,15 @@ int gb200_mxm(gb200_matrix_t C, gb200_matrix_t mask, int semiring,
               gb200_matrix_t A, gb200_matrix_t B, gb200_desc_t desc) {
   if (C == NULL || A == NULL || B == NULL || desc == NULL)
     return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
+  if (mask == NULL && C->f != NULL && A->f != NULL && B->f != NULL) {
+    GB200_REQUIRE_DEVICE();
+    GB200_SEMIRING_DISPATCH(semiring, {
+      return rc((graphblas::mxm<float, float, float, float>(C->f,
+          static_cast<graphblas::Matrix<float>*>(NULL), GrB_NULL, op, A->f, B->f,
+          &desc->desc)));
+    });
+    return 0;
+  }
   if (C->i == NULL || A->i == NULL || B->i == NULL ||
       (mask != NULL && mask->i == NULL))
     return rc(graphblas::GrB_DOMAIN_MISMATCH);

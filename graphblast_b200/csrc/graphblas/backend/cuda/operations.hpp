@@ -99,8 +99,9 @@ template <typename TC, typename TA, typename TB, typename TMask,
 Info mxm(Matrix<TC>* C, const Matrix<TMask>* mask, AccumT accum, SemiringT op,
     const Matrix<TA>* A, const Matrix<TB>* B, Descriptor* desc) {
   if (!A->isSparse() || !B->isSparse()) return notBuilt("mxm with a dense operand (SpMM / GEMM)");
-  if (mask == NULL) return notBuilt("unmasked SpGEMM");
   CHECK(C->setStorage(GrB_SPARSE));
+  if (mask == NULL)
+    return spgemmUnmasked(&C->sparse_, accum, op, &A->sparse_, &B->sparse_, desc);
   return spgemmMasked(&C->sparse_, mask, accum, op, &A->sparse_, &B->sparse_, desc);
 }
 

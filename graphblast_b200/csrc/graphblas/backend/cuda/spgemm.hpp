@@ -1,10 +1,11 @@
-// graphblast_b200 backend — masked SpGEMM host (triangle counting path).
+// graphblast_b200 backend — SpGEMM hosts.
 //
-// Replaces reference graphblas/backend/cuda/spgemm.hpp:22-110 (spgemmMasked).
-// C takes the mask's pattern (C->dup(mask)) and one value per mask entry is
-// computed as the dot product A(i,:) . B(:,j).  The reference's unmasked
-// cusparse_spgemm/cusparse_spgemm2 (:114-512) call cuSPARSE csrgemm2 entry
-// points that no longer exist in CUDA 12 and are out of scope (SURVEY.md §2 #13).
+// spgemmMasked replaces reference graphblas/backend/cuda/spgemm.hpp:22-110 (the
+// triangle counting path): C takes the mask's pattern (C->dup(mask)) and one value
+// per mask entry is computed as the dot product A(i,:) . B(:,j).
+// spgemmUnmasked is the unmasked product, this project's own hash-row kernels
+// (kernels/spgemm_unmasked.cuh) in place of the reference's cuSPARSE csrgemm2
+// calls (:114-512), which no longer exist in CUDA 12.
 #ifndef GRAPHBLAS_BACKEND_CUDA_SPGEMM_HPP_
 #define GRAPHBLAS_BACKEND_CUDA_SPGEMM_HPP_
 
@@ -191,6 +192,256 @@ Info spgemmMasked(SparseMatrix<c>* C, const Matrix<m>* mask, BinaryOpT accum,
   C->need_update_ = true;
   C->csr_initialized_ = true;
   C->csc_initialized_ = false;
+  return GrB_SUCCESS;
+}
+
+// Semirings whose add is not associative (greater, less, not_equal_to): their fold
+// depends on the order of the products, and a hash accumulator has none.
+template <typename S> struct FoldNeedsOrder : std::false_type {};
+template <typename X, typename Y, typename Z>
+struct FoldNeedsOrder<GreaterPlusSemiring<X, Y, Z> > : std::true_type {};
+template <typename X, typename Y, typename Z>
+struct FoldNeedsOrder<CustomLessPlusSemiring<X, Y, Z> > : std::true_type {};
+template <typename X, typename Y, typename Z>
+struct FoldNeedsOrder<NotEqualToPlusSemiring<X, Y, Z> > : std::true_type {};
+template <typename X, typename Y, typename Z>
+struct FoldNeedsOrder<CustomLessLessSemiring<X, Y, Z> > : std::true_type {};
+
+// Semirings whose add is plus: the numeric kernels combine with a native atomicAdd.
+template <typename S> struct AddIsPlus : std::false_type {};
+#define GB_MXM_PLUS_ADD(NAME)                                                 \
+  template <typename X, typename Y, typename Z>                               \
+  struct AddIsPlus<NAME<X, Y, Z> > : std::true_type {};
+GB_MXM_PLUS_ADD(PlusMultipliesSemiring)
+GB_MXM_PLUS_ADD(PlusDividesSemiring)
+GB_MXM_PLUS_ADD(PlusGreaterSemiring)
+GB_MXM_PLUS_ADD(PlusMinusSemiring)
+GB_MXM_PLUS_ADD(PlusLessSemiring)
+GB_MXM_PLUS_ADD(PlusNotEqualToSemiring)
+#undef GB_MXM_PLUS_ADD
+
+// Largest scratch the dense-accumulator kernels take for their per-CTA arrays; the
+// CTA count shrinks to fit.
+#define GB_MXM_DENSE_BYTES (size_t(1) << 29)
+
+template <typename KernelT>
+void mxmSetSmem(KernelT kernel, size_t bytes) {
+  CUDA_CALL(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+      static_cast<int>(bytes)));
+}
+
+// Numeric launches of spgemmUnmasked, one per bin that holds rows.
+template <bool PLUS, typename c, typename a, typename b, typename MulOp, typename AddOp>
+void mxmNumericPass(const unsigned int* count, const Index* lists, size_t stride,
+    MxmCells* cells, const Index* A_ptr, const Index* A_ind, const a* A_val,
+    const Index* B_ptr, const Index* B_ind, const b* B_val, Index ncols,
+    const Index* C_ptr, Index* C_ind, c* C_val, MulOp mul_op, AddOp add_op,
+    c identity, Descriptor* desc, cudaStream_t s) {
+  const int sms = runtime().sm_count;
+  if (count[0]) {
+    auto kernel = mxmNumericKernel<256, true, 2*GB_MXM_NUM_S, PLUS, c, a, b, MulOp, AddOp>;
+    const size_t smem = GB_MXM_WARPS*2*(2*GB_MXM_NUM_S)*sizeof(int);
+    static bool configured = false;
+    if (!configured) { mxmSetSmem(kernel, smem); configured = true; }
+    const unsigned int want = (count[0] + GB_MXM_WARPS - 1)/GB_MXM_WARPS;
+    kernel<<<want < 6u*sms ? want : 6u*sms, 256, smem, s>>>(lists, cells, 0,
+        cells->grab, A_ptr, A_ind, A_val, B_ptr, B_ind, B_val, C_ptr, C_ind, C_val,
+        mul_op, add_op, identity);
+    GB_KERNEL_CHECK();
+  }
+  if (count[1]) {
+    auto kernel = mxmNumericKernel<256, false, 2*GB_MXM_NUM_M, PLUS, c, a, b, MulOp, AddOp>;
+    const size_t smem = 2*(2*GB_MXM_NUM_M)*sizeof(int);
+    static bool configured = false;
+    if (!configured) { mxmSetSmem(kernel, smem); configured = true; }
+    kernel<<<count[1] < 6u*sms ? count[1] : 6u*sms, 256, smem, s>>>(lists + stride,
+        cells, 1, cells->grab + 1, A_ptr, A_ind, A_val, B_ptr, B_ind, B_val, C_ptr,
+        C_ind, C_val, mul_op, add_op, identity);
+    GB_KERNEL_CHECK();
+  }
+  if (count[2]) {
+    auto kernel = mxmNumericKernel<1024, false, 2*GB_MXM_NUM_L, PLUS, c, a, b, MulOp, AddOp>;
+    const size_t smem = 2*(2*GB_MXM_NUM_L)*sizeof(int);
+    static bool configured = false;
+    if (!configured) { mxmSetSmem(kernel, smem); configured = true; }
+    kernel<<<count[2] < 1u*sms ? count[2] : 1u*sms, 1024, smem, s>>>(
+        lists + 2*stride, cells, 2, cells->grab + 2, A_ptr, A_ind, A_val, B_ptr,
+        B_ind, B_val, C_ptr, C_ind, C_val, mul_op, add_op, identity);
+    GB_KERNEL_CHECK();
+  }
+  if (count[3]) {
+    const size_t words = (static_cast<size_t>(ncols) + 31)/32;
+    const size_t per_cta = static_cast<size_t>(ncols)*sizeof(c) + words*sizeof(unsigned int);
+    size_t ctas = GB_MXM_DENSE_BYTES/per_cta;
+    if (ctas > count[3]) ctas = count[3];
+    if (ctas > static_cast<size_t>(sms)) ctas = sms;
+    if (ctas < 1) ctas = 1;
+    c* acc = reinterpret_cast<c*>(desc->scratch(GB_SCRATCH_VEC_B, ctas*per_cta));
+    unsigned int* bits = reinterpret_cast<unsigned int*>(acc + ctas*ncols);
+    mxmFillKernel<<<gridFor(ctas*ncols, 256), 256, 0, s>>>(acc, ctas*ncols, identity);
+    GB_KERNEL_CHECK();
+    CUDA_CALL(cudaMemsetAsync(bits, 0, ctas*words*sizeof(unsigned int), s));
+    mxmNumericDenseKernel<1024, PLUS><<<static_cast<int>(ctas), 1024, 0, s>>>(
+        lists + 3*stride, cells, 3, cells->grab + 3, A_ptr, A_ind, A_val, B_ptr,
+        B_ind, B_val, C_ptr, C_ind, C_val, mul_op, add_op, identity, acc, bits, ncols,
+        words);
+    GB_KERNEL_CHECK();
+  }
+}
+
+// C = A (+.x) B without a mask (kernels/spgemm_unmasked.cuh).  C gets new arrays:
+// it may be A or B.  accum is ignored, as in the masked product: C is replaced.
+// Returns GrB_OUT_OF_MEMORY, with C untouched, when nnz(C) would not fit an Index.
+template <typename c, typename a, typename b, typename SemiringT>
+Info spgemmUnmaskedProduct(SparseMatrix<c>* C, SemiringT op,
+    const SparseMatrix<a>* A, const SparseMatrix<b>* B, Descriptor* desc);
+
+template <typename c, typename a, typename b, typename BinaryOpT, typename SemiringT>
+Info spgemmUnmasked(SparseMatrix<c>* C, BinaryOpT accum, SemiringT op,
+    const SparseMatrix<a>* A, const SparseMatrix<b>* B, Descriptor* desc) {
+  if constexpr (FoldNeedsOrder<SemiringT>::value) return GrB_NOT_IMPLEMENTED;
+  else return spgemmUnmaskedProduct(C, op, A, B, desc);
+}
+
+template <typename c, typename a, typename b, typename SemiringT>
+Info spgemmUnmaskedProduct(SparseMatrix<c>* C, SemiringT op,
+    const SparseMatrix<a>* A, const SparseMatrix<b>* B, Descriptor* desc) {
+  Desc_value inp0_mode, inp1_mode;
+  CHECK(desc->get(GrB_INP0, &inp0_mode));
+  CHECK(desc->get(GrB_INP1, &inp1_mode));
+  const bool use_tran_A = inp0_mode == GrB_TRAN;
+  const bool use_tran_B = inp1_mode == GrB_TRAN;
+
+  const Index* A_ptr = use_tran_A ? A->d_cscColPtr_ : A->d_csrRowPtr_;
+  const Index* A_ind = use_tran_A ? A->d_cscRowInd_ : A->d_csrColInd_;
+  const a*     A_val = use_tran_A ? A->d_cscVal_    : A->d_csrVal_;
+  const Index  m     = use_tran_A ? A->ncols_       : A->nrows_;
+  const Index* B_ptr = use_tran_B ? B->d_cscColPtr_ : B->d_csrRowPtr_;
+  const Index* B_ind = use_tran_B ? B->d_cscRowInd_ : B->d_csrColInd_;
+  const b*     B_val = use_tran_B ? B->d_cscVal_    : B->d_csrVal_;
+  const Index  n     = use_tran_B ? B->nrows_       : B->ncols_;
+  // op(A) is m x k, op(B) k x n: the kernels index B's pointer array with A's
+  // columns, and C's arrays with m and n
+  const Index A_ncols = use_tran_A ? A->nrows_ : A->ncols_;
+  const Index B_nrows = use_tran_B ? B->ncols_ : B->nrows_;
+  if (A_ncols != B_nrows || m != C->nrows_ || n != C->ncols_)
+    return GrB_DIMENSION_MISMATCH;
+  if (A_ptr == NULL || A_ind == NULL || A_val == NULL ||
+      B_ptr == NULL || B_ind == NULL || B_val == NULL)
+    return GrB_UNINITIALIZED_OBJECT;
+
+  cudaStream_t s = gbStream();
+  const int sms = runtime().sm_count;
+  const size_t stride = m > 0 ? static_cast<size_t>(m) : 1;
+  // row lists of the four bins, then the cells (8-byte aligned)
+  Index* lists = reinterpret_cast<Index*>(desc->scratch(GB_SCRATCH_VEC_A,
+      GB_MXM_NBIN*stride*sizeof(Index) + sizeof(MxmCells) + 8));
+  MxmCells* cells = reinterpret_cast<MxmCells*>(lists + GB_MXM_NBIN*stride);
+  // row bounds, then counts, then (scanned in place) C's row offsets
+  Index* rowptr = reinterpret_cast<Index*>(gbMalloc((static_cast<size_t>(m) + 1)*sizeof(Index)));
+  CUDA_CALL(cudaMemsetAsync(rowptr + m, 0, sizeof(Index), s));
+  CUDA_CALL(cudaMemsetAsync(cells, 0, sizeof(MxmCells), s));
+
+  // 1. bounds and symbolic bins
+  if (m > 0) {
+    mxmRowBoundKernel<<<gridFor(static_cast<size_t>(m), 256), 256, 0, s>>>(A_ptr, A_ind,
+        B_ptr, m, n, rowptr);
+    GB_KERNEL_CHECK();
+    mxmClassifyKernel<<<gridFor(static_cast<size_t>(m), 256), 256, 0, s>>>(rowptr, m,
+        A_ptr, GB_MXM_SYM_S, GB_MXM_SYM_M, GB_MXM_SYM_L, lists, stride, cells);
+    GB_KERNEL_CHECK();
+  }
+  const MxmCells sym = runtime().fetch(cells);
+  if (sym.exact > static_cast<unsigned long long>(INT32_MAX)) {
+    gbFree(rowptr);
+    return GrB_OUT_OF_MEMORY;
+  }
+
+  // 2. symbolic: distinct columns per row
+  if (sym.count[0]) {
+    auto kernel = mxmSymbolicKernel<256, true, 2*GB_MXM_SYM_S>;
+    const size_t smem = GB_MXM_WARPS*(2*GB_MXM_SYM_S)*sizeof(int);
+    static bool configured = false;
+    if (!configured) { mxmSetSmem(kernel, smem); configured = true; }
+    const unsigned int want = (sym.count[0] + GB_MXM_WARPS - 1)/GB_MXM_WARPS;
+    kernel<<<want < 3u*sms ? want : 3u*sms, 256, smem, s>>>(lists, cells, 0,
+        cells->grab, A_ptr, A_ind, B_ptr, B_ind, rowptr);
+    GB_KERNEL_CHECK();
+  }
+  if (sym.count[1]) {
+    auto kernel = mxmSymbolicKernel<256, false, 2*GB_MXM_SYM_M>;
+    const size_t smem = (2*GB_MXM_SYM_M)*sizeof(int);
+    static bool configured = false;
+    if (!configured) { mxmSetSmem(kernel, smem); configured = true; }
+    kernel<<<sym.count[1] < 6u*sms ? sym.count[1] : 6u*sms, 256, smem, s>>>(
+        lists + stride, cells, 1, cells->grab + 1, A_ptr, A_ind, B_ptr, B_ind, rowptr);
+    GB_KERNEL_CHECK();
+  }
+  if (sym.count[2]) {
+    auto kernel = mxmSymbolicKernel<1024, false, 2*GB_MXM_SYM_L>;
+    const size_t smem = (2*GB_MXM_SYM_L)*sizeof(int);
+    static bool configured = false;
+    if (!configured) { mxmSetSmem(kernel, smem); configured = true; }
+    kernel<<<sym.count[2] < 1u*sms ? sym.count[2] : 1u*sms, 1024, smem, s>>>(
+        lists + 2*stride, cells, 2, cells->grab + 2, A_ptr, A_ind, B_ptr, B_ind, rowptr);
+    GB_KERNEL_CHECK();
+  }
+  if (sym.count[3]) {
+    const size_t words = (static_cast<size_t>(n) + 31)/32;
+    size_t ctas = GB_MXM_DENSE_BYTES/(words*sizeof(unsigned int));
+    if (ctas > sym.count[3]) ctas = sym.count[3];
+    if (ctas > static_cast<size_t>(sms)) ctas = sms;
+    if (ctas < 1) ctas = 1;
+    unsigned int* bits = reinterpret_cast<unsigned int*>(desc->scratch(GB_SCRATCH_VEC_B,
+        ctas*words*sizeof(unsigned int)));
+    CUDA_CALL(cudaMemsetAsync(bits, 0, ctas*words*sizeof(unsigned int), s));
+    mxmSymbolicDenseKernel<1024><<<static_cast<int>(ctas), 1024, 0, s>>>(
+        lists + 3*stride, cells, 3, cells->grab + 3, A_ptr, A_ind, B_ptr, B_ind,
+        rowptr, bits, words);
+    GB_KERNEL_CHECK();
+  }
+
+  // 3. numeric bins by the exact counts, their 64-bit total, C's row offsets
+  CUDA_CALL(cudaMemsetAsync(cells, 0, sizeof(MxmCells), s));
+  if (m > 0) {
+    mxmClassifyKernel<<<gridFor(static_cast<size_t>(m), 256), 256, 0, s>>>(rowptr, m,
+        NULL, GB_MXM_NUM_S, GB_MXM_NUM_M, GB_MXM_NUM_L, lists, stride, cells);
+    GB_KERNEL_CHECK();
+  }
+  const MxmCells num = runtime().fetch(cells);
+  if (num.total > static_cast<unsigned long long>(INT32_MAX)) {
+    gbFree(rowptr);
+    return GrB_OUT_OF_MEMORY;
+  }
+  const Index nnz = static_cast<Index>(num.total);
+  scanExclusiveInPlace(rowptr, static_cast<long long>(m) + 1);
+  Index* colind = reinterpret_cast<Index*>(gbMalloc((nnz > 0 ? nnz : 1)*sizeof(Index)));
+  c* val = reinterpret_cast<c*>(gbMalloc((nnz > 0 ? nnz : 1)*sizeof(c)));
+
+  // 4. numeric
+  mxmNumericPass<AddIsPlus<SemiringT>::value>(num.count, lists, stride, cells, A_ptr,
+      A_ind, A_val, B_ptr, B_ind, B_val, n, rowptr, colind, val, extractMul(op),
+      extractAdd(op), static_cast<c>(op.identity()), desc, s);
+
+  // swap in: the old arrays (and every cache built on them) go, stream-ordered
+  // after the kernels above that may still read them through A or B
+  CHECK(C->clear());
+  C->d_csrRowPtr_ = rowptr;
+  C->d_csrColInd_ = colind;
+  C->d_csrVal_ = val;
+  C->csr_ownership_ = true;
+  C->nvals_ = nnz;
+  C->ncapacity_ = nnz;
+  C->symmetric_ = false;
+  if (C->format_ == GrB_SPARSE_MATRIX_CSRCSC) {
+    ingestCsrToCsc<c>(C->nrows_, C->ncols_, nnz, rowptr, colind, val,
+        &C->d_cscColPtr_, &C->d_cscRowInd_, &C->d_cscVal_);
+    C->csc_ownership_ = true;
+    C->cscval_ownership_ = true;
+    C->csc_initialized_ = true;
+  }
+  C->csr_initialized_ = true;
+  C->need_update_ = true;
   return GrB_SUCCESS;
 }
 }  // namespace backend

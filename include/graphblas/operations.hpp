@@ -105,11 +105,25 @@ Info mxm(Matrix<TC>* C, const Matrix<TMask>* mask, AccumT accum, SemiringT op,
          const Matrix<TA>* A, const Matrix<TB>* B, Descriptor* desc) {
   using namespace ops_detail;
   GB_REQUIRE(C, A, B, desc);
-  GB_SHAPES(Contract()
-      .equal(rowsOf(B), colsOf(A), "B.nrows != A.ncols")
-      .equal(rowsOf(A), rowsOf(C), "A.nrows != C.nrows")
-      .equal(colsOf(B), colsOf(C), "B.ncols != C.ncols")
-      .alike(C, mask, "C.nrows != mask.nrows", "C.ncols != mask.ncols"));
+  if (mask == NULL) {
+    // the unmasked product multiplies op(A) by op(B), with op what GrB_INP0 /
+    // GrB_INP1 name: its shapes are those of the transposes
+    Desc_value inp0, inp1;
+    CHECK(desc->get(GrB_INP0, &inp0));
+    CHECK(desc->get(GrB_INP1, &inp1));
+    const bool ta = inp0 == GrB_TRAN, tb = inp1 == GrB_TRAN;
+    GB_SHAPES(Contract()
+        .equal(tb ? colsOf(B) : rowsOf(B), ta ? rowsOf(A) : colsOf(A),
+               "op(B).nrows != op(A).ncols")
+        .equal(ta ? colsOf(A) : rowsOf(A), rowsOf(C), "op(A).nrows != C.nrows")
+        .equal(tb ? rowsOf(B) : colsOf(B), colsOf(C), "op(B).ncols != C.ncols"));
+  } else {
+    GB_SHAPES(Contract()
+        .equal(rowsOf(B), colsOf(A), "B.nrows != A.ncols")
+        .equal(rowsOf(A), rowsOf(C), "A.nrows != C.nrows")
+        .equal(colsOf(B), colsOf(C), "B.ncols != C.ncols")
+        .alike(C, mask, "C.nrows != mask.nrows", "C.ncols != mask.ncols"));
+  }
   return backend::mxm<TC, TA, TB, TMask>(raw(C), raw(mask), accum, op, raw(A), raw(B),
                                         raw(desc));
 }

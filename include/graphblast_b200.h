@@ -201,7 +201,13 @@ int gb200_vxm(gb200_vector_t w, gb200_vector_t mask, int use_accum, int semiring
               gb200_vector_t u, gb200_matrix_t A, gb200_desc_t desc);      /* vxm :59-87 */
 int gb200_mxv(gb200_vector_t w, gb200_vector_t mask, int use_accum, int semiring,
               gb200_matrix_t A, gb200_vector_t u, gb200_desc_t desc);      /* mxv :97-127 */
-/* INT32 matrices, PlusMultiplies<int> (the triangle-counting instantiation). */
+/* With a mask: INT32 matrices, PlusMultiplies<int> (the triangle-counting
+ * instantiation); C takes the mask's pattern.
+ * mask == NULL: C = A (+.x) B, C replaced (accum is not applied).  FP32 C/A/B over
+ * every semiring except the four whose add is not associative (GreaterPlus,
+ * CustomLessPlus, NotEqualToPlus, CustomLessLess: GrB_NOT_IMPLEMENTED); INT32
+ * C/A/B over PlusMultiplies only; mixed element types give GrB_DOMAIN_MISMATCH.
+ * GrB_OUT_OF_MEMORY, with C unchanged, when nnz(C) would exceed INT32_MAX. */
 int gb200_mxm(gb200_matrix_t C, gb200_matrix_t mask, int semiring,
               gb200_matrix_t A, gb200_matrix_t B, gb200_desc_t desc);      /* mxm :22-49 */
 int gb200_ewise_add(gb200_vector_t w, gb200_vector_t mask, int semiring,
