@@ -56,9 +56,11 @@ Info bfsFused(Vector<float>* v, const Matrix<a>* A, Index s, Descriptor* desc, i
   CHECK(v->setStorage(GrB_DENSE));
   CHECK(v->dense_.allocateGpu());
 
-  // first-neighbour summary of the pulled structure (shared with the Boolean pull)
+  // highest-degree-neighbour summary of the pulled structure: the entry each open
+  // row probes in the pull scan.  Built by the first traversal of a structure (2 nnz
+  // gathers of the offsets) and kept with the matrix, 4(n + 1) + n/8 bytes.
   const int fw = 1;                                   // vxm pulls over the CSC
-  const Index* first = pullFirstNeighbours(S, fw, S->d_cscColPtr_, S->d_cscRowInd_, n);
+  const Index* probe = pullMaxDegreeNeighbours(S, fw, S->d_cscColPtr_, S->d_cscRowInd_, n);
 
   const size_t nwords = (static_cast<size_t>(n) + 31)/32;
   const size_t words_bytes = ((nwords*sizeof(unsigned int) + 255)/256)*256;
@@ -74,14 +76,14 @@ Info bfsFused(Vector<float>* v, const Matrix<a>* A, Index s, Descriptor* desc, i
   BfsFusedArgs args;
   args.push_ptr = S->d_csrRowPtr_;  args.push_ind = S->d_csrColInd_;
   args.pull_ptr = S->d_cscColPtr_;  args.pull_ind = S->d_cscRowInd_;
-  args.pull_first = first;
+  args.pull_probe = probe;
   // Rows without in-neighbours may count as visited from the start only when they
   // have no out-neighbours either: a visited row is taken to have been expanded, so
   // in a directed graph one that points somewhere would let the pull discover what
   // it points at.  When the pulled structure is the pushed one, that is the same
   // bitmap; otherwise the pushed structure's empty rows are ANDed in.
   const bool same_structure = S->symmetric_ || S->d_cscColPtr_ == S->d_csrRowPtr_;
-  args.pull_empty = pullEmptyRowBits(first, n);
+  args.pull_empty = pullEmptyRowBits(probe, n);
   args.push_empty = same_structure ? NULL : pullEmptyRowBits(
       pullFirstNeighbours(S, 0, S->d_csrRowPtr_, S->d_csrColInd_, n), n);
   args.n = n;

@@ -24,16 +24,21 @@
 //     probing the visited bitmap AS OF THE LEVEL'S START (operand reuse, reference
 //     kernels/spmv.hpp:35-41), in two phases separated by a grid barrier:
 //     scan  — warps take chunks of 32 bitmap words (1024 rows) round-robin; a
-//             lane per word, fully visited words only move their bitmap words on;
-//             the open words go through the first-neighbour summary GB_BFS_BATCH
-//             at a time (all their summary loads, then all their probes, in
-//             flight together); rows whose first neighbour is not visited and
-//             that have more are written to the chunk's slice of the walk list,
-//             and a chunk with any to a list of such chunks.
+//             lane per word, fully visited words only move their bitmap words on.
+//             Every open row probes one neighbour, its highest-degree one (the
+//             one most likely to be visited; pullMaxDegreeNeighbourKernel), in
+//             batches of GB_BFS_BATCH rounds of 32 rows (all their summary loads,
+//             then all their probes, in flight together).  A dense chunk takes
+//             its open words a lane per row of the word; a sparse one takes its
+//             open rows 32 at a time, a lane per open row.  Rows whose probed
+//             neighbour is not visited and that have more entries are written to
+//             the chunk's slice of the walk list, and a chunk with any to a list
+//             of such chunks.
 //             The owner of a word writes N, the merged visited word of the other
 //             copy, the level bytes of the discovered rows and clears F.
 //     walk  — warps claim listed chunks from a counter; a lane walks its row's
-//             list GB_BFS_WALK_STEP entries per step, a list still longer than
+//             list from entry 0 (the probed entry is looked at again),
+//             GB_BFS_WALK_STEP entries per step, a list still longer than
 //             GB_BFS_WALK_WARP after the first step is walked by the whole warp,
 //             32 entries and one ballot per step.  Discoveries are ORed into N and
 //             the other visited copy.
@@ -72,7 +77,7 @@ namespace backend {
 #define GB_BFS_PUSH_MINB 2
 #endif
 #ifndef GB_BFS_BATCH
-#define GB_BFS_BATCH  4               // open words whose summaries a warp loads together
+#define GB_BFS_BATCH  4               // rounds of 32 rows whose summaries a warp loads together
 #endif
 #ifndef GB_BFS_WALK_STEP
 #define GB_BFS_WALK_STEP 4            // entries a lane requests at once walking a list
@@ -88,7 +93,8 @@ struct BfsFusedArgs {
   // structure: rows to expand when pushing, rows to inspect when pulling
   const Index* push_ptr;   const Index* push_ind;     // out-neighbours of a vertex
   const Index* pull_ptr;   const Index* pull_ind;     // in-neighbours of a vertex
-  const Index* pull_first;                            // first-neighbour summary of pull_*
+  const Index* pull_probe;                            // neighbour each pulled row probes
+                                                      // first: its highest-degree one
   const unsigned int* pull_empty;                     // bitmap of rows without in-neighbours
   const unsigned int* push_empty;                     // ... without out-neighbours; NULL
                                                       // when the structure is symmetric
@@ -193,6 +199,8 @@ bfsFusedKernel(BfsFusedArgs a) {
   namespace cg = cooperative_groups;
   cg::grid_group grid = cg::this_grid();
   __shared__ int s_red[NT/32];
+  // pull scan, per warp: the discovery words of its chunk (row path)
+  __shared__ unsigned int s_found[PULL ? NT/32 : 1][PULL ? 32 : 1];
 
   const Index n = a.n;
   const Index nwords = (n + 31) >> 5;
@@ -341,9 +349,90 @@ bfsFusedKernel(BfsFusedArgs a) {
         int nwalk = 0;                        // rows of this chunk left to walk
         unsigned int my_out = 0u;             // discoveries in this lane's word
         unsigned int open = __ballot_sync(GB_FULL_MASK, my_vis != 0xffffffffu);
+        // Row path: the chunk's open rows (rows past n are not), numbered in word
+        // order by a prefix of the per-word counts and taken 32 at a time, a lane
+        // per row; the lane of open row r finds the word holding it (binary search
+        // on the prefix) and its bit (binary search on bit counts).  Word path
+        // (below): the open words, a lane per row of the word.  A row batch costs
+        // about twice a word batch (the searches; DESIGN.md §6), so a chunk takes
+        // the row path when that needs fewer than half the batches: at RMAT-24 the
+        // second pull level (2.3 open rows per open word) takes it in nearly every
+        // chunk, the first (17) in some.
+        unsigned int my_open = ~my_vis;
+        if (word == nwords - 1 && (n & 31) != 0) my_open &= (1u << (n & 31)) - 1u;
+        const int nopen = __popc(my_open);
+        int first = nopen;                    // inclusive prefix, then exclusive
+#pragma unroll
+        for (int off = 1; off < 32; off <<= 1) {
+          const int t = __shfl_up_sync(GB_FULL_MASK, first, off);
+          if (lane >= off) first += t;
+        }
+        const int total = __shfl_sync(GB_FULL_MASK, first, 31);
+        first -= nopen;
+        const int word_batches = (__popc(open) + GB_BFS_BATCH - 1)/GB_BFS_BATCH;
+        const int row_batches = (total + 32*GB_BFS_BATCH - 1)/(32*GB_BFS_BATCH);
+        if (2*row_batches < word_batches) {
+          open = 0u;
+          unsigned int* const found_bits = s_found[threadIdx.x >> 5];
+          found_bits[lane] = 0u;
+          __syncwarp();
+          for (int r0 = 0; r0 < total; r0 += 32*GB_BFS_BATCH) {
+            // GB_BFS_BATCH rounds of 32 open rows: all summary loads, then all
+            // probes, then the decisions
+            int local[GB_BFS_BATCH];          // offset of the row in the chunk
+            Index f[GB_BFS_BATCH];
+#pragma unroll
+            for (int j = 0; j < GB_BFS_BATCH; ++j) {
+              const int r = r0 + 32*j + lane;
+              int wl = 0, base = 0;           // the last word whose prefix is <= r
+#pragma unroll
+              for (int step = 16; step > 0; step >>= 1) {
+                const int fs = __shfl_sync(GB_FULL_MASK, first, wl + step);
+                if (fs <= r) { wl += step; base = fs; }
+              }
+              unsigned int m = __shfl_sync(GB_FULL_MASK, my_open, wl);
+              int k = r - base, b = 0;        // bit of the k-th open row of the word
+#pragma unroll
+              for (int width = 16; width > 0; width >>= 1) {
+                const int lo = __popc(m & ((1u << width) - 1u));
+                if (k >= lo) { k -= lo; b += width; m >>= width; }
+              }
+              local[j] = wl*32 + b;
+              f[j] = (r < total) ? __ldg(a.pull_probe + c*GB_BFS_CHUNK + local[j])
+                                 : static_cast<Index>(-1);
+            }
+            unsigned int pword[GB_BFS_BATCH];
+#pragma unroll
+            for (int j = 0; j < GB_BFS_BATCH; ++j)
+              pword[j] = (f[j] != static_cast<Index>(-1))
+                         ? bfsVis(a, vsel)[(f[j] & 0x7fffffff) >> 5] : 0u;
+#pragma unroll
+            for (int j = 0; j < GB_BFS_BATCH; ++j) {
+              if (r0 + 32*j >= total) break;  // warp-uniform
+              const bool found = (pword[j] >> (f[j] & 31)) & 1u;
+              // the probed entry is looked at (-1: past the open rows, or a row
+              // without entries)
+              inspected += (f[j] != static_cast<Index>(-1)) ? 1 : 0;
+              // more entries and the probed one not visited: the row is walked after
+              // the scan, by whichever warp claims this chunk's slice of the list
+              const bool walk_row = f[j] >= 0 && !found;
+              const Index row = c*GB_BFS_CHUNK + local[j];
+              const unsigned int walkers = __ballot_sync(GB_FULL_MASK, walk_row);
+              if (walk_row) walk[nwalk + __popc(walkers & ((1u << lane) - 1u))] = row;
+              nwalk += __popc(walkers);
+              if (found) {
+                atomicOr(found_bits + (local[j] >> 5), 1u << (local[j] & 31));
+                bfsSetLevel(a, row, level + 1);
+                ++found_here;
+              }
+            }
+          }
+          __syncwarp();
+          my_out = found_bits[lane];
+        }
         while (open != 0u) {
-          // up to GB_BFS_BATCH open words: all first-neighbour loads, then all
-          // probes, then the decisions
+          // up to GB_BFS_BATCH open words: all summary loads, then all probes, then
+          // the decisions
           const unsigned int batch = open;
           Index f[GB_BFS_BATCH];
 #pragma unroll
@@ -354,7 +443,7 @@ bfsFusedKernel(BfsFusedArgs a) {
             if (wl >= 0) {
               const unsigned int m = __shfl_sync(GB_FULL_MASK, my_vis, wl);
               const Index row = c*GB_BFS_CHUNK + wl*32 + lane;
-              if (row < n && !((m >> lane) & 1u)) f[j] = __ldg(a.pull_first + row);
+              if (row < n && !((m >> lane) & 1u)) f[j] = __ldg(a.pull_probe + row);
             }
           }
           unsigned int pword[GB_BFS_BATCH];
@@ -366,10 +455,10 @@ bfsFusedKernel(BfsFusedArgs a) {
 #pragma unroll
           for (int j = 0; j < GB_BFS_BATCH; ++j) {
             const bool found = (pword[j] >> (f[j] & 31)) & 1u;
-            // the first entry is looked at (-1: not open, or a row without entries)
+            // the probed entry is looked at (-1: not open, or a row without entries)
             inspected += (f[j] != static_cast<Index>(-1)) ? 1 : 0;
             hit |= static_cast<unsigned int>(found) << j;
-            // more entries and the first one not visited: the row is walked after
+            // more entries and the probed one not visited: the row is walked after
             // the scan, by whichever warp claims this chunk's slice of the list
             more |= static_cast<unsigned int>(f[j] >= 0 && !found) << j;
           }
@@ -416,7 +505,9 @@ bfsFusedKernel(BfsFusedArgs a) {
           Index row = 0, k = 0, end = 0;
           if (i0 + lane < nwalk) {
             row = a.walk[c*GB_BFS_CHUNK + i0 + lane];
-            k = __ldg(a.pull_ptr + row) + 1;
+            // the walk starts at entry 0: the probed entry, wherever it is in the
+            // list, is looked at again (and counted again in inspected)
+            k = __ldg(a.pull_ptr + row);
             end = __ldg(a.pull_ptr + row + 1);
           }
           // most walks end after a few entries: every lane starts on its own list

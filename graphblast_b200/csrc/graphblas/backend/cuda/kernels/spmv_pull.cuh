@@ -408,6 +408,50 @@ __global__ void pullFirstNeighbourKernel(Index* __restrict__ first,
   }
 }
 
+// The same encoding with the neighbour most likely to be visited instead of the first:
+// probe[i] = -1 (empty row) | the entry u of row i with the longest row u
+// (rowptr[u+1] - rowptr[u]; the earliest entry on a tie) | that value with bit 31 set
+// when it is the row's only entry.  For a symmetric structure the row length is u's
+// degree; for the CSC of a directed one it is u's in-degree, how reachable u is.  A
+// warp per row, lanes striding the entries (R-MAT rows run to 10^6 entries); 2 nnz
+// gathers of rowptr, once per matrix structure.
+__global__ void pullMaxDegreeNeighbourKernel(Index* __restrict__ probe,
+                                             const Index* __restrict__ rowptr,
+                                             const Index* __restrict__ colind,
+                                             Index nrows) {
+  const int lane = threadIdx.x & 31;
+  Index i = (blockIdx.x*blockDim.x + threadIdx.x) >> 5;
+  const Index stride = (gridDim.x*blockDim.x) >> 5;
+  for (; i < nrows; i += stride) {
+    const Index beg = __ldg(rowptr + i);
+    const Index len = __ldg(rowptr + i + 1) - beg;
+    // key: row length above, the entry's position complemented below (the largest
+    // key is the longest row, earliest entry)
+    unsigned long long best = 0ull;
+    for (Index k = lane; k < len; k += 32) {
+      const Index u = __ldg(colind + beg + k);
+      const unsigned long long d =
+          static_cast<unsigned long long>(__ldg(rowptr + u + 1) - __ldg(rowptr + u));
+      const unsigned long long key = (d << 32) | (0xffffffffu - static_cast<unsigned int>(k));
+      if (key > best) best = key;
+    }
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+      const unsigned long long o = __shfl_xor_sync(GB_FULL_MASK, best, off);
+      if (o > best) best = o;
+    }
+    if (lane == 0) {
+      Index f = -1;
+      if (len > 0) {
+        const Index k = static_cast<Index>(0xffffffffu - static_cast<unsigned int>(best));
+        f = __ldg(colind + beg + k);
+        if (len == 1) f |= static_cast<Index>(0x80000000u);
+      }
+      probe[i] = f;
+    }
+  }
+}
+
 // bits[w] bit b = row 32w+b has no entry (first == -1); rows past the end read 0.
 // A traversal marks these rows visited up front: nothing can discover them, and a
 // third of an R-MAT's rows would otherwise be looked at on every pull level.

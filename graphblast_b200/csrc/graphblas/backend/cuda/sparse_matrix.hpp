@@ -168,6 +168,7 @@ class SparseMatrix {
   // rows, 1 = CSC columns), each valid for the arrays it was computed from:
   //   merge-path tile partition of the generic pull SpMV,
   //   first-neighbour summary of the Boolean pull,
+  //   highest-degree-neighbour summary of the fused BFS pull,
   //   hub index of the hub-cached pull SpMV (hub_state_: 0 not built, 1 in use,
   //   2 rejected because too few entries reference the hub columns).
   Index*       d_spmv_tiles_[2];
@@ -177,6 +178,9 @@ class SparseMatrix {
   Index*       d_pull_first_[2];
   const Index* pull_first_key_[2];
   Index        pull_first_nvals_[2];
+  Index*       d_pull_maxdeg_[2];
+  const Index* pull_maxdeg_key_[2];
+  Index        pull_maxdeg_nvals_[2];
   HubIndex     hub_[2];
   int          hub_state_[2];
 
@@ -226,6 +230,7 @@ void SparseMatrix<T>::reset(Index nrows, Index ncols) {
     d_spmv_tiles_[k] = NULL; spmv_tiles_key_[k] = NULL;
     spmv_tiles_nvals_[k] = -1; spmv_tiles_count_[k] = 0;
     d_pull_first_[k] = NULL; pull_first_key_[k] = NULL; pull_first_nvals_[k] = -1;
+    d_pull_maxdeg_[k] = NULL; pull_maxdeg_key_[k] = NULL; pull_maxdeg_nvals_[k] = -1;
     hub_state_[k] = 0;
   }
 }
@@ -237,6 +242,8 @@ void SparseMatrix<T>::dropSpmvTiles() {
     hub_state_[k] = 0;
     if (d_pull_first_[k] != NULL) gbFree(d_pull_first_[k]);
     d_pull_first_[k] = NULL; pull_first_key_[k] = NULL; pull_first_nvals_[k] = -1;
+    if (d_pull_maxdeg_[k] != NULL) gbFree(d_pull_maxdeg_[k]);
+    d_pull_maxdeg_[k] = NULL; pull_maxdeg_key_[k] = NULL; pull_maxdeg_nvals_[k] = -1;
     if (d_spmv_tiles_[k] != NULL) gbFree(d_spmv_tiles_[k]);
     d_spmv_tiles_[k] = NULL; spmv_tiles_key_[k] = NULL;
     spmv_tiles_nvals_[k] = -1; spmv_tiles_count_[k] = 0;
