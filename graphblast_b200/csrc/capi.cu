@@ -926,7 +926,8 @@ int gb200_bfs(gb200_vector_t v, gb200_matrix_t A, int source, gb200_desc_t desc,
   if (source < 0 || source >= n) return rc(graphblas::GrB_INVALID_INDEX);
   GB200_REQUIRE_DEVICE();
   graphblas::algorithm::lastStatus() = graphblas::GrB_SUCCESS;
-  float ms = graphblas::algorithm::bfs(v->f, A->f, source, &desc->desc);
+  const float ms = graphblas::algorithm::bfs(v->f, A->f, source, &desc->desc,
+                                             tight_ms != NULL);
   if (ms < 0.f) return rc(graphblas::algorithm::lastStatus());
   if (tight_ms) *tight_ms = ms;
   return 0;

@@ -23,14 +23,6 @@ inline bool bfsFusedApplies(Descriptor* desc) {
          inp1 == GrB_DEFAULT && !desc->debug() && desc->timing_ != 1;
 }
 
-__global__ void bfsAccountKernel(unsigned long long* cell,
-                                 const unsigned long long* counters, Index n) {
-  const unsigned long long bytes =
-      counters[8]*(12ull*static_cast<unsigned long long>(n) + 4ull) + 4ull*counters[7] +
-      12ull*counters[9] + 8ull*counters[10] + 8ull*counters[11];
-  atomicAdd(cell, bytes);
-}
-
 // Work counters of the last fused traversal run with this descriptor: levels,
 // entries inspected pulling, pull levels, vertices pushed, edges pushed, vertices
 // discovered pushing.  Zeros when none has run.
@@ -111,6 +103,11 @@ Info bfsFused(Vector<float>* v, const Matrix<a>* A, Index s, Descriptor* desc, i
 
   static const int trace = getEnv("GB200_BFS_TRACE", 0);
   args.trace = trace;
+  args.prof_bytes = NULL;               // the kernel adds its bytes when profiling
+  if (profiler().enabled) {
+    profiler().ensureCells();
+    args.prof_bytes = profiler().d_cells + GB_PROF_PULL_BOOL;
+  }
 
   // push-only traversals run the instantiation without the pull level, with more
   // warps per SM
@@ -133,15 +130,6 @@ Info bfsFused(Vector<float>* v, const Matrix<a>* A, Index s, Descriptor* desc, i
       dim3(resident), dim3(nt), params, 0, stream));
   GB_KERNEL_CHECK();
   profiler().end(GB_PROF_PULL_BOOL, stream, 0.0);
-  if (profiler().enabled) {
-    // algorithmic bytes of the traversal (SURVEY.md §8d), from the kernel's own
-    // work counters: per pull level 4(n+1) + 4n + 4n, 4 per inspected entry; per
-    // push 12 per frontier entry, 8 per expanded edge (colind + visited lookup),
-    // 8 per discovered vertex
-    bfsAccountKernel<<<1, 1, 0, stream>>>(profiler().d_cells + GB_PROF_PULL_BOOL,
-        args.counters, n);
-    GB_KERNEL_CHECK();
-  }
   v->dense_.touched();
   if (trace) {                           // per-level times of this traversal
     unsigned long long cells[GB_BFS_NCOUNTERS];

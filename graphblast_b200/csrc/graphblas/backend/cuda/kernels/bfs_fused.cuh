@@ -99,6 +99,8 @@ struct BfsFusedArgs {
   const unsigned int* push_empty;                     // ... without out-neighbours; NULL
                                                       // when the structure is symmetric
   int   trace;               // count the rows walked per level (GB200_BFS_TRACE)
+  unsigned long long* prof_bytes;  // profiler cell the traversal's algorithmic bytes
+                                   // are added to; NULL when profiling is off
   Index n;
   Index source;
   int   max_levels;
@@ -656,6 +658,27 @@ bfsFusedKernel(BfsFusedArgs a) {
   if (gtid == 0) {
     a.counters[6] = static_cast<unsigned long long>(level - 1);
     a.counters[8] = static_cast<unsigned long long>(pull_levels);
+  }
+  if (a.prof_bytes != NULL) {
+    // The traversal's algorithmic bytes (SURVEY.md §8d): per pull level 4(n+1) + 4n
+    // + 4n, 4 per inspected entry; per push 12 per frontier entry, 8 per expanded
+    // edge (colind + visited lookup), 8 per discovered vertex.  The sum is linear in
+    // the work counters, so every CTA adds its own share and CTA 0 the per-level
+    // terms ([11] is complete: the last level ended with a grid barrier).  A last-CTA
+    // ticket would need a device-scope fence, and with one in the kernel ptxas turns
+    // every fire-and-forget reduction (REDG) into an atomic that waits (ATOMG),
+    // the push levels' visited and next-frontier ORs included: push-only BFS
+    // 156.7-157.5 ms per launch against 149.7-150.7 (DESIGN.md §9).
+    if (pushed_edges) atomicAdd(a.prof_bytes, 8ull*pushed_edges);
+    if (threadIdx.x == 0) {
+      unsigned long long bytes = 4ull*static_cast<unsigned long long>(block_insp) +
+                                 12ull*static_cast<unsigned long long>(block_pv);
+      if (blockIdx.x == 0)
+        bytes += static_cast<unsigned long long>(pull_levels)*
+                     (12ull*static_cast<unsigned long long>(n) + 4ull) +
+                 8ull*(*reinterpret_cast<volatile unsigned long long*>(a.counters + 11));
+      if (bytes) atomicAdd(a.prof_bytes, bytes);
+    }
   }
 }
 
