@@ -52,6 +52,11 @@ SIGNATURES = [
     ("gb200_matrix_ncols", _I, [_P, _IP]),
     ("gb200_matrix_nvals", _I, [_P, _IP]),
     ("gb200_matrix_extract_csr", _I, [_P, _P, _P, _P]),
+    ("gb200_matrix_build_dense", _I, [_P, _P, _LL]),
+    ("gb200_matrix_adopt_dense", _I, [_P, _P]),
+    ("gb200_matrix_extract_dense", _I, [_P, _P, _LL]),
+    ("gb200_matrix_dense_ptr", _I, [_P, C.POINTER(_P)]),
+    ("gb200_matrix_storage", _I, [_P, _IP]),
     ("gb200_matrix_tril", _I, [_P, _P]),
     ("gb200_matrix_apply_uniform_random", _I, [_P, _P, _I, _I, _I]),
     ("gb200_host_uniform_weights", _I, [_I, _I, _I, _LL, _P]),

@@ -3,7 +3,9 @@
 mxm with a mask is the int plus-times product of triangle counting (C takes the
 mask's pattern); mxm(C, None, None, op, A, B, desc) is the unmasked sparse
 product C = A (+.x) B for FP32 matrices over any order-independent semiring and
-for INT32 matrices over PlusMultiplies.
+for INT32 matrices over PlusMultiplies.  With a sparse A and a dense FP32 B
+(Matrix.build_dense / build_dense_device) the same call is SpMM: C becomes a dense
+(nrows x ncols) matrix, read back with Matrix.extract_dense().
 
 Classes and functions keep the reference's names, argument meaning and error
 behaviour (every call returns/raises a graphblas::Info code):
@@ -450,6 +452,49 @@ class Matrix(object):
                                                   _ptr(colind), _ptr(val)),
                "Matrix extract CSR")
         return rowptr, colind[:nv], val[:nv]
+
+    def build_dense(self, values):
+        """Matrix::build(values, nvals): dense storage from a host array of shape
+        (nrows, ncols), row-major (a flat array of fewer values leaves the rest 0)."""
+        v = np.ascontiguousarray(values, dtype=np.float32)
+        if v.ndim == 2 and v.shape != (self.nrows(), self.ncols()):
+            raise ValueError("build_dense: shape %r, matrix is %d x %d" % (
+                v.shape, self.nrows(), self.ncols()))
+        _check(self._lib.gb200_matrix_build_dense(self._h, _ptr(v), v.size),
+               "Matrix::build(values)")
+
+    def build_dense_device(self, d_values):
+        """Dense storage adopting a row-major float32 DEVICE tensor of at least
+        nrows*ncols elements, read and written in place; the tensor is kept
+        alive here and stays the caller's."""
+        import torch
+        need = self.nrows()*self.ncols()
+        if d_values.dtype != torch.float32 or not d_values.is_contiguous() or \
+                d_values.numel() < need:
+            raise ValueError("build_dense_device: need a contiguous float32 tensor "
+                             "of at least %d elements" % need)
+        self._keep = [d_values]
+        _check(self._lib.gb200_matrix_adopt_dense(self._h, _dev(d_values)),
+               "Matrix adopt dense")
+
+    def extract_dense(self):
+        """Host copy of dense storage as an (nrows, ncols) float32 array."""
+        out = np.empty((self.nrows(), self.ncols()), dtype=np.float32)
+        _check(self._lib.gb200_matrix_extract_dense(self._h, _ptr(out), out.size),
+               "Matrix::extractTuples(values)")
+        return out
+
+    def dense_ptr(self):
+        out = C.c_void_p()
+        _check(self._lib.gb200_matrix_dense_ptr(self._h, C.byref(out)),
+               "Matrix dense_ptr")
+        return out.value
+
+    def getStorage(self):
+        out = C.c_int(0)
+        _check(self._lib.gb200_matrix_storage(self._h, C.byref(out)),
+               "Matrix::getStorage")
+        return Storage(out.value)
 
     def tril(self, desc):
         _check(self._lib.gb200_matrix_tril(self._h, desc._h), "tril")

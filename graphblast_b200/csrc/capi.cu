@@ -384,11 +384,11 @@ int gb200_matrix_build_coo_device(gb200_matrix_t A, const int* d_rows,
   const int mode = flags & 7;
   const bool symmetric = (flags & GB200_INGEST_SYMMETRIC_STRUCTURE) != 0;
   if (A->f) {
-    A->f->matrix_.mat_type_ = graphblas::GrB_SPARSE;
+    CHECK(A->f->matrix_.setStorage(graphblas::GrB_SPARSE));
     return rc(A->f->matrix_.sparse_.buildFromDeviceTuples(d_rows, d_cols,
         static_cast<const float*>(d_vals), ntuples, mode, symmetric));
   }
-  A->i->matrix_.mat_type_ = graphblas::GrB_SPARSE;
+  CHECK(A->i->matrix_.setStorage(graphblas::GrB_SPARSE));
   return rc(A->i->matrix_.sparse_.buildFromDeviceTuples(d_rows, d_cols,
       static_cast<const int*>(d_vals), ntuples, mode, symmetric));
 }
@@ -533,6 +533,7 @@ int gb200_matrix_nvals(gb200_matrix_t A, int* out) {
 namespace {
 template <typename T>
 Info extractCsr(graphblas::Matrix<T>* M, int* rowptr, int* colind, void* val) {
+  if (!M->matrix_.isSparse()) return graphblas::GrB_UNINITIALIZED_OBJECT;
   graphblas::backend::SparseMatrix<T>& S = M->matrix_.sparse_;
   CHECK(S.gpuToCpu());
   memcpy(rowptr, S.h_csrRowPtr_, (S.nrows_ + 1)*sizeof(int));
@@ -552,6 +553,44 @@ int gb200_matrix_extract_csr(gb200_matrix_t A, int* h_rowptr, int* h_colind,
   GB200_REQUIRE_DEVICE();
   if (A->f) return rc(extractCsr(A->f, h_rowptr, h_colind, h_val));
   return rc(extractCsr(A->i, h_rowptr, h_colind, h_val));
+}
+
+int gb200_matrix_build_dense(gb200_matrix_t A, const void* h_vals, long long nvals) {
+  if (A == NULL || (h_vals == NULL && nvals > 0)) return rc(graphblas::GrB_NULL_POINTER);
+  GB200_REQUIRE_DEVICE();
+  if (A->f == NULL) return rc(graphblas::GrB_NOT_IMPLEMENTED);
+  return rc(A->f->matrix_.buildDense(static_cast<const float*>(h_vals), nvals));
+}
+
+int gb200_matrix_adopt_dense(gb200_matrix_t A, void* d_vals) {
+  if (A == NULL || d_vals == NULL) return rc(graphblas::GrB_NULL_POINTER);
+  GB200_REQUIRE_DEVICE();
+  if (A->f == NULL) return rc(graphblas::GrB_NOT_IMPLEMENTED);
+  return rc(A->f->adoptDense(static_cast<float*>(d_vals)));
+}
+
+int gb200_matrix_extract_dense(gb200_matrix_t A, void* h_out, long long n) {
+  if (A == NULL || h_out == NULL) return rc(graphblas::GrB_NULL_POINTER);
+  GB200_REQUIRE_DEVICE();
+  if (A->f == NULL || !A->f->matrix_.isDense())
+    return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
+  return rc(A->f->matrix_.dense_.extract(static_cast<float*>(h_out), n, NULL));
+}
+
+int gb200_matrix_dense_ptr(gb200_matrix_t A, void** d_vals) {
+  if (A == NULL || d_vals == NULL) return rc(graphblas::GrB_NULL_POINTER);
+  if (A->f == NULL || !A->f->matrix_.isDense() || A->f->matrix_.dense_.d_val_ == NULL)
+    return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
+  *d_vals = A->f->matrix_.dense_.d_val_;
+  return 0;
+}
+
+int gb200_matrix_storage(gb200_matrix_t A, int* out) {
+  if (A == NULL || out == NULL) return rc(graphblas::GrB_NULL_POINTER);
+  graphblas::Storage s;
+  Info info = A->f ? A->f->getStorage(&s) : A->i->getStorage(&s);
+  *out = static_cast<int>(s);
+  return rc(info);
 }
 
 int gb200_matrix_tril(gb200_matrix_t A, gb200_desc_t desc) {
@@ -794,12 +833,15 @@ int gb200_mxm(gb200_matrix_t C, gb200_matrix_t mask, int semiring,
               gb200_matrix_t A, gb200_matrix_t B, gb200_desc_t desc) {
   if (C == NULL || A == NULL || B == NULL || desc == NULL)
     return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
-  if (mask == NULL && C->f != NULL && A->f != NULL && B->f != NULL) {
+  const bool fp32 = C->f != NULL && A->f != NULL && B->f != NULL;
+  // a float mask only reaches the backend beside a dense operand, which refuses it
+  const bool dense_operand = fp32 &&
+      (A->f->matrix_.isDense() || B->f->matrix_.isDense());
+  if (fp32 && (mask == NULL || (dense_operand && mask->f != NULL))) {
     GB200_REQUIRE_DEVICE();
     GB200_SEMIRING_DISPATCH(semiring, {
       return rc((graphblas::mxm<float, float, float, float>(C->f,
-          static_cast<graphblas::Matrix<float>*>(NULL), GrB_NULL, op, A->f, B->f,
-          &desc->desc)));
+          mask != NULL ? mask->f : NULL, GrB_NULL, op, A->f, B->f, &desc->desc)));
     });
     return 0;
   }

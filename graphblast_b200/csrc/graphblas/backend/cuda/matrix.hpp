@@ -1,5 +1,7 @@
 // graphblast_b200 backend — Matrix<T>: storage-tagged wrapper over SparseMatrix
-// (the only storage any hot-path operation uses) and the DenseMatrix placeholder.
+// and DenseMatrix (the row-major array SpMM reads and writes).  Only the storage
+// the tag names holds data: switching drops the other one, and with the sparse
+// arrays every cache derived from them (SpMV tiles, hub index, pull summaries).
 //
 // Replaces reference graphblas/backend/cuda/matrix.hpp:21-352: same method set
 // (the frontend graphblas::Matrix<T> forwards to every one of them) and the same
@@ -39,7 +41,11 @@ class Matrix {
   }
 
   Info dup(const Matrix* rhs) {
-    mat_type_ = rhs->mat_type_;
+    if (rhs->isDense()) {
+      CHECK(dense_.dup(&rhs->dense_));
+      return setStorage(GrB_DENSE);
+    }
+    CHECK(setStorage(rhs->mat_type_));
     if (isSparse()) return sparse_.dup(&rhs->sparse_);
     std::cout << "Error: Failed to call dup!\n";
     return GrB_UNINITIALIZED_OBJECT;
@@ -78,25 +84,35 @@ class Matrix {
   Info build(const std::vector<Index>* row_indices,
       const std::vector<Index>* col_indices, const std::vector<T>* values, Index nvals,
       BinaryOpT dup, char* dat_name) {
-    mat_type_ = GrB_SPARSE;
+    CHECK(setStorage(GrB_SPARSE));
     if (sparse_.nvals_ > 0) sparse_.clear();
     return sparse_.build(row_indices, col_indices, values, nvals, dup,
         dat_name);
   }
 
   Info build(char* dat_name) {
-    mat_type_ = GrB_SPARSE;
+    CHECK(setStorage(GrB_SPARSE));
     return sparse_.build(dat_name);
   }
 
+  // Dense row-major values; on a refusal the matrix is left as it was.
   Info build(const std::vector<T>* values, Index nvals) {
-    mat_type_ = GrB_DENSE;
-    return dense_.build(values, nvals);
+    CHECK(dense_.build(values, nvals));
+    return setStorage(GrB_DENSE);
+  }
+  Info buildDense(const T* h_values, long long nvals) {
+    CHECK(dense_.build(h_values, nvals));
+    return setStorage(GrB_DENSE);
+  }
+  // A caller-owned row-major device array, used in place.
+  Info adoptDense(T* d_values) {
+    CHECK(dense_.adopt(d_values));
+    return setStorage(GrB_DENSE);
   }
 
   // Device CSR pointers, adopted without ownership.
   Info build(Index* row_ptr, Index* col_ind, T* values, Index nvals) {
-    mat_type_ = GrB_SPARSE;
+    CHECK(setStorage(GrB_SPARSE));
     return sparse_.build(row_ptr, col_ind, values, nvals);
   }
 
@@ -118,6 +134,7 @@ class Matrix {
   }
 
   Info extractTuples(std::vector<T>* values, Index* n) {
+    if (isDense()) return dense_.extractTuples(values, n);
     return GrB_UNINITIALIZED_OBJECT;   // dense storage only (reference :204-209)
   }
 
@@ -155,9 +172,12 @@ class Matrix {
     return GrB_UNINITIALIZED_OBJECT;
   }
 
-  // Storage for a sparse output is sized by the operation that fills it
-  // (spgemmMasked dups the mask pattern), so nothing is allocated here.
+  // Storage for an output is sized by the operation that fills it (spgemmMasked
+  // dups the mask pattern, spmm swaps in its result), so nothing is allocated
+  // here; the storage left behind is released.
   Info setStorage(Storage mat_type) {
+    if (mat_type == GrB_SPARSE && mat_type_ != GrB_SPARSE) CHECK(dense_.clear());
+    if (mat_type == GrB_DENSE && mat_type_ != GrB_DENSE)   CHECK(sparse_.clear());
     mat_type_ = mat_type;
     return GrB_SUCCESS;
   }

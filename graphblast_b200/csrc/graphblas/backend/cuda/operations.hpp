@@ -29,6 +29,7 @@
 #include "graphblas/backend/cuda/spmv.hpp"
 #include "graphblas/backend/cuda/spmspv.hpp"
 #include "graphblas/backend/cuda/spgemm.hpp"
+#include "graphblas/backend/cuda/spmm.hpp"
 #include "graphblas/backend/cuda/ewiseadd.hpp"
 #include "graphblas/backend/cuda/ewisemult.hpp"
 #include "graphblas/backend/cuda/assign.hpp"
@@ -98,11 +99,23 @@ template <typename TC, typename TA, typename TB, typename TMask,
           typename AccumT,     typename SemiringT>
 Info mxm(Matrix<TC>* C, const Matrix<TMask>* mask, AccumT accum, SemiringT op,
     const Matrix<TA>* A, const Matrix<TB>* B, Descriptor* desc) {
-  if (!A->isSparse() || !B->isSparse()) return notBuilt("mxm with a dense operand (SpMM / GEMM)");
-  CHECK(C->setStorage(GrB_SPARSE));
-  if (mask == NULL)
-    return spgemmUnmasked(&C->sparse_, accum, op, &A->sparse_, &B->sparse_, desc);
-  return spgemmMasked(&C->sparse_, mask, accum, op, &A->sparse_, &B->sparse_, desc);
+  if (A->isSparse() && B->isDense()) {
+    if (mask != NULL) return notBuilt("masked mxm with a dense operand");
+    Desc_value inp1_mode;
+    CHECK(desc->get(GrB_INP1, &inp1_mode));
+    if (inp1_mode == GrB_TRAN) return notBuilt("mxm with a transposed dense B");
+    return spmm(C, accum, op, A, B, desc);
+  }
+  if (!A->isSparse() || !B->isSparse()) return notBuilt("mxm with a dense A (GEMM / dense x sparse)");
+  // A dense C turns sparse only once the product has replaced it: a refused
+  // product leaves it as it was.
+  const bool was_dense = C->isDense();
+  if (!was_dense) CHECK(C->setStorage(GrB_SPARSE));
+  const Info info = (mask == NULL)
+      ? spgemmUnmasked(&C->sparse_, accum, op, &A->sparse_, &B->sparse_, desc)
+      : spgemmMasked(&C->sparse_, mask, accum, op, &A->sparse_, &B->sparse_, desc);
+  if (info == GrB_SUCCESS && was_dense) CHECK(C->setStorage(GrB_SPARSE));
+  return info;
 }
 
 // Shared body of vxm / mxv once the descriptor says which side is transposed.

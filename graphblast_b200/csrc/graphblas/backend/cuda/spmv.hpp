@@ -21,6 +21,31 @@
 namespace graphblas {
 namespace backend {
 
+// Merge-path tile partition of one orientation of A (which: 0 CSR rows, 1 CSC
+// columns; rowptr and nrows of that orientation): tiles of GB_SPMV_TILE rows +
+// entries, computed on the device once per structure and cached on A.  The pull
+// SpMV and the SpMM share it.  Returns the tile count.
+template <typename a>
+int mergeTiles(SparseMatrix<a>* A, int which, const Index* rowptr, Index nrows) {
+  const long long merge_total = static_cast<long long>(nrows) + A->nvals_;
+  const int ntiles = static_cast<int>((merge_total + GB_SPMV_TILE - 1)/GB_SPMV_TILE);
+  if (A->d_spmv_tiles_[which] == NULL ||
+      A->spmv_tiles_key_[which] != rowptr ||
+      A->spmv_tiles_nvals_[which] != A->nvals_ ||
+      A->spmv_tiles_count_[which] != ntiles) {
+    if (A->d_spmv_tiles_[which] != NULL) gbFree(A->d_spmv_tiles_[which]);
+    A->d_spmv_tiles_[which] = reinterpret_cast<Index*>(
+        gbMalloc((static_cast<size_t>(ntiles) + 1)*sizeof(Index)));
+    spmvMergePartitionKernel<<<(ntiles + 256)/256, 256, 0, gbStream()>>>(
+        A->d_spmv_tiles_[which], rowptr, nrows, A->nvals_, ntiles, GB_SPMV_TILE);
+    GB_KERNEL_CHECK();
+    A->spmv_tiles_key_[which]   = rowptr;
+    A->spmv_tiles_nvals_[which] = A->nvals_;
+    A->spmv_tiles_count_[which] = ntiles;
+  }
+  return ntiles;
+}
+
 // Generic SpMV into `out` (raw result, no mask/accum).  2 launches (+1 the first
 // time a matrix is used, to compute its tile partition).
 template <typename W, typename a, typename U, typename SemiringT>
@@ -253,27 +278,9 @@ Info spmv(DenseVector<W>* w, const Vector<M>* mask, BinaryOpT accum, SemiringT o
     else
       w_val = w->d_val_;
 
-    // Tile partition of this structure, computed once per matrix.
     SparseMatrix<a>* A_t = const_cast<SparseMatrix<a>*>(A);
     const int which = use_tran ? 1 : 0;
-    const long long merge_total = static_cast<long long>(A_nrows) + A->nvals_;
-    const int ntiles = static_cast<int>((merge_total + GB_SPMV_TILE - 1)/
-        GB_SPMV_TILE);
-    if (A_t->d_spmv_tiles_[which] == NULL ||
-        A_t->spmv_tiles_key_[which] != A_csrRowPtr ||
-        A_t->spmv_tiles_nvals_[which] != A->nvals_ ||
-        A_t->spmv_tiles_count_[which] != ntiles) {
-      if (A_t->d_spmv_tiles_[which] != NULL) gbFree(A_t->d_spmv_tiles_[which]);
-      A_t->d_spmv_tiles_[which] = reinterpret_cast<Index*>(
-          gbMalloc((static_cast<size_t>(ntiles) + 1)*sizeof(Index)));
-      spmvMergePartitionKernel<<<(ntiles + 256)/256, 256, 0, s>>>(
-          A_t->d_spmv_tiles_[which], A_csrRowPtr, A_nrows, A->nvals_, ntiles,
-          GB_SPMV_TILE);
-      GB_KERNEL_CHECK();
-      A_t->spmv_tiles_key_[which]   = A_csrRowPtr;
-      A_t->spmv_tiles_nvals_[which] = A->nvals_;
-      A_t->spmv_tiles_count_[which] = ntiles;
-    }
+    mergeTiles(A_t, which, A_csrRowPtr, A_nrows);
     // Large matrices whose entries mostly reference a few columns (power-law
     // graphs) take the hub-cached kernel (kernels/spmv_hub.cuh): hub columns are
     // served from shared memory, the rest as before.  The per-matrix index is

@@ -40,7 +40,8 @@
 #define GB_PROF_PULL_BOOL  1
 #define GB_PROF_PUSH       2
 #define GB_PROF_SPGEMM     3
-#define GB_PROF_NKINDS     4
+#define GB_PROF_SPMM       4
+#define GB_PROF_NKINDS     5
 
 namespace graphblas {
 namespace backend {

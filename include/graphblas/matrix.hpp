@@ -46,7 +46,13 @@ class Matrix {
       return m.build(row_indices, col_indices, values, nvals, dup, dat_name);
     }, row_indices, col_indices, values);
   }
-  Info build(const std::vector<T>* values, Index nvals) { return matrix_.build(values, nvals); }
+  Info build(const std::vector<T>* values, Index nvals) {
+    return given([&](Impl& m) { return m.build(values, nvals); }, values);
+  }
+  // Dense row-major DEVICE values (nrows*ncols), adopted without ownership.
+  Info adoptDense(T* d_values) {
+    return given([&](Impl& m) { return m.adoptDense(d_values); }, d_values);
+  }
   // DEVICE CSR arrays: row_ptr (nrows+1), col_ind (nvals), values (nvals).
   Info build(Index* d_row_ptr, Index* d_col_ind, T* d_values, Index nvals) {
     return given([&](Impl& m) {

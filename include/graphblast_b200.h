@@ -151,9 +151,28 @@ int gb200_matrix_nrows(gb200_matrix_t A, int* out);                 /* :104-108 
 int gb200_matrix_ncols(gb200_matrix_t A, int* out);                 /* :111-115 */
 int gb200_matrix_nvals(gb200_matrix_t A, int* out);                 /* :118-122 */
 /* Host copy of the CSR (what the reference CPU verifiers read,
- * algorithm/bfs.hpp:101-107).  Buffers: nrows+1, nvals, nvals. */
+ * algorithm/bfs.hpp:101-107).  Buffers: nrows+1, nvals, nvals.
+ * GrB_UNINITIALIZED_OBJECT when A holds dense storage. */
 int gb200_matrix_extract_csr(gb200_matrix_t A, int* h_rowptr, int* h_colind,
                              void* h_val);
+/* ---- Dense matrices (FP32 only; INT32 answers GrB_NOT_IMPLEMENTED) -----------
+ * A dense matrix holds nrows x ncols values, row-major, every entry present
+ * (nvals = nrows * ncols); more than INT32_MAX elements is GrB_OUT_OF_MEMORY.
+ * Giving A dense storage drops its sparse arrays, and the reverse.
+ * Matrix::build(values, nvals) (reference :147-150): HOST values; more than
+ * nrows*ncols is GrB_DIMENSION_MISMATCH, fewer leave the rest 0. */
+int gb200_matrix_build_dense(gb200_matrix_t A, const void* h_vals, long long nvals);
+/* Adopts a caller-owned DEVICE array of nrows*ncols values, read and written in
+ * place (any 4-byte alignment; 16-byte alignment takes the vector loads). */
+int gb200_matrix_adopt_dense(gb200_matrix_t A, void* d_vals);
+/* extractTuples(values, n) (reference dense_matrix.hpp): the first min(n, nvals)
+ * values; n > nvals gives GrB_UNINITIALIZED_OBJECT, n < nvals
+ * GrB_INSUFFICIENT_SPACE.  GrB_UNINITIALIZED_OBJECT on sparse storage. */
+int gb200_matrix_extract_dense(gb200_matrix_t A, void* h_out, long long n);
+/* Device address of the dense values (valid while the storage is dense). */
+int gb200_matrix_dense_ptr(gb200_matrix_t A, void** d_vals);
+/* getStorage: GB200_SPARSE, GB200_DENSE or GB200_UNKNOWN. */
+int gb200_matrix_storage(gb200_matrix_t A, int* out);
 /* tril(A, A) under GrB_BACKEND = GrB_SEQUENTIAL (operations.hpp:872-886,
  * example/gtc.cu:80-82). */
 int gb200_matrix_tril(gb200_matrix_t A, gb200_desc_t desc);
@@ -207,7 +226,14 @@ int gb200_mxv(gb200_vector_t w, gb200_vector_t mask, int use_accum, int semiring
  * every semiring except the four whose add is not associative (GreaterPlus,
  * CustomLessPlus, NotEqualToPlus, CustomLessLess: GrB_NOT_IMPLEMENTED); INT32
  * C/A/B over PlusMultiplies only; mixed element types give GrB_DOMAIN_MISMATCH.
- * GrB_OUT_OF_MEMORY, with C unchanged, when nnz(C) would exceed INT32_MAX. */
+ * GrB_OUT_OF_MEMORY, with C unchanged, when nnz(C) would exceed INT32_MAX.
+ * Sparse A, dense FP32 B (SpMM): C becomes dense, m x N, every entry the fold of
+ * A(i,k) * B(k,j) over the stored entries of row i of op(A) from the semiring's
+ * identity; GrB_INP0 = GrB_TRAN reads A's CSC (GrB_UNINITIALIZED_OBJECT without
+ * one); C may be A or B.  Same semirings as above; GrB_OUT_OF_MEMORY, checked
+ * before anything is allocated and with C unchanged, when m*N > INT32_MAX.
+ * GrB_NOT_IMPLEMENTED, with C unchanged: a mask beside a dense operand, a dense A,
+ * GrB_INP1 = GrB_TRAN on a dense B. */
 int gb200_mxm(gb200_matrix_t C, gb200_matrix_t mask, int semiring,
               gb200_matrix_t A, gb200_matrix_t B, gb200_desc_t desc);      /* mxm :22-49 */
 int gb200_ewise_add(gb200_vector_t w, gb200_vector_t mask, int semiring,
@@ -273,7 +299,8 @@ int gb200_vector_import_bits(gb200_vector_t v, const uint32_t* d_bits, long long
 
 /* ---- Measurement hooks (bench.py; no reference counterpart) --------------- */
 /* Hot-kernel kinds: 0 merge-path SpMV (pull, generic semiring), 1 fused Boolean
- * pull, 2 push (SpMSpV expand), 3 masked SpGEMM.  When enabled every launch of
+ * pull, 2 push (SpMSpV expand), 3 masked SpGEMM, 4 SpMM (bytes: 4(m+1) + 8 nnz +
+ * 4 k N + 4 m N).  When enabled every launch of
  * those kernels is bracketed by CUDA events on the launching stream. */
 int gb200_profile_enable(int on);
 int gb200_profile_reset(void);
