@@ -186,8 +186,10 @@ __device__ __forceinline__ void atomicCombine(T* addr, T val, AddOp add_op) {
 // the semiring's add answers for add(3, 5) — the reference's own way of telling
 // monoids apart (spmv.hpp:76-85): 3 = minimum, 5 = maximum, 8 = plus.  For float
 // cells those three map to one native atomic (ordered-int trick for min/max:
-// non-negative floats order like signed ints, negative floats like reversed
-// unsigned ints); everything else takes the CAS loop.
+// floats with a clear sign bit order like signed ints, floats with the sign bit
+// set like reversed unsigned ints); everything else takes the CAS loop.  The
+// branch goes by the sign bit, not by `>= 0`: -0.0 compares equal to 0 but is
+// INT_MIN as a signed int, so atomicMin(int) would overwrite a negative cell.
 template <typename T, typename AddOp>
 __device__ __forceinline__ T atomicCombineFetch(T* addr, T val, AddOp add_op,
                                                 int kind) {
@@ -200,7 +202,8 @@ __device__ __forceinline__ T atomicCombineFetch(T* addr, T val, AddOp add_op,
     if (kind == 8) {
       old = atomicAdd(fa, fv);
     } else {
-      const bool as_signed = (kind == 3) ? (fv >= 0.f) : (fv < 0.f);
+      const bool neg = (__float_as_uint(fv) >> 31) != 0u;
+      const bool as_signed = (kind == 3) ? !neg : neg;
       if (kind == 3) {
         old = as_signed
             ? __int_as_float(atomicMin(reinterpret_cast<int*>(fa),

@@ -268,6 +268,17 @@ Info spmv(DenseVector<W>* w, const Vector<M>* mask, BinaryOpT accum, SemiringT o
       return GrB_UNINITIALIZED_OBJECT;
     }
   } else {
+    // Refuse a sparse mask before anything is written: without accum the SpMV
+    // writes straight into w.
+    if (use_mask) {
+      Storage mask_vec_type;
+      CHECK(mask->getStorage(&mask_vec_type));
+      if (mask_vec_type != GrB_DENSE) {
+        std::cout << "Spmv generic semiring with sparse mask\n";
+        std::cout << "Error: Feature not implemented yet!\n";
+        return GrB_NOT_IMPLEMENTED;
+      }
+    }
     CHECK(u_t->materialize());
     if (use_mask) CHECK(mask->materialize());
     if (use_accum) CHECK(w->materialize());
@@ -320,13 +331,6 @@ Info spmv(DenseVector<W>* w, const Vector<M>* mask, BinaryOpT accum, SemiringT o
         A_csrVal, u_t->d_val_, A_nrows, A->nvals_, desc));
 
     if (use_mask) {
-      Storage mask_vec_type;
-      CHECK(mask->getStorage(&mask_vec_type));
-      if (mask_vec_type != GrB_DENSE) {
-        std::cout << "Spmv generic semiring with sparse mask\n";
-        std::cout << "Error: Feature not implemented yet!\n";
-        return GrB_NOT_IMPLEMENTED;
-      }
       const int grid = gridFor(A_nrows, 256);
       // GrB_SCMP keeps entries whose mask is zero: overwrite where mask != 0.
       if (use_scmp)
