@@ -141,11 +141,12 @@ Info bfsFused(Vector<float>* v, const Matrix<a>* A, Index s, Descriptor* desc, i
             1e-3*static_cast<double>((cells[12] >> 1) - cells[28]));
     for (int l = 1; l <= levels; ++l) {
       const unsigned long long start = cells[12 + l - 1] >> 1, end = cells[12 + l] >> 1;
-      if (cells[12 + l] & 1ull)          // pull: scan, walk, rows walked
-        fprintf(stderr, " L%d pull %.1fus (scan %.1f walk %.1f, %llu walked)", l,
-                1e-3*static_cast<double>(end - start),
+      if (cells[12 + l] & 1ull)          // pull: scan, walk, rows walked, chunks listed
+        fprintf(stderr, " L%d pull %.1fus (scan %.1f walk %.1f, %llu walked, %llu listed)",
+                l, 1e-3*static_cast<double>(end - start),
                 1e-3*static_cast<double>(cells[44 + l] - start),
-                1e-3*static_cast<double>(end - cells[44 + l]), cells[60 + l]);
+                1e-3*static_cast<double>(end - cells[44 + l]), cells[60 + l],
+                cells[76 + l]);
       else
         fprintf(stderr, " L%d push %.1fus", l, 1e-3*static_cast<double>(end - start));
     }

@@ -32,16 +32,18 @@
 //             its open words a lane per row of the word; a sparse one takes its
 //             open rows 32 at a time, a lane per open row.  Rows whose probed
 //             neighbour is not visited and that have more entries are written to
-//             the chunk's slice of the walk list, and a chunk with any to a list
-//             of such chunks.
+//             the chunk's slice of the walk list.  A chunk with at most
+//             GB_BFS_WALK_INLINE of them is walked right there by the warp that
+//             scanned it (bfsWalkRows), discoveries going into the chunk's words;
+//             a chunk with more goes to a list of such chunks.
 //             The owner of a word writes N, the merged visited word of the other
 //             copy, the level bytes of the discovered rows and clears F.
-//     walk  — warps claim listed chunks from a counter; a lane walks its row's
-//             list from entry 0 (the probed entry is looked at again),
-//             GB_BFS_WALK_STEP entries per step, a list still longer than
-//             GB_BFS_WALK_WARP after the first step is walked by the whole warp,
-//             32 entries and one ballot per step.  Discoveries are ORed into N and
-//             the other visited copy.
+//     walk  — warps claim listed chunks from a counter and walk their rows by the
+//             same rules; discoveries are ORed into N and the other visited copy.
+//   The walk (bfsWalkRows): a lane walks its row's list from entry 0 (the probed
+//   entry is looked at again), GB_BFS_WALK_STEP entries per step, a list still
+//   longer than GB_BFS_WALK_WARP after the first step is walked by the whole warp,
+//   32 entries and one ballot per step.
 //   v is written once per row, after the last level, in one pass of full-line
 //   stores: the level byte of every reached row, 0 for the others (and, when
 //   max_levels cuts the traversal off, for the rows found at the last level: only
@@ -85,6 +87,9 @@ namespace backend {
 #ifndef GB_BFS_WALK_WARP
 #define GB_BFS_WALK_WARP 32           // list remainder longer than this: walked by a warp
 #endif
+#ifndef GB_BFS_WALK_INLINE
+#define GB_BFS_WALK_INLINE 64         // chunk with at most this many rows to walk: walked
+#endif                                // by the warp that scanned it (DESIGN.md §4.5)
 #define GB_BFS_HEAVY  2048            // adjacency longer than this: grid-wide expansion
 #define GB_BFS_HEAVY_CAP 4096         // heavy vertices per level kept in the list
 #define GB_BFS_CHUNK  1024            // rows of a pull chunk (32 bitmap words)
@@ -127,7 +132,8 @@ struct BfsFusedArgs {
                                   // levels, [38..40] chunks listed in walk_chunks
                                   // (both rotating like [0..2]),
                                   // [44..59] time at the scan barrier of every pull
-                                  // level, [60..75] rows it left to walk; [12..] and
+                                  // level, [60..75] rows it left to walk (inline and
+                                  // listed), [76..91] chunks it listed; [12..] and
                                   // [44..] for GB200_BFS_TRACE (GB_BFS_NCOUNTERS cells)
   Index*        heavy;            // [GB_BFS_HEAVY_CAP]
   Index*        walk;             // [nchunks * GB_BFS_CHUNK] rows to walk, by chunk
@@ -191,6 +197,67 @@ __device__ __forceinline__ unsigned int* bfsN(const BfsFusedArgs& a, int fsel) {
 // as visited from the start and are unreached unless one is the source.
 __device__ __forceinline__ unsigned int bfsIsolated(const BfsFusedArgs& a, Index w) {
   return a.pull_empty[w] & (a.push_empty != NULL ? a.push_empty[w] : 0xffffffffu);
+}
+
+// The pull walk of one row per lane (warp-collective; a lane without a row passes
+// active = false).  True when the row has an entry visited as of the level's start.
+// The scan's inline walk and the grid-wide walk both come here, so the rules and the
+// count of inspected entries are the same whichever walks a row.  The list is walked
+// from entry 0: the probed entry, wherever it is in the list, is looked at again (and
+// counted again in inspected).  It reads only visited[vsel], which no thread writes
+// during a pull level, so it sees the same bits during the scan as after it.
+__device__ __forceinline__ bool bfsWalkRows(const BfsFusedArgs& a, int vsel, Index row,
+                                            bool active, int lane, int& inspected) {
+  Index k = 0, end = 0;
+  if (active) {
+    k = __ldg(a.pull_ptr + row);
+    end = __ldg(a.pull_ptr + row + 1);
+  }
+  // most walks end after a few entries: every lane starts on its own list
+  const Index stop = (end - k > GB_BFS_WALK_WARP + GB_BFS_WALK_STEP)
+                     ? k + GB_BFS_WALK_STEP : end;
+  bool found = false;
+  // GB_BFS_WALK_STEP entries per step: their bitmap words are fetched together, then
+  // examined in list order (the count stops at the first visited one)
+  while (k < stop && !found) {
+    Index col[GB_BFS_WALK_STEP];
+    unsigned int wv[GB_BFS_WALK_STEP];
+#pragma unroll
+    for (int u = 0; u < GB_BFS_WALK_STEP; ++u)
+      col[u] = (k + u < stop) ? __ldg(a.pull_ind + k + u) : static_cast<Index>(-1);
+#pragma unroll
+    for (int u = 0; u < GB_BFS_WALK_STEP; ++u)
+      wv[u] = (col[u] >= 0) ? bfsVis(a, vsel)[col[u] >> 5] : 0u;
+#pragma unroll
+    for (int u = 0; u < GB_BFS_WALK_STEP; ++u) {
+      if (found || col[u] < 0) continue;
+      ++inspected;
+      found = (wv[u] >> (col[u] & 31)) & 1u;
+    }
+    k += GB_BFS_WALK_STEP;
+  }
+  // a list with more than GB_BFS_WALK_WARP entries left: the whole warp walks it,
+  // 32 entries and one ballot per step
+  unsigned int longs = __ballot_sync(GB_FULL_MASK, !found && k < end);
+  while (longs != 0u) {
+    const int src = __ffs(longs) - 1;
+    longs &= longs - 1u;
+    const Index lend = __shfl_sync(GB_FULL_MASK, end, src);
+    bool hit = false;
+    for (Index lk = __shfl_sync(GB_FULL_MASK, k, src); lk < lend && !hit; lk += 32) {
+      bool v = false;
+      if (lk + lane < lend) {
+        const Index col = __ldg(a.pull_ind + lk + lane);
+        v = (bfsVis(a, vsel)[col >> 5] >> (col & 31)) & 1u;
+      }
+      const unsigned int b = __ballot_sync(GB_FULL_MASK, v);
+      hit = (b != 0u);
+      if (lane == 0)
+        inspected += hit ? __ffs(b) : (lend - lk < 32 ? lend - lk : 32);
+    }
+    if (lane == src) found = hit;
+  }
+  return found;
 }
 
 // NT x MINB: the CTA shape; PULL = false compiles the pull level out (push-only
@@ -415,8 +482,8 @@ bfsFusedKernel(BfsFusedArgs a) {
               // the probed entry is looked at (-1: past the open rows, or a row
               // without entries)
               inspected += (f[j] != static_cast<Index>(-1)) ? 1 : 0;
-              // more entries and the probed one not visited: the row is walked after
-              // the scan, by whichever warp claims this chunk's slice of the list
+              // more entries and the probed one not visited: the row goes into the
+              // chunk's slice of the walk list
               const bool walk_row = f[j] >= 0 && !found;
               const Index row = c*GB_BFS_CHUNK + local[j];
               const unsigned int walkers = __ballot_sync(GB_FULL_MASK, walk_row);
@@ -460,8 +527,8 @@ bfsFusedKernel(BfsFusedArgs a) {
             // the probed entry is looked at (-1: not open, or a row without entries)
             inspected += (f[j] != static_cast<Index>(-1)) ? 1 : 0;
             hit |= static_cast<unsigned int>(found) << j;
-            // more entries and the probed one not visited: the row is walked after
-            // the scan, by whichever warp claims this chunk's slice of the list
+            // more entries and the probed one not visited: the row goes into the
+            // chunk's slice of the walk list
             more |= static_cast<unsigned int>(f[j] >= 0 && !found) << j;
           }
           unsigned int rest = batch;
@@ -479,83 +546,64 @@ bfsFusedKernel(BfsFusedArgs a) {
             if (lane == wl) my_out = out;
           }
         }
+        if (nwalk > 0 && nwalk <= GB_BFS_WALK_INLINE) {
+          // A light chunk's rows are walked here, by this warp, instead of after the
+          // barrier: at RMAT-24 the first pull level leaves at most a few dozen
+          // short rows per chunk, and listing them for the grid costs more than
+          // walking them (DESIGN.md §4.5).  The rows are the ones the lanes just
+          // stored in the chunk's slice of a.walk; the __syncwarp orders those
+          // stores for the warp.  Discoveries are ORed into the chunk's shared words
+          // (seeded with the scan's) and go out with the owners' stores below, so
+          // no global atomics.  The walk reads visited[vsel] only, which no thread
+          // writes during a pull level: it finds what the walk after the barrier
+          // would, and counts the same entries.
+          unsigned int* const found_bits = s_found[threadIdx.x >> 5];
+          found_bits[lane] = my_out;
+          __syncwarp();
+          for (int i0 = 0; i0 < nwalk; i0 += 32) {
+            const bool active = i0 + lane < nwalk;
+            const Index row = active ? walk[i0 + lane] : 0;
+            if (bfsWalkRows(a, vsel, row, active, lane, inspected)) {
+              const int local = row & (GB_BFS_CHUNK - 1);
+              atomicOr(found_bits + (local >> 5), 1u << (local & 31));
+              bfsSetLevel(a, row, level + 1);
+              ++found_here;
+            }
+          }
+          __syncwarp();
+          my_out = found_bits[lane];
+        }
         if (word < nwords) {
           bfsN(a, fsel)[word] = my_out;
           bfsVisOther(a, vsel)[word] = my_vis | my_out;
           bfsF(a, fsel)[word] = 0u;
         }
         if (lane == 0 && nwalk > 0) {
-          a.walk_count[c] = nwalk;
-          a.walk_chunks[atomicAdd(list_cell, 1ull)] = c;
+          if (nwalk > GB_BFS_WALK_INLINE) {
+            a.walk_count[c] = nwalk;
+            a.walk_chunks[atomicAdd(list_cell, 1ull)] = c;
+          }
           if (a.trace && level < 16)
             atomicAdd(a.counters + 60 + level, static_cast<unsigned long long>(nwalk));
         }
         c = c_next;
       }
       grid.sync();
-      if (gtid == 0 && level < 16) a.counters[44 + level] = bfsClockNs();
-      // walk: the chunks with rows to walk, claimed from a counter, a lane per row;
-      // a list with more than GB_BFS_WALK_WARP entries left after the lane has
-      // looked at GB_BFS_WALK_STEP of them is walked by the whole warp
       const Index nlisted = static_cast<Index>(
           *reinterpret_cast<volatile unsigned long long*>(list_cell));
+      if (gtid == 0 && level < 16) {
+        a.counters[44 + level] = bfsClockNs();
+        if (a.trace) a.counters[76 + level] = static_cast<unsigned long long>(nlisted);
+      }
+      // walk: the heavy chunks' rows, chunks claimed from a counter, a lane per row
       for (Index i = gwarp; i < nlisted; ) {
         const Index i_next = gwarps + bfsClaimChunk(walk_cell, lane);
         const Index c = a.walk_chunks[i];
         const int nwalk = a.walk_count[c];
         for (int i0 = 0; i0 < nwalk; i0 += 32) {
-          Index row = 0, k = 0, end = 0;
-          if (i0 + lane < nwalk) {
-            row = a.walk[c*GB_BFS_CHUNK + i0 + lane];
-            // the walk starts at entry 0: the probed entry, wherever it is in the
-            // list, is looked at again (and counted again in inspected)
-            k = __ldg(a.pull_ptr + row);
-            end = __ldg(a.pull_ptr + row + 1);
-          }
-          // most walks end after a few entries: every lane starts on its own list
-          const Index stop = (end - k > GB_BFS_WALK_WARP + GB_BFS_WALK_STEP)
-                             ? k + GB_BFS_WALK_STEP : end;
-          bool found = false;
-          // GB_BFS_WALK_STEP entries per step: their bitmap words are fetched
-          // together, then examined in list order (the count stops at the first
-          // visited one)
-          while (k < stop && !found) {
-            Index col[GB_BFS_WALK_STEP];
-            unsigned int wv[GB_BFS_WALK_STEP];
-#pragma unroll
-            for (int u = 0; u < GB_BFS_WALK_STEP; ++u)
-              col[u] = (k + u < stop) ? __ldg(a.pull_ind + k + u) : static_cast<Index>(-1);
-#pragma unroll
-            for (int u = 0; u < GB_BFS_WALK_STEP; ++u)
-              wv[u] = (col[u] >= 0) ? bfsVis(a, vsel)[col[u] >> 5] : 0u;
-#pragma unroll
-            for (int u = 0; u < GB_BFS_WALK_STEP; ++u) {
-              if (found || col[u] < 0) continue;
-              ++inspected;
-              found = (wv[u] >> (col[u] & 31)) & 1u;
-            }
-            k += GB_BFS_WALK_STEP;
-          }
-          unsigned int longs = __ballot_sync(GB_FULL_MASK, !found && k < end);
-          while (longs != 0u) {
-            const int src = __ffs(longs) - 1;
-            longs &= longs - 1u;
-            const Index lend = __shfl_sync(GB_FULL_MASK, end, src);
-            bool hit = false;
-            for (Index lk = __shfl_sync(GB_FULL_MASK, k, src); lk < lend && !hit; lk += 32) {
-              bool v = false;
-              if (lk + lane < lend) {
-                const Index col = __ldg(a.pull_ind + lk + lane);
-                v = (bfsVis(a, vsel)[col >> 5] >> (col & 31)) & 1u;
-              }
-              const unsigned int b = __ballot_sync(GB_FULL_MASK, v);
-              hit = (b != 0u);
-              if (lane == 0)
-                inspected += hit ? __ffs(b) : (lend - lk < 32 ? lend - lk : 32);
-            }
-            if (lane == src) found = hit;
-          }
-          if (found) {
+          const bool active = i0 + lane < nwalk;
+          const Index row = active ? a.walk[c*GB_BFS_CHUNK + i0 + lane] : 0;
+          if (bfsWalkRows(a, vsel, row, active, lane, inspected)) {
             const unsigned int bit = 1u << (row & 31);
             atomicOr(bfsN(a, fsel) + (row >> 5), bit);
             atomicOr(bfsVisOther(a, vsel) + (row >> 5), bit);

@@ -10,9 +10,13 @@ smallest-id neighbour) and `maxdeg` (the neighbour with the longest row, earlies
 entry on a tie: the one the fused kernel probes).  It also gives entries_inspected_pulling as
 the kernel counts it under `maxdeg`: one per probed open row, plus, per walked row,
 its entries from entry 0 up to and including the first visited one (all of them
-when none is).
+when none is).  Per pull level it gives the walk's shape: rows to walk per chunk of
+1024 rows (p50, p99, max), the entries those walks inspect, and the chunks and rows
+above GB_BFS_WALK_INLINE, which the kernel lists and walks grid-wide after the scan
+instead of in the warp that scanned them.
 
     python tools/bfs_pull_model.py [--scale 24] [--seed 1] [--mxvmode 0]
+                                   [--walk-inline 64]
 
 uses the oracle's R-MAT (tests/oracle_binding.py, symmetric) and the highest-degree
 vertex as the source, as bench.py does.
@@ -24,6 +28,7 @@ import sys
 import numpy as np
 
 BLOCK = 1 << 21          # rows per block of the entry-wise passes (bounds memory)
+WALK_INLINE = 64         # GB_BFS_WALK_INLINE: a chunk with more rows to walk is listed
 
 
 def probe_summary(rp, ci, rule, lengths=None):
@@ -79,12 +84,14 @@ def has_visited_neighbour(rp, ci, rows, visited):
     return first_visited(rp, ci, rows, visited) < (rp[rows + 1] - rp[rows])
 
 
-def replay(rp, ci, source, mode=0, switchpoint=0.01, isolated=None, probes=None):
+def replay(rp, ci, source, mode=0, switchpoint=0.01, isolated=None, probes=None,
+           walk_inline=WALK_INLINE):
     """Level loop of the fused kernel on the pulled structure (rp, ci): row i's
     entries are the vertices it is discovered from.  isolated: rows visited from
     the start (default: the empty rows, as for a symmetric structure).  probes:
-    {name: probe array}.  Returns a list of per-pull-iteration dicts and the total
-    entries inspected pulling for each probe summary."""
+    {name: probe array}.  walk_inline: the kernel's GB_BFS_WALK_INLINE.  Returns a
+    list of per-pull-iteration dicts and the total entries inspected pulling for
+    each probe summary."""
     n = len(rp) - 1
     lens = np.diff(rp).astype(np.int64)
     if isolated is None:
@@ -136,8 +143,24 @@ def replay(rp, ci, source, mode=0, switchpoint=0.01, isolated=None, probes=None)
                 if name == "maxdeg":
                     fv = first_visited(rp, ci, open_rows[walk], visited)
                     wl = lens[open_rows[walk]]
-                    inspected[name] += int(nonempty.sum()) + int(
-                        np.where(fv < wl, fv + 1, wl).sum())
+                    walked = np.where(fv < wl, fv + 1, wl)
+                    inspected[name] += int(nonempty.sum()) + int(walked.sum())
+                    # the walk's split: chunks with at most walk_inline rows to
+                    # walk are walked inline by the warp that scanned them, the
+                    # others listed and walked grid-wide after the barrier
+                    per_chunk = np.bincount(open_rows[walk] >> 10)
+                    per_chunk = per_chunk[per_chunk > 0]
+                    heavy = per_chunk > walk_inline
+                    it["walk_counts"] = per_chunk
+                    it["walk_chunks"] = len(per_chunk)
+                    it["walk_per_chunk"] = (
+                        tuple(int(np.percentile(per_chunk, q, method="lower"))
+                              for q in (50, 99)) + (int(per_chunk.max()),)
+                        if len(per_chunk) else (0, 0, 0))
+                    it["walk_entries"] = int(walked.sum())
+                    it["walk_entries_row_max"] = int(walked.max()) if len(wl) else 0
+                    it["listed_chunks"] = int(heavy.sum())
+                    it["listed_rows"] = int(per_chunk[heavy].sum())
             iters.append(it)
         visited[new] = True
         fcount = len(new)
@@ -152,6 +175,8 @@ def main():
     ap.add_argument("--seed", type=int, default=1)
     ap.add_argument("--mxvmode", type=int, default=0, choices=[0, 2])
     ap.add_argument("--switchpoint", type=float, default=0.01)
+    ap.add_argument("--walk-inline", type=int, default=WALK_INLINE,
+                    help="rows to walk per chunk above which a chunk is listed")
     args = ap.parse_args()
     sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)),
                                     "..", "tests"))
@@ -159,7 +184,8 @@ def main():
     rp, ci = orc.rmat_csr(args.scale, args.edgefactor, args.seed)
     rp = rp.astype(np.int64)
     source = int(np.argmax(np.diff(rp)))
-    iters, inspected = replay(rp, ci, source, args.mxvmode, np.float32(args.switchpoint))
+    iters, inspected = replay(rp, ci, source, args.mxvmode, np.float32(args.switchpoint),
+                              walk_inline=args.walk_inline)
     print("R-MAT-%d, edge factor %d, seed %d, source %d, mxvmode %d"
           % (args.scale, args.edgefactor, args.seed, source, args.mxvmode))
     print("%-5s %10s %10s %24s %24s" % ("level", "open rows", "open words",
@@ -174,6 +200,14 @@ def main():
     for it in iters:
         print("L%d scan batches: word path %d, row path %d, chosen per chunk %d" % (
             it["level"], it["batches_word"], it["batches_row"], it["batches_chosen"]))
+    for it in iters:
+        p50, p99, top = it["walk_per_chunk"]
+        print("L%d walk (maxdeg): %d rows in %d chunks, per chunk p50 %d p99 %d max %d; "
+              "%d entries inspected, at most %d per row; above %d per chunk: "
+              "%d chunks, %d rows" % (
+                  it["level"], it["walked_maxdeg"], it["walk_chunks"], p50, p99, top,
+                  it["walk_entries"], it["walk_entries_row_max"], args.walk_inline,
+                  it["listed_chunks"], it["listed_rows"]))
     print("entries inspected pulling (maxdeg probe, walk from entry 0): %d"
           % inspected["maxdeg"])
 
