@@ -6,8 +6,11 @@
 // Semantics follow reference graphblas/backend/cuda/scatter.hpp:11-138,
 // gather.hpp:11-52 and their kernels (kernels/scatter.hpp:8-50, gather.hpp:9-35),
 // including their guards: scatter skips targets <= 0 (kernels/scatter.hpp:16),
-// the indexed forms skip targets outside [0, size of w).  Where several sources
-// name the same target, which one lands is unspecified there and here.
+// assignScatter skips targets outside [0, size of w), and extractGather skips
+// sources outside [0, length of u), leaving w[i] as it was.  The frontend refuses
+// more indices than the vector indexed by position i (u for assignScatter, w for
+// extractGather) holds.  Where several sources name the same target, which one
+// lands is unspecified there and here.
 // Grid-stride kernels on the backend stream instead of <<<n/nt, nt>>> on stream 0.
 #ifndef GRAPHBLAS_BACKEND_CUDA_INDEXED_HPP_
 #define GRAPHBLAS_BACKEND_CUDA_INDEXED_HPP_
@@ -116,10 +119,12 @@ Info indexedMove(Vector<W>* w, const Vector<M>* mask, const Vector<U>* u,
   CHECK(w->materialize());
   Index w_size;
   CHECK(w->dense_.nvals(&w_size));
+  // the gather reads u's value array: its sources are bounded by that array
+  const Index u_len = (u_type == GrB_DENSE) ? u->dense_.nvals_ : u->sparse_.nvals_;
   if (nindices > 0) {
     const int grid = gridFor(nindices, 256);
     if (Gather)
-      gatherByIndexKernel<<<grid, 256, 0, gbStream()>>>(w->dense_.d_val_, w_size,
+      gatherByIndexKernel<<<grid, 256, 0, gbStream()>>>(w->dense_.d_val_, u_len,
           storedValues(ind, u_type), storedValues(u, u_type), nindices);
     else
       scatterByIndexKernel<<<grid, 256, 0, gbStream()>>>(w->dense_.d_val_, w_size,

@@ -38,7 +38,9 @@ ssspRelaxKernel(T* __restrict__ dist, T* __restrict__ relaxed, Index n, T inf,
 }
 
 // PageRank, after contrib = rank_before (+.*) A:
-//   rank = contrib + jump ; partials = sum((rank - rank_before)^2)
+//   rank = contrib + jump ; partials = sum(diff^2), where diff is what the dense
+//   eWiseMult PlusMinus of the separate route gives: rank - rank_before, or its
+//   identity 0 where either rank is 0 (ewiseMultDenseKernel)
 template <typename T>
 __global__ void __launch_bounds__(GB_REDUCE_NT)
 prUpdateKernel(T* __restrict__ rank, const T* __restrict__ contrib,
@@ -50,8 +52,10 @@ prUpdateKernel(T* __restrict__ rank, const T* __restrict__ contrib,
   PlusMonoid<T> add;
   T acc = static_cast<T>(0);
   for (; i < n; i += stride) {
-    const T now  = contrib[i] + jump;
-    const T diff = now - rank_before[i];
+    const T now    = contrib[i] + jump;
+    const T before = rank_before[i];
+    const T diff   = (now == static_cast<T>(0) || before == static_cast<T>(0))
+                         ? static_cast<T>(0) : now - before;
     rank[i] = now;
     // the separate operations round the square before it is added: no fma here
     const T square = static_cast<T>(__fmul_rn(static_cast<float>(diff),

@@ -54,6 +54,12 @@ template <typename T> Extent sizeOf(const Vector<T>* v) {
   if (e.known) v->size(&e.n);
   return e;
 }
+// stored entries of a vector: the count the index-driven operations run over
+template <typename T> Extent nvalsOf(const Vector<T>* v) {
+  Extent e = {0, v != NULL};
+  if (e.known) v->nvals(&e.n);
+  return e;
+}
 // A shape contract: relations are added one by one, the first one that fails is
 // reported (with the reference's wording) and remembered.
 class Contract {
@@ -61,6 +67,13 @@ class Contract {
   Contract() : verdict_(GrB_SUCCESS) {}
   Contract& equal(Extent lhs, Extent rhs, const char* broken) {
     if (verdict_ == GrB_SUCCESS && lhs.known && rhs.known && lhs.n != rhs.n) {
+      std::cout << broken << std::endl;
+      verdict_ = GrB_DIMENSION_MISMATCH;
+    }
+    return *this;
+  }
+  Contract& atMost(Extent lhs, Extent rhs, const char* broken) {
+    if (verdict_ == GrB_SUCCESS && lhs.known && rhs.known && lhs.n > rhs.n) {
       std::cout << broken << std::endl;
       verdict_ = GrB_DIMENSION_MISMATCH;
     }
@@ -251,6 +264,7 @@ Info eWiseAdd(Vector<TW>* w, const Vector<TMask>* mask, AccumT accum, SemiringT 
   GB_REQUIRE(w, u, v, desc);
   GB_SHAPES(Contract()
       .equal(sizeOf(u), sizeOf(v), "u.size != v.size")
+      .equal(sizeOf(u), sizeOf(w), "u.size != w.size")
       .equal(sizeOf(u), sizeOf(mask), "u.size != mask.size")
       .equal(sizeOf(v), sizeOf(mask), "v.size != mask.size")
       .equal(sizeOf(w), sizeOf(mask), "w.size != mask.size"));
@@ -309,6 +323,9 @@ Info reduce(Vector<TW>* w, const Vector<TMask>* mask, AccumT accum, MonoidT op,
             const Matrix<TA>* A, Descriptor* desc) {
   using namespace ops_detail;
   GB_REQUIRE(w, A, desc);
+  GB_SHAPES(Contract()
+      .equal(rowsOf(A), sizeOf(w), "A.nrows != w.size")
+      .equal(sizeOf(w), sizeOf(mask), "w.size  != mask.size"));
   return backend::reduce(raw(w), raw(mask), accum, op, raw(A), raw(desc));
 }
 
@@ -381,7 +398,9 @@ Info assignScatter(Vector<TW>* w, const Vector<TMask>* mask, AccumT accum,
                    const Vector<TU>* u, const Vector<TIndex>* indices, Descriptor* desc) {
   using namespace ops_detail;
   GB_REQUIRE(w, u, indices, desc);
-  GB_SHAPES(Contract().equal(sizeOf(w), sizeOf(mask), "w.size  != mask.size"));
+  GB_SHAPES(Contract()
+      .equal(sizeOf(w), sizeOf(mask), "w.size  != mask.size")
+      .atMost(nvalsOf(indices), sizeOf(u), "indices.nvals > u.size"));
   return backend::assignScatter(raw(w), raw(mask), accum, raw(u), raw(indices), raw(desc));
 }
 
@@ -391,6 +410,9 @@ Info extractGather(Vector<TW>* w, const Vector<TMask>* mask, AccumT accum,
                    const Vector<TU>* u, const Vector<TIndex>* indices, Descriptor* desc) {
   using namespace ops_detail;
   GB_REQUIRE(u, w, indices, desc);
+  GB_SHAPES(Contract()
+      .equal(sizeOf(w), sizeOf(mask), "w.size  != mask.size")
+      .atMost(nvalsOf(indices), sizeOf(w), "indices.nvals > w.size"));
   return backend::extractGather(raw(w), raw(mask), accum, raw(u), raw(indices), raw(desc));
 }
 
