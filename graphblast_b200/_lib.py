@@ -86,6 +86,9 @@ SIGNATURES = [
     ("gb200_ewise_add", _I, [_P, _P, _I, _P, _P, _P]),
     ("gb200_ewise_add_scalar", _I, [_P, _P, _I, _P, _D, _P]),
     ("gb200_ewise_mult", _I, [_P, _P, _I, _P, _P, _P]),
+    ("gb200_ewise_add_matrix", _I, [_P, _P, _I, _P, _P, _P]),
+    ("gb200_ewise_mult_matrix", _I, [_P, _P, _I, _P, _P, _P]),
+    ("gb200_transpose", _I, [_P, _P, _P, _P]),
     ("gb200_assign_scalar", _I, [_P, _P, _D, _P]),
     ("gb200_reduce_vector", _I, [C.POINTER(_D), _I, _P, _P]),
     ("gb200_reduce_matrix", _I, [C.POINTER(_D), _I, _P, _P]),

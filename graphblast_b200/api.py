@@ -3,7 +3,10 @@
 mxm with a mask is the int plus-times product of triangle counting (C takes the
 mask's pattern); mxm(C, None, None, op, A, B, desc) is the unmasked sparse
 product C = A (+.x) B for FP32 matrices over any order-independent semiring and
-for INT32 matrices over PlusMultiplies.  With a sparse A and a dense FP32 B
+for INT32 matrices over PlusMultiplies.  eWiseAdd / eWiseMult with Matrix
+operands are the union / intersection of two sparse matrices (FP32 over every
+semiring, INT32 over PlusMultiplies), and transpose(C, None, None, A, desc) gives
+C = A'.  With a sparse A and a dense FP32 B
 (Matrix.build_dense / build_dense_device) the same call is SpMM: C becomes a dense
 (nrows x ncols) matrix, read back with Matrix.extract_dense().
 
@@ -13,8 +16,8 @@ behaviour (every call returns/raises a graphblas::Info code):
   Descriptor   reference graphblas/descriptor.hpp:17-62
   Vector       reference graphblas/vector.hpp:13-264
   Matrix       reference graphblas/matrix.hpp:14-252
-  vxm/mxv/mxm/eWiseAdd/eWiseMult/assign/reduce
-               reference graphblas/operations.hpp:22-49,59-127,137-158,277-353,509-530,620-673
+  vxm/mxv/mxm/eWiseAdd/eWiseMult/transpose/assign/reduce
+               reference graphblas/operations.hpp:22-49,59-127,137-158,277-353,682-688,509-530,620-673
 
 All compute goes through the C ABI (include/graphblast_b200.h); there is no
 Python or CPU implementation of any operation here.
@@ -542,8 +545,13 @@ def mxm(C_, mask, accum, op, A, B, desc):
 
 
 def eWiseAdd(w, mask, accum, op, u, v, desc):
+    """w = u + v.  With Matrix operands: the union of the two patterns, add(a, b)
+    where both hold an entry, the one value where one does; C is replaced."""
     lib = _lib.load()
-    if isinstance(v, Vector):
+    if isinstance(w, Matrix):
+        _check(lib.gb200_ewise_add_matrix(w._h, _h(mask), int(op), u._h, v._h,
+                                          desc._h), "eWiseAdd(matrix)")
+    elif isinstance(v, Vector):
         _check(lib.gb200_ewise_add(w._h, _h(mask), int(op), u._h, v._h,
                                    desc._h), "eWiseAdd")
     else:
@@ -553,8 +561,22 @@ def eWiseAdd(w, mask, accum, op, u, v, desc):
 
 
 def eWiseMult(w, mask, accum, op, u, v, desc):
-    _check(_lib.load().gb200_ewise_mult(w._h, _h(mask), int(op), u._h, v._h,
-                                        desc._h), "eWiseMult")
+    """w = u .* v.  With Matrix operands: the intersection of the two patterns,
+    mul(a, b); C is replaced."""
+    lib = _lib.load()
+    if isinstance(w, Matrix):
+        _check(lib.gb200_ewise_mult_matrix(w._h, _h(mask), int(op), u._h, v._h,
+                                           desc._h), "eWiseMult(matrix)")
+    else:
+        _check(lib.gb200_ewise_mult(w._h, _h(mask), int(op), u._h, v._h,
+                                    desc._h), "eWiseMult")
+
+
+def transpose(C_, mask, accum, A, desc):
+    """C = A' (C = A when GrB_INP0 is GrB_TRAN); C may be A.  accum is not
+    applied."""
+    _check(_lib.load().gb200_transpose(C_._h, _h(mask), A._h, desc._h),
+           "transpose")
 
 
 def assign(w, mask, accum, val, indices, nindices, desc):

@@ -146,6 +146,37 @@ inline bool cudaOk() {
 
 graphblas::Vector<float>* vec(gb200_vector_t v) { return v ? v->f : NULL; }
 
+// C = A (+) B (IsAdd) or A (x) B of two matrices: FP32 over every semiring,
+// INT32 over PlusMultiplies only, no mixing.
+template <bool IsAdd>
+int ewiseMatrix(gb200_matrix_t C, gb200_matrix_t mask, int semiring, gb200_matrix_t A,
+                gb200_matrix_t B, gb200_desc_t desc) {
+  if (C == NULL || A == NULL || B == NULL || desc == NULL)
+    return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
+  if (C->f != NULL && A->f != NULL && B->f != NULL && (mask == NULL || mask->f != NULL)) {
+    GB200_REQUIRE_DEVICE();
+    GB200_SEMIRING_DISPATCH(semiring, {
+      if constexpr (IsAdd)
+        return rc((graphblas::eWiseAdd<float, float, float, float>(C->f,
+            mask != NULL ? mask->f : NULL, GrB_NULL, op, A->f, B->f, &desc->desc)));
+      else
+        return rc((graphblas::eWiseMult<float, float, float, float>(C->f,
+            mask != NULL ? mask->f : NULL, GrB_NULL, op, A->f, B->f, &desc->desc)));
+    });
+    return 0;
+  }
+  if (C->i == NULL || A->i == NULL || B->i == NULL || (mask != NULL && mask->i == NULL))
+    return rc(graphblas::GrB_DOMAIN_MISMATCH);
+  if (semiring != GB200_PLUS_MULTIPLIES) return rc(graphblas::GrB_NOT_IMPLEMENTED);
+  GB200_REQUIRE_DEVICE();
+  if constexpr (IsAdd)
+    return rc((graphblas::eWiseAdd<int, int, int, int>(C->i, mask ? mask->i : NULL,
+        GrB_NULL, graphblas::PlusMultipliesSemiring<int>(), A->i, B->i, &desc->desc)));
+  else
+    return rc((graphblas::eWiseMult<int, int, int, int>(C->i, mask ? mask->i : NULL,
+        GrB_NULL, graphblas::PlusMultipliesSemiring<int>(), A->i, B->i, &desc->desc)));
+}
+
 }  // namespace
 
 extern "C" {
@@ -854,6 +885,32 @@ int gb200_mxm(gb200_matrix_t C, gb200_matrix_t mask, int semiring,
   return rc((graphblas::mxm<int, int, int, int>(C->i, mask ? mask->i : NULL,
       GrB_NULL, graphblas::PlusMultipliesSemiring<int>(), A->i, B->i,
       &desc->desc)));
+}
+
+int gb200_ewise_add_matrix(gb200_matrix_t C, gb200_matrix_t mask, int semiring,
+                           gb200_matrix_t A, gb200_matrix_t B, gb200_desc_t desc) {
+  return ewiseMatrix<true>(C, mask, semiring, A, B, desc);
+}
+
+int gb200_ewise_mult_matrix(gb200_matrix_t C, gb200_matrix_t mask, int semiring,
+                            gb200_matrix_t A, gb200_matrix_t B, gb200_desc_t desc) {
+  return ewiseMatrix<false>(C, mask, semiring, A, B, desc);
+}
+
+int gb200_transpose(gb200_matrix_t C, gb200_matrix_t mask, gb200_matrix_t A,
+                    gb200_desc_t desc) {
+  if (C == NULL || A == NULL || desc == NULL)
+    return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
+  if (C->f != NULL && A->f != NULL && (mask == NULL || mask->f != NULL)) {
+    GB200_REQUIRE_DEVICE();
+    return rc((graphblas::transpose<float, float, float>(C->f,
+        mask != NULL ? mask->f : NULL, GrB_NULL, A->f, &desc->desc)));
+  }
+  if (C->i == NULL || A->i == NULL || (mask != NULL && mask->i == NULL))
+    return rc(graphblas::GrB_DOMAIN_MISMATCH);
+  GB200_REQUIRE_DEVICE();
+  return rc((graphblas::transpose<int, int, int>(C->i, mask ? mask->i : NULL, GrB_NULL,
+      A->i, &desc->desc)));
 }
 
 int gb200_ewise_add(gb200_vector_t w, gb200_vector_t mask, int semiring,

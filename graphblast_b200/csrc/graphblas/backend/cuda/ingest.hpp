@@ -33,14 +33,13 @@ inline int ingestBitsFor(Index extent) {        // bits that hold 0 .. extent-1
 
 // ---- scan / sort drivers -------------------------------------------------------
 
-// In-place exclusive scan of n ints; returns the grand total (one host read).
-inline unsigned long long scanExclusiveInPlace(int* data, long long n) {
-  if (n <= 0) return 0ull;
+// In-place exclusive scan of n ints, stream-ordered, no host read; *grand (device,
+// may be NULL) receives the total.
+inline void scanExclusiveAsync(int* data, long long n, unsigned long long* grand) {
+  if (n <= 0) return;
   cudaStream_t s = gbStream();
   const int ntiles = static_cast<int>((n + GB_SCAN_TILE - 1)/GB_SCAN_TILE);
   int* totals = reinterpret_cast<int*>(gbMalloc((static_cast<size_t>(ntiles) + 1)*sizeof(int)));
-  unsigned long long* grand = reinterpret_cast<unsigned long long*>(
-      gbMalloc(sizeof(unsigned long long)));
   scanTileKernel<<<ntiles, GB_SCAN_NT, 0, s>>>(data, totals, n);
   GB_KERNEL_CHECK();
   scanTotalsKernel<<<1, GB_SCAN_NT, 0, s>>>(totals, ntiles, grand);
@@ -49,9 +48,17 @@ inline unsigned long long scanExclusiveInPlace(int* data, long long n) {
     scanAddKernel<<<ntiles, GB_SCAN_NT, 0, s>>>(data, totals, n);
     GB_KERNEL_CHECK();
   }
+  gbFree(totals);
+}
+
+// In-place exclusive scan of n ints; returns the grand total (one host read).
+inline unsigned long long scanExclusiveInPlace(int* data, long long n) {
+  if (n <= 0) return 0ull;
+  unsigned long long* grand = reinterpret_cast<unsigned long long*>(
+      gbMalloc(sizeof(unsigned long long)));
+  scanExclusiveAsync(data, n, grand);
   const unsigned long long total = runtime().fetch(grand);
   gbFree(grand);
-  gbFree(totals);
   return total;
 }
 

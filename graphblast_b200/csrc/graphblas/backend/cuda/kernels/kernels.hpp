@@ -13,6 +13,7 @@
 #include "graphblas/backend/cuda/kernels/spgemm_masked.cuh"
 #include "graphblas/backend/cuda/kernels/spgemm_hash.cuh"
 #include "graphblas/backend/cuda/kernels/spgemm_unmasked.cuh"
+#include "graphblas/backend/cuda/kernels/ewise_matrix.cuh"
 #include "graphblas/backend/cuda/kernels/spmm.cuh"
 
 #endif  // GRAPHBLAS_BACKEND_CUDA_KERNELS_KERNELS_HPP_

@@ -32,6 +32,7 @@
 #include "graphblas/backend/cuda/spmm.hpp"
 #include "graphblas/backend/cuda/ewiseadd.hpp"
 #include "graphblas/backend/cuda/ewisemult.hpp"
+#include "graphblas/backend/cuda/ewise_matrix.hpp"
 #include "graphblas/backend/cuda/assign.hpp"
 #include "graphblas/backend/cuda/reduce.hpp"
 #include "graphblas/backend/cuda/apply.hpp"
@@ -89,7 +90,6 @@ Info settle(const Vector<X>* x, Rest... rest) {
 
 GB_DECLARED_ONLY(extract,           "extract of a vector")
 GB_DECLARED_ONLY(assignIndexed,     "assignIndexed")
-GB_DECLARED_ONLY(transpose,         "transpose")
 GB_DECLARED_ONLY(traceMxmTranspose, "traceMxmTranspose")
 GB_DECLARED_ONLY(graphColor,        "graphColor (cuSPARSE csrcolor, gone from CUDA 12)")
 GB_DECLARED_ONLY(applyVxm,          "applyVxm")
@@ -114,6 +114,24 @@ Info mxm(Matrix<TC>* C, const Matrix<TMask>* mask, AccumT accum, SemiringT op,
   const Info info = (mask == NULL)
       ? spgemmUnmasked(&C->sparse_, accum, op, &A->sparse_, &B->sparse_, desc)
       : spgemmMasked(&C->sparse_, mask, accum, op, &A->sparse_, &B->sparse_, desc);
+  if (info == GrB_SUCCESS && was_dense) CHECK(C->setStorage(GrB_SPARSE));
+  return info;
+}
+
+// C = op(A) (+) op(B) (IsAdd: union) or op(A) (x) op(B) (intersection) of two
+// sparse matrices (ewise_matrix.hpp).  The refusals come before anything changes;
+// a dense C turns sparse only once the result has replaced it.
+template <bool IsAdd, typename TC, typename TA, typename TB, typename TMask,
+          typename SemiringT>
+Info ewiseMatrixDispatch(Matrix<TC>* C, const Matrix<TMask>* mask, SemiringT op,
+    const Matrix<TA>* A, const Matrix<TB>* B, Descriptor* desc) {
+  if (mask != NULL)
+    return notBuilt(IsAdd ? "masked eWiseAdd of two matrices" : "masked eWiseMult of two matrices");
+  if (!A->isSparse() || !B->isSparse())
+    return notBuilt(IsAdd ? "eWiseAdd with a dense matrix" : "eWiseMult with a dense matrix");
+  const bool was_dense = C->isDense();
+  if (!was_dense) CHECK(C->setStorage(GrB_SPARSE));
+  const Info info = ewiseMatrix<IsAdd>(&C->sparse_, op, &A->sparse_, &B->sparse_, desc);
   if (info == GrB_SUCCESS && was_dense) CHECK(C->setStorage(GrB_SPARSE));
   return info;
 }
@@ -263,7 +281,7 @@ template <typename TC, typename TA, typename TB, typename TMask,
           typename AccumT,     typename SemiringT>
 Info eWiseMult(Matrix<TC>* C, const Matrix<TMask>* mask, AccumT accum, SemiringT op,
     const Matrix<TA>* A, const Matrix<TB>* B, Descriptor* desc) {
-  return notBuilt("eWiseMult of two matrices");
+  return ewiseMatrixDispatch<false>(C, mask, op, A, B, desc);
 }
 
 // Extension: matrix (x) broadcast scalar
@@ -348,7 +366,22 @@ template <typename TC, typename TA, typename TB, typename TMask,
           typename AccumT,     typename SemiringT>
 Info eWiseAdd(Matrix<TC>* C, const Matrix<TMask>* mask, AccumT accum, SemiringT op,
     const Matrix<TA>* A, const Matrix<TB>* B, Descriptor* desc) {
-  return notBuilt("eWiseAdd of two matrices");
+  return ewiseMatrixDispatch<true>(C, mask, op, A, B, desc);
+}
+
+// C = Aᵀ (C = A when GrB_INP0 is GrB_TRAN); C may be A.
+template <typename TC, typename TMask, typename TA, typename AccumT>
+Info transpose(Matrix<TC>* C, const Matrix<TMask>* mask, AccumT accum,
+    const Matrix<TA>* A, Descriptor* desc) {
+  if (mask != NULL) return notBuilt("masked transpose");
+  if (!A->isSparse()) return notBuilt("transpose of a dense matrix");
+  Desc_value inp0_mode;
+  CHECK(desc->get(GrB_INP0, &inp0_mode));
+  const bool was_dense = C->isDense();
+  if (!was_dense) CHECK(C->setStorage(GrB_SPARSE));
+  const Info info = transposeSparse(&C->sparse_, &A->sparse_, inp0_mode == GrB_TRAN);
+  if (info == GrB_SUCCESS && was_dense) CHECK(C->setStorage(GrB_SPARSE));
+  return info;
 }
 
 // Extension: vector (+) broadcast scalar

@@ -97,6 +97,23 @@ template <typename T> const backend::Matrix<T>* raw(const Matrix<T>* m) { return
 template <typename T> backend::Matrix<T>*       raw(Matrix<T>* m)       { return m ? &m->matrix_ : NULL; }
 inline backend::Descriptor*                     raw(Descriptor* d)      { return d ? &d->descriptor_ : NULL; }
 
+// Shapes of an element-wise operation on two matrices: op(A), op(B) and C alike,
+// op(X) being Xᵀ when GrB_INP0 / GrB_INP1 is GrB_TRAN.
+template <typename TC, typename TMask, typename TA, typename TB>
+Contract ewiseShapes(const Matrix<TC>* C, const Matrix<TMask>* mask, const Matrix<TA>* A,
+                     const Matrix<TB>* B, Descriptor* desc) {
+  Desc_value inp0 = GrB_DEFAULT, inp1 = GrB_DEFAULT;
+  desc->get(GrB_INP0, &inp0);
+  desc->get(GrB_INP1, &inp1);
+  const bool ta = inp0 == GrB_TRAN, tb = inp1 == GrB_TRAN;
+  return Contract()
+      .equal(ta ? colsOf(A) : rowsOf(A), rowsOf(C), "op(A).nrows != C.nrows")
+      .equal(ta ? rowsOf(A) : colsOf(A), colsOf(C), "op(A).ncols != C.ncols")
+      .equal(tb ? colsOf(B) : rowsOf(B), rowsOf(C), "op(B).nrows != C.nrows")
+      .equal(tb ? rowsOf(B) : colsOf(B), colsOf(C), "op(B).ncols != C.ncols")
+      .alike(C, mask, "C.nrows != mask.nrows", "C.ncols != mask.ncols");
+}
+
 inline Info declaredOnly(const char* what) {
   std::cout << "Error: " << what << " not implemented yet!\n";
   return GrB_NOT_IMPLEMENTED;
@@ -214,17 +231,15 @@ Info eWiseMult(Vector<TW>* w, const Vector<TMask>* mask, AccumT accum, SemiringT
   return backend::eWiseMult(raw(w), raw(mask), accum, op, raw(u), raw(v), raw(desc));
 }
 
-// C<mask> = accum(C, A .* B)
+// C<mask> = accum(C, op(A) .* op(B)), op what GrB_INP0 / GrB_INP1 name: the
+// shapes compared are those of the transposes
 template <typename TC, typename TMask, typename TA, typename TB, typename AccumT,
           typename SemiringT>
 Info eWiseMult(Matrix<TC>* C, const Matrix<TMask>* mask, AccumT accum, SemiringT op,
                const Matrix<TA>* A, const Matrix<TB>* B, Descriptor* desc) {
   using namespace ops_detail;
   GB_REQUIRE(C, A, B, desc);
-  GB_SHAPES(Contract()
-      .alike(B, A, "B.nrows != A.nrows", "B.ncols != A.ncols")
-      .alike(A, C, "A.nrows != C.nrows", "A.ncols != C.ncols")
-      .alike(C, mask, "C.nrows != mask.nrows", "C.ncols != mask.ncols"));
+  GB_SHAPES(ewiseShapes(C, mask, A, B, desc));
   return backend::eWiseMult(raw(C), raw(mask), accum, op, raw(A), raw(B), raw(desc));
 }
 
@@ -284,11 +299,32 @@ Info eWiseAdd(Vector<TW>* w, const Vector<TMask>* mask, AccumT accum, SemiringT 
   return backend::eWiseAdd(raw(w), raw(mask), accum, op, raw(u), val, raw(desc));
 }
 
+// C<mask> = accum(C, op(A) + op(B)), shapes as in the matrix eWiseMult
 template <typename TC, typename TMask, typename TA, typename TB, typename AccumT,
           typename SemiringT>
 Info eWiseAdd(Matrix<TC>* C, const Matrix<TMask>* mask, AccumT accum, SemiringT op,
               const Matrix<TA>* A, const Matrix<TB>* B, Descriptor* desc) {
-  return ops_detail::declaredOnly("eWiseAdd matrix variant");
+  using namespace ops_detail;
+  GB_REQUIRE(C, A, B, desc);
+  GB_SHAPES(ewiseShapes(C, mask, A, B, desc));
+  return backend::eWiseAdd(raw(C), raw(mask), accum, op, raw(A), raw(B), raw(desc));
+}
+
+// C<mask> = accum(C, Aᵀ); C = A when GrB_INP0 is GrB_TRAN (the transpose of the
+// transposed input)
+template <typename TC, typename TMask, typename TA, typename AccumT>
+Info transpose(Matrix<TC>* C, const Matrix<TMask>* mask, AccumT accum, const Matrix<TA>* A,
+               Descriptor* desc) {
+  using namespace ops_detail;
+  GB_REQUIRE(C, A, desc);
+  Desc_value inp0;
+  CHECK(desc->get(GrB_INP0, &inp0));
+  const bool ta = inp0 == GrB_TRAN;
+  GB_SHAPES(Contract()
+      .equal(ta ? rowsOf(A) : colsOf(A), rowsOf(C), "C.nrows != A.ncols")
+      .equal(ta ? colsOf(A) : rowsOf(A), colsOf(C), "C.ncols != A.nrows")
+      .alike(C, mask, "C.nrows != mask.nrows", "C.ncols != mask.ncols"));
+  return backend::transpose(raw(C), raw(mask), accum, raw(A), raw(desc));
 }
 
 // ---- apply, reduce, tril -----------------------------------------------------------------
@@ -458,11 +494,6 @@ Info assign(Matrix<TC>* C, const Matrix<TMask>* mask, AccumT accum, TScalar val,
             const std::vector<Index>* row_indices, Index nrows,
             const std::vector<Index>* col_indices, Index ncols, Descriptor* desc) {
   return ops_detail::declaredOnly("assign matrix variant");
-}
-template <typename TC, typename TMask, typename TA, typename AccumT>
-Info transpose(Matrix<TC>* C, const Matrix<TMask>* mask, AccumT accum, const Matrix<TA>* A,
-               Descriptor* desc) {
-  return ops_detail::declaredOnly("transpose");
 }
 template <typename TB, typename TA, typename TScalar, typename MonoidT>
 Info scale(Matrix<TB>* B, MonoidT op, const Matrix<TA>* A, TScalar val, Descriptor* desc) {

@@ -236,6 +236,30 @@ int gb200_mxv(gb200_vector_t w, gb200_vector_t mask, int use_accum, int semiring
  * GrB_INP1 = GrB_TRAN on a dense B. */
 int gb200_mxm(gb200_matrix_t C, gb200_matrix_t mask, int semiring,
               gb200_matrix_t A, gb200_matrix_t B, gb200_desc_t desc);      /* mxm :22-49 */
+/* Element-wise operations on two sparse matrices, C = op(A) (+) op(B) and
+ * C = op(A) (x) op(B), op(X) = X or, with GrB_INP0 / GrB_INP1 = GrB_TRAN, X' (read
+ * from X's CSC).  op(A), op(B) and C have one shape (else GrB_DIMENSION_MISMATCH).
+ * add: the union of the two patterns; where both hold an entry C(i,j) =
+ *   add(a, b), the semiring's ADD with A's value first; where one does, C takes
+ *   that value unchanged (no identity; unlike the vector eWiseAdd, C is sparse).
+ * mult: the intersection, C(i,j) = mul(a, b), the semiring's MUL, A's value first.
+ * C is replaced (accum is not applied) by a sorted CSR, with its CSC in the
+ * default format; stored zeros and results equal to 0 or NaN stay stored.  C may
+ * be A, B or both.  FP32 C/A/B over every semiring; INT32 C/A/B over
+ * PlusMultiplies only; mixed element types give GrB_DOMAIN_MISMATCH.  These leave
+ * C unchanged: a mask or a dense A or B (GrB_NOT_IMPLEMENTED), a transposed operand
+ * without a CSC (GrB_UNINITIALIZED_OBJECT), nnz(C) > INT32_MAX
+ * (GrB_OUT_OF_MEMORY). */
+int gb200_ewise_add_matrix(gb200_matrix_t C, gb200_matrix_t mask, int semiring,
+                           gb200_matrix_t A, gb200_matrix_t B, gb200_desc_t desc);
+int gb200_ewise_mult_matrix(gb200_matrix_t C, gb200_matrix_t mask, int semiring,
+                            gb200_matrix_t A, gb200_matrix_t B, gb200_desc_t desc);
+/* C = A' (C = A with GrB_INP0 = GrB_TRAN), C of the transposed shape (else
+ * GrB_DIMENSION_MISMATCH).  C's CSR is a copy of A's CSC, or built from A's CSR
+ * when A has none; C's CSC, in the default format, is a copy of A's CSR.  C may be
+ * A.  A mask gives GrB_NOT_IMPLEMENTED; C and A of one element type. */
+int gb200_transpose(gb200_matrix_t C, gb200_matrix_t mask, gb200_matrix_t A,
+                    gb200_desc_t desc);
 int gb200_ewise_add(gb200_vector_t w, gb200_vector_t mask, int semiring,
                     gb200_vector_t u, gb200_vector_t v, gb200_desc_t desc); /* :277-299 */
 int gb200_ewise_add_scalar(gb200_vector_t w, gb200_vector_t mask, int semiring,
