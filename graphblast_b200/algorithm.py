@@ -1,8 +1,9 @@
 """graphblas::algorithm — the GraphBLAS algorithm drivers of the reference
 (graphblas/algorithm/{bfs,sssp,pr,tc}.hpp), executed inside the native library as
-loops of backend operations (include/graphblas/algorithm/*.hpp).
+loops of backend operations (include/graphblas/algorithm/*.hpp), and the graph
+colouring gc, one kernel on the device.
 
-sssp, pr and tc return the device time of the operation loop in milliseconds
+sssp, pr, tc and gc return the device time of the operation loop in milliseconds
 ("tight" in the reference drivers, example/gbfs.cu:110-115).  bfs returns it only
 when called with timed=True; otherwise it returns None and, when the traversal runs
 as the fused kernel, only enqueues it, so that back-to-back traversals keep the GPU
@@ -51,3 +52,15 @@ def tc(A, B, desc):
     _check(_lib.load().gb200_tc(C.byref(n), A._h, B._h, desc._h, C.byref(ms)),
            "algorithm::tc")
     return n.value, ms.value
+
+
+def gc(v, A, seed, desc):
+    """v[i] = colour of vertex i (1-based) in the undirected graph of A's pattern:
+    greedy first-fit colouring in decreasing priority (hash(seed, i), i) order, one
+    cooperative kernel (include/graphblas/algorithm/gc.hpp).  A is FP32 or INT32; a
+    non-symmetric A needs its CSC.  Returns (ncolors, tight_ms)."""
+    ms = C.c_float(0)
+    k = C.c_int(0)
+    _check(_lib.load().gb200_gc(v._h, A._h, int(seed), desc._h, C.byref(k), C.byref(ms)),
+           "algorithm::gc")
+    return k.value, ms.value

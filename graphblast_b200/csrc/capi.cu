@@ -24,6 +24,7 @@
 #include "graphblas/algorithm/sssp.hpp"
 #include "graphblas/algorithm/pr.hpp"
 #include "graphblas/algorithm/tc.hpp"
+#include "graphblas/algorithm/gc.hpp"
 
 #include "graphblast_b200.h"
 
@@ -1079,6 +1080,23 @@ int gb200_sssp(gb200_vector_t v, gb200_matrix_t A, int source,
   graphblas::algorithm::lastStatus() = graphblas::GrB_SUCCESS;
   float ms = graphblas::algorithm::sssp(v->f, A->f, source, &desc->desc);
   if (ms < 0.f) return rc(graphblas::algorithm::lastStatus());
+  if (tight_ms) *tight_ms = ms;
+  return 0;
+}
+
+int gb200_gc(gb200_vector_t v, gb200_matrix_t A, int seed, gb200_desc_t desc,
+             int* ncolors, float* tight_ms) {
+  if (v == NULL || A == NULL || desc == NULL)
+    return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
+  if (A->f == NULL && A->i == NULL) return rc(graphblas::GrB_DOMAIN_MISMATCH);
+  GB200_REQUIRE_DEVICE();
+  int count = 0;
+  graphblas::algorithm::lastStatus() = graphblas::GrB_SUCCESS;
+  const float ms = A->f != NULL
+      ? graphblas::algorithm::gc(v->f, A->f, seed, &desc->desc, &count)
+      : graphblas::algorithm::gc(v->f, A->i, seed, &desc->desc, &count);
+  if (ms < 0.f) return rc(graphblas::algorithm::lastStatus());
+  if (ncolors) *ncolors = count;
   if (tight_ms) *tight_ms = ms;
   return 0;
 }

@@ -38,6 +38,7 @@
 #include "graphblas/backend/cuda/apply.hpp"
 #include "graphblas/backend/cuda/indexed.hpp"
 #include "graphblas/backend/cuda/tri.hpp"
+#include "graphblas/backend/cuda/color.hpp"
 
 namespace graphblas {
 namespace backend {
@@ -91,9 +92,15 @@ Info settle(const Vector<X>* x, Rest... rest) {
 GB_DECLARED_ONLY(extract,           "extract of a vector")
 GB_DECLARED_ONLY(assignIndexed,     "assignIndexed")
 GB_DECLARED_ONLY(traceMxmTranspose, "traceMxmTranspose")
-GB_DECLARED_ONLY(graphColor,        "graphColor (cuSPARSE csrcolor, gone from CUDA 12)")
 GB_DECLARED_ONLY(applyVxm,          "applyVxm")
 #undef GB_DECLARED_ONLY
+
+// w = greedy Jones–Plassmann colouring of A's pattern with seed 0 (color.hpp); W is
+// int or float.  algorithm::gc takes other seeds.
+template <typename W, typename a>
+Info graphColor(Vector<W>* w, const Matrix<a>* A, Descriptor* desc) {
+  return graphColorRun(w, A, 0u, static_cast<int*>(NULL));
+}
 
 template <typename TC, typename TA, typename TB, typename TMask,
           typename AccumT,     typename SemiringT>

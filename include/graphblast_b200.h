@@ -300,6 +300,12 @@ int gb200_extract_gather(gb200_vector_t w, gb200_vector_t u, gb200_vector_t indi
 int gb200_bfs_stats(gb200_desc_t desc, int n, unsigned long long* out6);
 int gb200_sssp(gb200_vector_t v, gb200_matrix_t A, int source, gb200_desc_t desc,
                float* tight_ms);                                /* algorithm/sssp.hpp:15-103 */
+/* Greedy Jones-Plassmann colouring of the undirected graph of A's pattern (FP32 or
+ * INT32 A; a non-symmetric A needs its CSC): v[i] = colour of i, 1-based, exact up to
+ * 2^24 colours; *ncolors = the largest colour.  The result is greedy first-fit in
+ * decreasing priority (hash(seed, i), i) order.  include/graphblas/algorithm/gc.hpp */
+int gb200_gc(gb200_vector_t v, gb200_matrix_t A, int seed, gb200_desc_t desc,
+             int* ncolors, float* tight_ms);
 int gb200_pr(gb200_vector_t p, gb200_matrix_t A, float alpha, float eps,
              gb200_desc_t desc, float* tight_ms);               /* algorithm/pr.hpp:15-94 */
 int gb200_tc(long long* ntris, gb200_matrix_t A, gb200_matrix_t B,
