@@ -104,8 +104,6 @@ SIGNATURES = [
     ("gb200_tc", _I, [C.POINTER(_LL), _P, _P, _P, C.POINTER(_F)]),
     ("gb200_rmat_edges", _I, [_I, _LL, _ULL, _LL, _P, _P]),
     ("gb200_vector_export_bits", _I, [_P, _P, C.POINTER(_LL)]),
-    ("gb200_vector_export_bits_async", _I, [_P, _P, _P]),
-    ("gb200_vector_import_bits", _I, [_P, _P, _LL]),
     ("gb200_profile_enable", _I, [_I]),
     ("gb200_profile_reset", _I, []),
     ("gb200_profile_read", _I, [_I, C.POINTER(_D), C.POINTER(_LL),
@@ -115,9 +113,6 @@ SIGNATURES = [
     ("gb200_xchg_handle", _I, [_P, _P]),
     ("gb200_xchg_connect", _I, [_P, _P]),
     ("gb200_xchg_free", _I, [_P]),
-    ("gb200_xchg_allgather_bits", _I, [_P, _P, C.POINTER(_LL)]),
-    ("gb200_xchg_bits_ptr", _I, [_P, C.POINTER(_P)]),
-    ("gb200_dist_bfs", _I, [_P, _P, _P, _LL, _LL, _P, C.POINTER(_I)]),
     ("gb200_dist_bfs_fused", _I, [_P, _P, _P, _LL, _LL, _P, C.POINTER(_I)]),
     ("gb200_xchg_allgather_words", _I, [_P, _P, _D, C.POINTER(_D)]),
     ("gb200_dist_pr", _I, [_P, _P, _P, _LL, _F, _F, _P, C.POINTER(_I)]),

@@ -1129,7 +1129,7 @@ int gb200_tc(long long* ntris, gb200_matrix_t A, gb200_matrix_t B,
   return 0;
 }
 
-// ---- Frontier exchange helpers --------------------------------------------------
+// ---- Vector as a bitmap ---------------------------------------------------------
 
 int gb200_vector_export_bits(gb200_vector_t v, uint32_t* d_bits,
                              long long* count_out) {
@@ -1165,52 +1165,6 @@ int gb200_vector_export_bits(gb200_vector_t v, uint32_t* d_bits,
       GB_KERNEL_CHECK();
       *count_out = static_cast<long long>(runtime().fetch(cell));
     }
-  }
-  return 0;
-}
-
-int gb200_vector_export_bits_async(gb200_vector_t v, uint32_t* d_bits,
-                                   unsigned long long* d_count) {
-  if (v == NULL || d_bits == NULL || d_count == NULL)
-    return rc(graphblas::GrB_NULL_POINTER);
-  int info = gb200_vector_export_bits(v, d_bits, NULL);
-  if (info != 0) return info;
-  using namespace graphblas::backend;
-  cudaStream_t s = gbStream();
-  const size_t nwords =
-      (static_cast<size_t>(v->f->vector_.nsize_) + 31)/32;
-  CUDA_CALL(cudaMemsetAsync(d_count, 0, sizeof(unsigned long long), s));
-  popcountKernel<<<gridFor(nwords, 256), 256, 0, s>>>(d_count, d_bits,
-      static_cast<graphblas::Index>(nwords));
-  GB_KERNEL_CHECK();
-  return 0;
-}
-
-int gb200_vector_import_bits(gb200_vector_t v, const uint32_t* d_bits,
-                             long long nnz) {
-  if (v == NULL || d_bits == NULL) return rc(graphblas::GrB_NULL_POINTER);
-  GB200_REQUIRE_DEVICE();
-  using namespace graphblas::backend;
-  graphblas::backend::Vector<float>& b = v->f->vector_;
-  cudaStream_t s = gbStream();
-  Info info = b.setStorage(graphblas::GrB_DENSE);
-  if (info != GrB_SUCCESS) return rc(info);
-  DenseVector<float>& d = b.dense_;
-  const graphblas::Index n = d.nvals_;
-  unsigned int* bits = d.bitsStorage();
-  CUDA_CALL(cudaMemcpyAsync(bits, d_bits, d.bitWords()*sizeof(unsigned int),
-      cudaMemcpyDeviceToDevice, s));
-  // values are held lazily: the bitmap is the content until somebody needs
-  // the float array (DenseVector::materialize)
-  (void)n;
-  d.touched();
-  d.bits_valid_ = true;
-  d.vals_stale_ = true;
-  d.zero_one_   = true;
-  if (nnz >= 0) {
-    d.nnz_          = static_cast<graphblas::Index>(nnz);
-    d.nnz_valid_    = true;
-    d.nnz_identity_ = 0.f;
   }
   return 0;
 }

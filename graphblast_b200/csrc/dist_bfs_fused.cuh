@@ -6,16 +6,15 @@
 //   flags2[world]         flags2[r] = (last epoch rank r has published << 32) | size of
 //                         the slice it published
 //
-// The host-loop form (gb200_dist_bfs) pays per level: bitmap export, publish kernel,
-// one-warp wait kernel, a host mailbox read, OR / import passes and the generic
-// assign + mxv launches — about 40 us of latency against 10..100 us of work, which
-// is why two GPUs were slower than one in r01.  Here a level is:
+// A level loop on the host paid about 40 us of launches and host round trips per
+// level against 10..100 us of work, so two GPUs were slower than one.  Here a level is:
 //   local phase   push: scan the global frontier, expand the columns of the local
 //                 CSC (owned out-neighbours), claiming owned vertices in the
 //                 replicated visited bitmap; heavy columns by the whole grid.
 //                 pull: every owned unvisited row probes the replicated visited
 //                 bitmap (first-neighbour summary, early exit) — operand reuse in
-//                 its global form, as in gb200_dist_bfs.
+//                 its global form (reference kernels/spmv.hpp:36-38): any visited
+//                 neighbour discovers an unvisited row.
 //   publish       all threads store the owned slice of the new frontier into
 //                 data[epoch & 1] of EVERY rank (peer stores), then one thread
 //                 writes this rank's count and flag to every rank and spins on the
@@ -348,7 +347,15 @@ bfsFusedDistKernel(BfsDistArgs a) {
 
 extern "C" {
 
-// Same contract as gb200_dist_bfs (dist_exchange.cuh), one cooperative launch.
+// Level-synchronous BFS over the 1-D row partition, one cooperative launch:
+//   v    (length nl = owned vertices)  levels of the owned vertices (output)
+//   M    nl x n local matrix: CSR rows = owned destinations (pull), CSC = the
+//        same entries by global source column (push)
+// A pull level probes the replicated cumulative visited bitmap, a push level expands
+// the global frontier.  The direction follows desc's mxvmode (push only, pull only,
+// or the frontier ratio against desc's switchpoint with the hysteresis of reference
+// vector.hpp:318-342); at most desc's max_niter levels.  The exchange x must carry
+// one bit per vertex.
 int gb200_dist_bfs_fused(gb200_xchg_t x, gb200_vector_t v, gb200_matrix_t M,
                          long long n, long long source, gb200_desc_t desc,
                          int* levels_out) {

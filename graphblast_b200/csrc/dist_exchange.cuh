@@ -1,22 +1,23 @@
-// graphblast_b200 — multi-GPU frontier exchange over peer memory and the native
-// level loop of the 1-D row-partitioned BFS (SURVEY.md §8e).  Included by capi.cu.
+// graphblast_b200 — multi-GPU exchange over peer memory and the PageRank / SSSP
+// loops of the 1-D row partition (SURVEY.md §8e).  Included by capi.cu; the BFS
+// runs as one kernel over the same block (dist_bfs_fused.cuh).
 //
 // One process per GPU.  Every rank owns a block of device memory that all ranks
 // map through CUDA IPC:
 //
-//   data[2][total_words]   the replicated frontier (bitmap words), double buffered
-//   counts[2][world]       per-rank entry counts of the published slice
+//   data[2][total_words]   the replicated array (float words, or the fused BFS's
+//                          frontier bitmap), double buffered
+//   counts[2][world]       per-rank partial (a double) of the published slice
 //   flags[world]           flags[r] = number of publishes rank r has completed
 //   visited[2][total_words] (fused BFS only) replicated visited bitmap, by level parity
 //
 // publish(): ONE kernel stores the owned slice into data[parity] of EVERY peer
-// (NVLink stores), then the last CTA writes the slice's count and the new flag
+// (NVLink stores), then the last CTA writes the slice's partial and the new flag
 // value to every peer.  wait(): one warp spins on the local flags until every
-// rank has published this epoch and sums the counts.  No NCCL call, no host
-// round trip besides reading the 8-byte total that decides termination and
-// direction.  Double buffering makes the scheme race free: a rank can only run
-// one publish ahead of the slowest rank, and that publish goes to the other
-// buffer.
+// rank has published this epoch and adds the partials.  No NCCL call, no host
+// round trip besides reading the 8-byte total that decides termination.  Double
+// buffering makes the scheme race free: a rank can only run one publish ahead of
+// the slowest rank, and that publish goes to the other buffer.
 #ifndef GRAPHBLAST_B200_DIST_EXCHANGE_CUH_
 #define GRAPHBLAST_B200_DIST_EXCHANGE_CUH_
 
@@ -29,14 +30,9 @@ struct gb200_xchg_s {
   std::vector<char*> peer;               // peer[rank] == local
   char** d_peer;                         // device copy of peer[]
   unsigned long long  epoch;             // publishes issued so far
-  unsigned long long* d_cells;           // [0] finished CTAs, [1] popcount, [2] total
-  unsigned int*       d_visited;         // cumulative visited bitmap (total_words)
-  unsigned int*       d_seed;            // owned-slice scratch
+  unsigned long long* d_cells;           // [0] finished CTAs, [1] total
+  unsigned int*       d_seed;            // level-1 frontier of the fused BFS
   bool connected;
-  // vectors of the level loop, kept across traversals
-  graphblas::Vector<float>* f_own;
-  graphblas::Vector<float>* f2;
-  graphblas::Vector<float>* f_glob;
   // vectors of the PageRank loop: p_glob, p_prev_own, p_swap, r, r_temp
   graphblas::Vector<float>* pr_vec[5];
   // vectors of the SSSP loop: frontier_glob (view), relaxed, improved
@@ -50,17 +46,13 @@ using namespace graphblas::backend;  // NOLINT(build/namespaces)
 #define GBX_NT 256
 
 // Stores src[0..nwords) at word offset word_lo of data[] in every peer's block,
-// then (last CTA) the count and the flag.  d_count_in != NULL: the count is
-// already on the device; otherwise it is the popcount of the words.
+// then (last CTA) the 8-byte partial and the flag.
 __global__ void __launch_bounds__(GBX_NT)
 xchgPublishKernel(const unsigned int* __restrict__ src, size_t nwords,
                   size_t word_lo, char* const* __restrict__ peers, int world,
                   int rank, size_t off_data, size_t off_counts, size_t off_flags,
                   unsigned long long epoch, unsigned long long* d_cells,
-                  const unsigned long long* d_count_in, int use_imm,
-                  unsigned long long imm) {
-  __shared__ int s_red[GBX_NT/32];
-  int pop = 0;
+                  unsigned long long partial) {
   size_t i = static_cast<size_t>(blockIdx.x)*GBX_NT + threadIdx.x;
   const size_t stride = static_cast<size_t>(gridDim.x)*GBX_NT;
   const bool vec = ((nwords | word_lo) & 3) == 0 &&
@@ -71,7 +63,6 @@ xchgPublishKernel(const unsigned int* __restrict__ src, size_t nwords,
     const size_t n4 = nwords >> 2;
     for (; i < n4; i += stride) {
       const uint4 w = src4[i];
-      pop += __popc(w.x) + __popc(w.y) + __popc(w.z) + __popc(w.w);
       for (int p = 0; p < world; ++p) {
         uint4* dst = reinterpret_cast<uint4*>(
             reinterpret_cast<unsigned int*>(peers[p] + off_data) + word_lo) + i;
@@ -81,7 +72,6 @@ xchgPublishKernel(const unsigned int* __restrict__ src, size_t nwords,
   } else {
     for (; i < nwords; i += stride) {
       const unsigned int w = src[i];
-      pop += __popc(w);
       for (int p = 0; p < world; ++p) {
         unsigned int* dst =
             reinterpret_cast<unsigned int*>(peers[p] + off_data) + word_lo + i;
@@ -89,22 +79,16 @@ xchgPublishKernel(const unsigned int* __restrict__ src, size_t nwords,
       }
     }
   }
-  const int total = blockSum<GBX_NT>(pop, s_red);
-  if (threadIdx.x == 0 && total != 0 && d_count_in == NULL && !use_imm)
-    atomicAdd(d_cells + 1, static_cast<unsigned long long>(total));
   __threadfence_system();          // this CTA's peer stores before its "done"
   __syncthreads();
   if (threadIdx.x == 0) {
     const unsigned long long done = atomicAdd(d_cells, 1ull);
     if (done == gridDim.x - 1) {
       __threadfence();
-      const unsigned long long cnt = use_imm ? imm : (d_count_in != NULL)
-          ? *d_count_in
-          : *reinterpret_cast<volatile unsigned long long*>(d_cells + 1);
       for (int p = 0; p < world; ++p) {
         volatile unsigned long long* c = reinterpret_cast<
             volatile unsigned long long*>(peers[p] + off_counts) + rank;
-        *c = cnt;
+        *c = partial;
       }
       __threadfence_system();      // data + counts before the flag
       for (int p = 0; p < world; ++p) {
@@ -113,20 +97,18 @@ xchgPublishKernel(const unsigned int* __restrict__ src, size_t nwords,
         *f = epoch;
       }
       d_cells[0] = 0ull;
-      d_cells[1] = 0ull;
     }
   }
 }
 
-// One warp: waits until every rank's flag has reached `epoch`, then
-// d_cells[2] = sum of the published counts (all ones on timeout).
+// One warp: waits until every rank's flag has reached `epoch`, then d_cells[1] =
+// the bits of the ranks' partials (doubles) added in rank order, so every rank
+// computes the identical total (all ones on timeout).
 __global__ void xchgWaitKernel(const char* __restrict__ local, size_t off_counts,
                                size_t off_flags, int world,
                                unsigned long long epoch,
                                unsigned long long* d_cells,
-                               long long timeout_cycles, int as_double,
-                               unsigned long long* mail,
-                               unsigned long long ticket) {
+                               long long timeout_cycles) {
   const int lane = threadIdx.x;
   bool ok = true;
   if (lane < world) {
@@ -144,45 +126,19 @@ __global__ void xchgWaitKernel(const char* __restrict__ local, size_t off_counts
   if (ok && lane < world)
     c = *(reinterpret_cast<const volatile unsigned long long*>(
         local + off_counts) + lane);
-  if (as_double) {
-    // the per-rank cells hold doubles (partial sums); lane 0 adds them in rank
-    // order so every rank computes the identical total
-    double sum = 0.0;
-    for (int p = 0; p < world; ++p) {
-      const unsigned long long bits = __shfl_sync(GB_FULL_MASK, c, p);
-      sum += __longlong_as_double(static_cast<long long>(bits));
-    }
-    if (lane == 0)
-      d_cells[2] = ok ? static_cast<unsigned long long>(
-          __double_as_longlong(sum)) : ~0ull;
-    return;
+  double sum = 0.0;
+#pragma unroll 1   // at most 32 ranks once per exchange; unrolled it takes more registers
+  for (int p = 0; p < world; ++p) {
+    const unsigned long long bits = __shfl_sync(GB_FULL_MASK, c, p);
+    sum += __longlong_as_double(static_cast<long long>(bits));
   }
-  for (int d = 16; d > 0; d >>= 1)
-    c += __shfl_down_sync(GB_FULL_MASK, c, d);
-  if (lane == 0) {
-    d_cells[2] = ok ? c : ~0ull;
-    if (mail != NULL && ok && c < (1ull << 40)) {   // host mailbox (util.hpp)
-      *reinterpret_cast<volatile unsigned long long*>(mail) = (ticket << 40) | c;
-      __threadfence_system();
-    }
-  }
+  if (lane == 0)
+    d_cells[1] = ok ? static_cast<unsigned long long>(
+        __double_as_longlong(sum)) : ~0ull;
 }
 
-// dst[i] |= src[i]
-__global__ void orWordsKernel(unsigned int* __restrict__ dst,
-                              const unsigned int* __restrict__ src, size_t n) {
-  size_t i = static_cast<size_t>(blockIdx.x)*blockDim.x + threadIdx.x;
-  const size_t stride = static_cast<size_t>(gridDim.x)*blockDim.x;
-  for (; i < n; i += stride) dst[i] |= src[i];
-}
-
-__global__ void setBitKernel(unsigned int* words, long long bit) {
-  words[bit >> 5] = 1u << (bit & 31);
-}
-
-inline int publish(gb200_xchg_s* x, const unsigned int* d_words,
-                   const unsigned long long* d_count, int use_imm = 0,
-                   unsigned long long imm = 0ull) {
+inline void publish(gb200_xchg_s* x, const unsigned int* d_words,
+                    unsigned long long partial) {
   cudaStream_t s = gbStream();
   x->epoch += 1;
   const int par = static_cast<int>(x->epoch & 1ull);
@@ -192,33 +148,20 @@ inline int publish(gb200_xchg_s* x, const unsigned int* d_words,
   if (grid < 1) grid = 1;
   xchgPublishKernel<<<grid, GBX_NT, 0, s>>>(d_words, nw, x->word_off[x->rank],
       x->d_peer, x->world, x->rank, x->off_data[par], x->off_counts[par],
-      x->off_flags, x->epoch, x->d_cells, d_count, use_imm, imm);
+      x->off_flags, x->epoch, x->d_cells, partial);
   GB_KERNEL_CHECK();
-  return 0;
 }
 
-// Waits for the epoch just published; returns the raw 8-byte total (integer
-// sum of the ranks' cells, or the bits of their double sum), ~0 on timeout.
-inline unsigned long long waitRaw(gb200_xchg_s* x, int as_double) {
+// Waits for the epoch just published; returns the bits of the total (a double),
+// ~0 on timeout.
+inline unsigned long long wait(gb200_xchg_s* x) {
   cudaStream_t s = gbStream();
   const int par = static_cast<int>(x->epoch & 1ull);
   // ~10 s at 2 GHz: a rank that died must not hang the others' GPUs
-  // integer totals are posted to the host mailbox: no stream synchronisation
-  const bool mail = !as_double;
-  const unsigned long long ticket = mail ? runtime().mailTicket() : 0ull;
   xchgWaitKernel<<<1, 32, 0, s>>>(x->local, x->off_counts[par], x->off_flags,
-      x->world, x->epoch, x->d_cells, 20000000000ll, as_double,
-      mail ? runtime().mailSlot(3) : NULL, ticket);
+      x->world, x->epoch, x->d_cells, 20000000000ll);
   GB_KERNEL_CHECK();
-  if (mail) return runtime().mailWait(3, ticket, x->d_cells + 2);
-  return runtime().fetch(x->d_cells + 2);
-}
-
-// Returns the global count of the epoch just published, or -1 on timeout.
-inline long long wait(gb200_xchg_s* x) {
-  const unsigned long long total = waitRaw(x, 0);
-  if (total == ~0ull) return -1;
-  return static_cast<long long>(total);
+  return runtime().fetch(x->d_cells + 1);
 }
 
 inline const unsigned int* current(gb200_xchg_s* x) {
@@ -256,9 +199,8 @@ int gb200_xchg_create(gb200_xchg_t* out, int world, int rank,
   x->bytes = off;
   CUDA_CALL(cudaMalloc(&x->local, x->bytes));
   CUDA_CALL(cudaMemset(x->local, 0, x->bytes));
-  CUDA_CALL(cudaMalloc(&x->d_cells, 8*sizeof(unsigned long long)));
-  CUDA_CALL(cudaMemset(x->d_cells, 0, 8*sizeof(unsigned long long)));
-  CUDA_CALL(cudaMalloc(&x->d_visited, (x->total_words + 8)*4));
+  CUDA_CALL(cudaMalloc(&x->d_cells, 2*sizeof(unsigned long long)));
+  CUDA_CALL(cudaMemset(x->d_cells, 0, 2*sizeof(unsigned long long)));
   CUDA_CALL(cudaMalloc(&x->d_seed, (x->total_words + 8)*4));
   CUDA_CALL(cudaMalloc(&x->d_peer, world*sizeof(char*)));
   x->peer.assign(world, static_cast<char*>(NULL));
@@ -268,7 +210,6 @@ int gb200_xchg_create(gb200_xchg_t* out, int world, int rank,
   if (world == 1)
     CUDA_CALL(cudaMemcpy(x->d_peer, x->peer.data(), sizeof(char*),
         cudaMemcpyHostToDevice));
-  x->f_own = NULL; x->f2 = NULL; x->f_glob = NULL;
   for (int i = 0; i < 5; ++i) x->pr_vec[i] = NULL;
   for (int i = 0; i < 3; ++i) x->ss_vec[i] = NULL;
   *out = x;
@@ -312,141 +253,16 @@ int gb200_xchg_free(gb200_xchg_t x) {
   cudaDeviceSynchronize();
   for (int p = 0; p < x->world; ++p)
     if (p != x->rank && x->peer[p] != NULL) cudaIpcCloseMemHandle(x->peer[p]);
-  cudaFree(x->local); cudaFree(x->d_cells); cudaFree(x->d_visited);
-  cudaFree(x->d_seed); cudaFree(x->d_peer);
-  delete x->f_own; delete x->f2; delete x->f_glob;
+  cudaFree(x->local); cudaFree(x->d_cells); cudaFree(x->d_seed);
+  cudaFree(x->d_peer);
   for (int i = 0; i < 5; ++i) delete x->pr_vec[i];
   for (int i = 0; i < 3; ++i) delete x->ss_vec[i];
   delete x;
   return 0;
 }
 
-// Publishes the owned slice held in vector v (dense or sparse, length = owned
-// vertex count) and returns the global entry count once every rank has done so.
-int gb200_xchg_allgather_bits(gb200_xchg_t x, gb200_vector_t v,
-                              long long* total_out) {
-  if (x == NULL || v == NULL || total_out == NULL)
-    return rc(graphblas::GrB_NULL_POINTER);
-  if (!x->connected) return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
-  GB200_REQUIRE_DEVICE();
-  int info = gb200_vector_export_bits_async(v, x->d_seed, x->d_cells + 3);
-  if (info != 0) return info;
-  gbx::publish(x, x->d_seed, x->d_cells + 3);
-  const long long total = gbx::wait(x);
-  if (total < 0) return rc(graphblas::GrB_PANIC);
-  *total_out = total;
-  return 0;
-}
-
-int gb200_xchg_bits_ptr(gb200_xchg_t x, const uint32_t** d_bits) {
-  if (x == NULL || d_bits == NULL) return rc(graphblas::GrB_NULL_POINTER);
-  *d_bits = gbx::current(x);
-  return 0;
-}
-
-// Level-synchronous BFS over the 1-D row partition, host loop in C++:
-//   v    (length nl = owned vertices)  levels of the owned vertices (output)
-//   M    nl x n local matrix: CSR rows = owned destinations (pull), CSC = the
-//        same entries by global source column (push)
-// Per level: v<f_own> = level;  f2<!v> = M (||.&&) u  with u = the cumulative
-// visited set when pulling (any visited neighbour discovers an unvisited row —
-// the operand-reuse shortcut of reference kernels/spmv.hpp:36-38 in its global
-// form) and u = the frontier when pushing;  all ranks exchange f2 through peer
-// memory.  The direction follows the frontier ratio with the hysteresis of
-// reference vector.hpp:318-342.
-int gb200_dist_bfs(gb200_xchg_t x, gb200_vector_t v, gb200_matrix_t M,
-                   long long n, long long source, gb200_desc_t desc,
-                   int* levels_out) {
-  if (x == NULL || v == NULL || M == NULL || desc == NULL)
-    return rc(graphblas::GrB_NULL_POINTER);
-  if (!x->connected || M->f == NULL) return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
-  GB200_REQUIRE_DEVICE();
-  using namespace graphblas;          // NOLINT(build/namespaces)
-  using graphblas::backend::gbStream;
-  using graphblas::backend::gridFor;
-  cudaStream_t s = gbStream();
-  Descriptor* d = &desc->desc;
-  const size_t w_lo = x->word_off[x->rank];
-  const size_t nw   = x->word_off[x->rank + 1] - w_lo;
-  Index nl;
-  CHECK(v->f->size(&nl));
-  const long long lo = static_cast<long long>(w_lo)*32;
-  if (x->f_own == NULL) {
-    x->f_own  = new Vector<float>(nl);
-    x->f2     = new Vector<float>(nl);
-    x->f_glob = new Vector<float>(static_cast<Index>(n));
-  }
-  gb200_vector_s own_h  = {GB200_FP32, x->f_own};
-  gb200_vector_s f2_h   = {GB200_FP32, x->f2};
-  gb200_vector_s glob_h = {GB200_FP32, x->f_glob};
-
-  CHECK(v->f->fill(0.f));
-  CUDA_CALL(cudaMemsetAsync(x->d_visited, 0, x->total_words*4, s));
-  // level-1 frontier = {source}, published by its owner
-  CUDA_CALL(cudaMemsetAsync(x->d_seed, 0, (nw + 1)*4, s));
-  const bool own_src = source >= lo && source < lo + static_cast<long long>(nl);
-  if (own_src) {
-    gbx::setBitKernel<<<1, 1, 0, s>>>(x->d_seed, source - lo);
-    GB_KERNEL_CHECK();
-  }
-  CUDA_CALL(cudaMemsetAsync(x->d_cells + 3, 0, 8, s));
-  if (own_src) {
-    const unsigned long long one = 1ull;
-    CUDA_CALL(cudaMemcpyAsync(x->d_cells + 3, &one, 8, cudaMemcpyHostToDevice, s));
-  }
-  gbx::publish(x, x->d_seed, x->d_cells + 3);
-  long long total = gbx::wait(x);
-  if (total < 0) return rc(GrB_PANIC);
-
-  Desc_value saved_mode;
-  CHECK(d->get(GrB_MXVMODE, &saved_mode));
-  const float switchpoint = d->descriptor_.switchpoint();
-  float prev_ratio = 0.f;
-  bool  pulling = false;
-  int   level = 0;
-  Info  info = GrB_SUCCESS;
-  while (total > 0) {
-    ++level;
-    const unsigned int* gbits = gbx::current(x);
-    gbx::orWordsKernel<<<gridFor(x->total_words, 256), 256, 0, s>>>(
-        x->d_visited, gbits, x->total_words);
-    GB_KERNEL_CHECK();
-    // v<f_own> = level
-    if (gb200_vector_import_bits(&own_h, gbits + w_lo, -1) != 0) { info = GrB_PANIC; break; }
-    info = graphblas::assign<float, float, float, Index>(v->f, x->f_own,
-        GrB_NULL, static_cast<float>(level), GrB_ALL, nl, d);
-    if (info != GrB_SUCCESS) break;
-    // direction
-    const float ratio = static_cast<float>(total)/static_cast<float>(n);
-    if (!pulling) { if (ratio > switchpoint && ratio > prev_ratio) pulling = true; }
-    else          { if (ratio <= switchpoint && ratio < prev_ratio) pulling = false; }
-    prev_ratio = ratio;
-    if (pulling) {
-      if (gb200_vector_import_bits(&glob_h, x->d_visited, -1) != 0) { info = GrB_PANIC; break; }
-      CHECK(d->set(GrB_MXVMODE, GrB_PULLONLY));
-      CHECK(x->f2->vector_.setStorage(GrB_DENSE));
-    } else {
-      if (gb200_vector_import_bits(&glob_h, gbits, total) != 0) { info = GrB_PANIC; break; }
-      CHECK(d->set(GrB_MXVMODE, GrB_PUSHONLY));
-    }
-    CHECK(d->toggle(GrB_MASK));
-    info = graphblas::mxv<float, float, float, float>(x->f2, v->f, GrB_NULL,
-        LogicalOrAndSemiring<float>(), M->f, x->f_glob, d);
-    CHECK(d->toggle(GrB_MASK));
-    if (info != GrB_SUCCESS) break;
-    // the publish kernel counts the bits it sends
-    if (gb200_vector_export_bits(&f2_h, x->d_seed, NULL) != 0) { info = GrB_PANIC; break; }
-    gbx::publish(x, x->d_seed, NULL);
-    total = gbx::wait(x);
-    if (total < 0) { info = GrB_PANIC; break; }
-  }
-  d->set(GrB_MXVMODE, saved_mode);
-  if (levels_out != NULL) *levels_out = level;
-  return rc(info);
-}
-
-// Generic form for 32-bit payloads (float vectors): publishes nwords_owned words
-// from d_words with this rank's partial scalar; *sum_out = sum over ranks.
+// Publishes the owned 32-bit words (float vectors) from d_words with this rank's
+// partial scalar; *sum_out = sum over ranks.
 int gb200_xchg_allgather_words(gb200_xchg_t x, const void* d_words,
                                double partial, double* sum_out) {
   if (x == NULL || d_words == NULL || sum_out == NULL)
@@ -455,8 +271,8 @@ int gb200_xchg_allgather_words(gb200_xchg_t x, const void* d_words,
   GB200_REQUIRE_DEVICE();
   unsigned long long bits;
   memcpy(&bits, &partial, 8);
-  gbx::publish(x, static_cast<const unsigned int*>(d_words), NULL, 1, bits);
-  const unsigned long long total = gbx::waitRaw(x, 1);
+  gbx::publish(x, static_cast<const unsigned int*>(d_words), bits);
+  const unsigned long long total = gbx::wait(x);
   if (total == ~0ull) return rc(graphblas::GrB_PANIC);
   memcpy(sum_out, &total, 8);
   return 0;

@@ -311,21 +311,10 @@ int gb200_pr(gb200_vector_t p, gb200_matrix_t A, float alpha, float eps,
 int gb200_tc(long long* ntris, gb200_matrix_t A, gb200_matrix_t B,
              gb200_desc_t desc, float* tight_ms);               /* algorithm/tc.hpp:15-54 */
 
-/* ---- Frontier exchange helpers for the 1-D row-partitioned multi-GPU path ----
- * (SURVEY.md §8e; the reference has no distributed path.)  A Boolean frontier
- * travels between ranks as a bitmap, n/8 bytes for n vertices. */
+/* ---- Vector as a bitmap (no reference counterpart) ------------------------- */
 /* Bitmap (bit == value != 0) of v into DEVICE words d_bits[(size+31)/32]; works
  * for dense and sparse storage.  count_out (may be NULL) receives the popcount. */
 int gb200_vector_export_bits(gb200_vector_t v, uint32_t* d_bits, long long* count_out);
-/* Same, without any host synchronisation: the 64-bit popcount is written on the
- * device into d_count (8-byte aligned DEVICE address), e.g. the tail of the
- * record a rank contributes to the frontier all-gather. */
-int gb200_vector_export_bits_async(gb200_vector_t v, uint32_t* d_bits,
-                                   unsigned long long* d_count);
-/* v becomes a dense 0/1 vector with the given bitmap (DEVICE words).
- * nnz >= 0 tells the number of set bits (saves the counting pass of the next
- * direction decision); pass -1 when unknown. */
-int gb200_vector_import_bits(gb200_vector_t v, const uint32_t* d_bits, long long nnz);
 
 /* ---- Measurement hooks (bench.py; no reference counterpart) --------------- */
 /* Hot-kernel kinds: 0 merge-path SpMV (pull, generic semiring), 1 fused Boolean
@@ -361,27 +350,19 @@ int gb200_xchg_create(gb200_xchg_t* out, int world, int rank,
 int gb200_xchg_handle(gb200_xchg_t x, void* out64);
 int gb200_xchg_connect(gb200_xchg_t x, const void* handles /* world x 64 bytes */);
 int gb200_xchg_free(gb200_xchg_t x);
-/* Publishes the owned slice (vector of the owned length, dense or sparse) and
- * waits for all ranks; *total_out = global number of entries. */
-int gb200_xchg_allgather_bits(gb200_xchg_t x, gb200_vector_t v,
-                              long long* total_out);
-/* DEVICE pointer to the replicated bitmap of the last completed exchange. */
-int gb200_xchg_bits_ptr(gb200_xchg_t x, const uint32_t** d_bits);
-/* Level-synchronous BFS over the 1-D row partition with the level loop in the
- * library: v = levels of the owned vertices (length = owned rows of M), M = the
- * owned rows of A^T as an (owned x n) matrix with CSR and CSC.  Collective: every
- * rank calls it with the same n and source. */
-int gb200_dist_bfs(gb200_xchg_t x, gb200_vector_t v, gb200_matrix_t M,
-                   long long n, long long source, gb200_desc_t desc,
-                   int* levels_out);
-/* The same traversal as ONE persistent cooperative kernel per GPU: level loop,
- * direction decision, peer-memory exchange of the frontier slice and the cross-GPU
- * level barrier all on the device (csrc/dist_bfs_fused.cuh). */
+/* Direction-optimised BFS over the 1-D row partition as ONE persistent cooperative
+ * kernel per GPU: level loop, direction decision, peer-memory exchange of the
+ * frontier slice and the cross-GPU level barrier all on the device
+ * (csrc/dist_bfs_fused.cuh).  The exchange carries one bit per vertex
+ * (word_offsets = vertex bounds / 32, rounded up).  v_own = levels of the owned
+ * vertices (length = owned rows of M_local), M_local = the owned rows of A^T as an
+ * (owned x n) matrix with CSR and CSC.  Collective: every rank calls it with the
+ * same n and source. */
 int gb200_dist_bfs_fused(gb200_xchg_t x, gb200_vector_t v_own, gb200_matrix_t M_local,
                          long long n, long long source, gb200_desc_t desc,
                          int* levels_out);
 
-/* Same exchange for 32-bit payloads (float vectors: create the exchange with one
+/* The exchange for 32-bit payloads (float vectors: create the exchange with one
  * word per vertex).  Publishes the owned words from DEVICE memory together with
  * this rank's partial scalar; *sum_out = the ranks' partials added in rank order
  * (identical on every rank). */

@@ -1,7 +1,8 @@
-"""GPU tests of the multi-GPU layer: the peer-memory exchange and the native level
-loop (gb200_dist_bfs) against the oracle.  World size 1 runs on any GPU box (the
-owner stores into its own replica).  The 2-rank tests run two processes; on a box
-with one GPU both share it (graphblast_b200.dist.init_rank)."""
+"""GPU tests of the multi-GPU layer: the peer-memory exchange and the BFS, PageRank
+and SSSP over it (gb200_dist_bfs_fused, gb200_dist_pr, gb200_dist_sssp) against the
+oracle.  World size 1 runs on any GPU box (the owner stores into its own replica).
+The 2-rank tests run two processes; on a box with one GPU both share it
+(graphblast_b200.dist.init_rank)."""
 import json
 import os
 import subprocess
@@ -16,54 +17,32 @@ import oracle_binding as orc
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _setup(scale, dev):
+@pytest.mark.gpu
+@pytest.mark.parametrize("scale", [10, 14, 17])
+def test_dist_bfs_world1(scale):
+    """gb200_dist_bfs_fused on one rank against the oracle: exact levels."""
     import graphblast_b200 as gb
     from graphblast_b200 import dist as gdist
+    dev = torch.device("cuda", 0)
     rp, ci = orc.rmat_csr(scale)
     n = len(rp) - 1
     rowptr = torch.from_numpy(rp).to(dev)
     colind = torch.from_numpy(ci).to(dev)
-    rp_l, ci_l, colptr, rowind = gdist.local_slice(rowptr, colind, 0, n, n)
+    M, keep = gdist.weighted_local_matrix(gb, n, rowptr, colind, None, 0, n)
+    v = gb.Vector(n)
     desc = gb.Descriptor(mxvmode=0, struconly=1, opreuse=0, earlyexit=1)
-    ops = gdist.GpuLocalOps(gb, n, 0, n, rp_l, ci_l, colptr, rowind, desc)
-    comm = gdist.Comm([0, n], dev)
-    return gb, gdist, rp, ci, n, ops, comm
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("scale", [10, 14, 17])
-def test_native_level_loop_world1(scale):
-    dev = torch.device("cuda", 0)
-    gb, gdist, rp, ci, n, ops, comm = _setup(scale, dev)
-    x = gdist.PeerExchange(gb, comm, dev)
+    x = gdist.PeerExchange(gb, [0, n], dev, bits=True)
     try:
         deg = np.diff(rp)
         for source in (int(np.argmax(deg)), int(np.nonzero(deg)[0][-1])):
             want = orc.bfs(rp, ci, source)
             for _ in range(2):                      # state is reset per traversal
-                levels = x.bfs(ops, n, source)
-                got = ops.levels().astype(np.int32)
+                levels = x.bfs(v, M, n, source, desc)
+                got = v.extractTuples()[:n].astype(np.int32)
                 assert np.array_equal(got, want)
                 assert levels == int(want.max())
     finally:
         x.close()
-
-
-@pytest.mark.gpu
-def test_python_and_native_loops_agree():
-    dev = torch.device("cuda", 0)
-    gb, gdist, rp, ci, n, ops, comm = _setup(13, dev)
-    source = int(np.argmax(np.diff(rp)))
-    gdist.run_bfs(ops, comm, source)
-    a = ops.levels().copy()
-    x = gdist.PeerExchange(gb, comm, dev)
-    try:
-        x.bfs(ops, n, source)
-        b = ops.levels().copy()
-    finally:
-        x.close()
-    assert np.array_equal(a, b)
-    assert np.array_equal(a.astype(np.int32), orc.bfs(rp, ci, source))
 
 
 @pytest.mark.gpu
@@ -85,7 +64,7 @@ def test_two_ranks_peer_exchange():
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("scale", [10, 15])
-def test_native_pagerank_world1(scale):
+def test_dist_pr_world1(scale):
     """gb200_dist_pr on one rank (the owner publishes into its own replica) against
     the oracle: 10 power iterations, 1e-5 relative."""
     import ctypes as C
@@ -106,8 +85,7 @@ def test_native_pagerank_world1(scale):
                                       C.c_void_p(val.data_ptr()), int(len(ci))) == 0
     p = gb.Vector(n)
     desc = gb.Descriptor(mxvmode=0, max_niter=10)
-    comm = gdist.Comm([0, n], dev)
-    x = gdist.PeerExchange(gb, comm, dev, offsets=[0, n])
+    x = gdist.PeerExchange(gb, [0, n], dev, bits=False)
     try:
         for _ in range(2):
             iters = x.pr(p, M, n, alpha, 0.0, desc)
@@ -138,7 +116,7 @@ def test_two_ranks_pagerank():
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("scale", [10, 15])
-def test_native_sssp_world1(scale):
+def test_dist_sssp_world1(scale):
     """gb200_dist_sssp on one rank against the oracle: bit-exact distances."""
     import graphblast_b200 as gb
     from graphblast_b200 import dist as gdist, graphs
@@ -153,8 +131,7 @@ def test_native_sssp_world1(scale):
     M, keep = gdist.weighted_local_matrix(gb, n, rowptr, colind, d_wt, 0, n)
     v = gb.Vector(n)
     desc = gb.Descriptor(mxvmode=0, switchpoint=0.025)
-    comm = gdist.Comm([0, n], dev)
-    x = gdist.PeerExchange(gb, comm, dev, offsets=[0, n])
+    x = gdist.PeerExchange(gb, [0, n], dev, bits=False)
     try:
         deg = np.diff(rp)
         for source in (int(np.argmax(deg)), int(np.nonzero(deg)[0][-1])):
