@@ -1,9 +1,9 @@
 """graphblas::algorithm — the GraphBLAS algorithm drivers of the reference
 (graphblas/algorithm/{bfs,sssp,pr,tc}.hpp), executed inside the native library as
 loops of backend operations (include/graphblas/algorithm/*.hpp), and the graph
-colouring gc, one kernel on the device.
+colouring gc and the maximal independent set mis, one kernel each on the device.
 
-sssp, pr, tc and gc return the device time of the operation loop in milliseconds
+sssp, pr, tc, gc and mis return the device time of the operation loop in milliseconds
 ("tight" in the reference drivers, example/gbfs.cu:110-115).  bfs returns it only
 when called with timed=True; otherwise it returns None and, when the traversal runs
 as the fused kernel, only enqueues it, so that back-to-back traversals keep the GPU
@@ -63,4 +63,20 @@ def gc(v, A, seed, desc):
     k = C.c_int(0)
     _check(_lib.load().gb200_gc(v._h, A._h, int(seed), desc._h, C.byref(k), C.byref(ms)),
            "algorithm::gc")
+    return k.value, ms.value
+
+
+def mis(v, A, seed, desc, candidates=None):
+    """v[i] = 1 when vertex i is in the maximal independent set of the undirected graph
+    of A's pattern, else 0: the greedy set in decreasing priority (hash(seed, i), i)
+    order over the candidates, the priority of gc (include/graphblas/algorithm/mis.hpp).
+    candidates: None (every vertex) or a Vector whose non-zero entries name the
+    candidates; it is not converted and may be v itself.  A is FP32 or INT32; a
+    non-symmetric A needs its CSC.  Returns (nmembers, tight_ms)."""
+    ms = C.c_float(0)
+    k = C.c_int(0)
+    _check(_lib.load().gb200_mis(v._h, A._h, int(seed),
+                                 candidates._h if candidates is not None else None,
+                                 desc._h, C.byref(k), C.byref(ms)),
+           "algorithm::mis")
     return k.value, ms.value

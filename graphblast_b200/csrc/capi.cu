@@ -25,6 +25,7 @@
 #include "graphblas/algorithm/pr.hpp"
 #include "graphblas/algorithm/tc.hpp"
 #include "graphblas/algorithm/gc.hpp"
+#include "graphblas/algorithm/mis.hpp"
 
 #include "graphblast_b200.h"
 
@@ -1097,6 +1098,24 @@ int gb200_gc(gb200_vector_t v, gb200_matrix_t A, int seed, gb200_desc_t desc,
       : graphblas::algorithm::gc(v->f, A->i, seed, &desc->desc, &count);
   if (ms < 0.f) return rc(graphblas::algorithm::lastStatus());
   if (ncolors) *ncolors = count;
+  if (tight_ms) *tight_ms = ms;
+  return 0;
+}
+
+int gb200_mis(gb200_vector_t v, gb200_matrix_t A, int seed, gb200_vector_t candidates,
+              gb200_desc_t desc, int* nmembers, float* tight_ms) {
+  if (v == NULL || A == NULL || desc == NULL)
+    return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
+  if (A->f == NULL && A->i == NULL) return rc(graphblas::GrB_DOMAIN_MISMATCH);
+  GB200_REQUIRE_DEVICE();
+  int count = 0;
+  const graphblas::Vector<float>* cand = candidates != NULL ? candidates->f : NULL;
+  graphblas::algorithm::lastStatus() = graphblas::GrB_SUCCESS;
+  const float ms = A->f != NULL
+      ? graphblas::algorithm::mis(v->f, A->f, seed, &desc->desc, &count, cand)
+      : graphblas::algorithm::mis(v->f, A->i, seed, &desc->desc, &count, cand);
+  if (ms < 0.f) return rc(graphblas::algorithm::lastStatus());
+  if (nmembers) *nmembers = count;
   if (tight_ms) *tight_ms = ms;
   return 0;
 }

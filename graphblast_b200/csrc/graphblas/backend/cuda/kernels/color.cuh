@@ -97,12 +97,15 @@ __device__ __forceinline__ void gcStoreColour(unsigned int* p, unsigned int c) {
   asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" :: "l"(p), "r"(c) : "memory");
 }
 
-// A vertex's list: its CSR row, then its CSC column (dc = 0 when symmetric).
+// A vertex's list: its CSR row, then its CSC column (dc = 0 when symmetric).  Args is
+// any kernel argument struct with GcArgs's row_ptr / row_ind / col_ptr / col_ind
+// (GcArgs here, MisArgs in kernels/mis.cuh).
 struct GcList {
   Index r0, dr, c0, dc;
 };
 
-__device__ __forceinline__ GcList gcListOf(const GcArgs a, Index v) {
+template <typename Args>
+__device__ __forceinline__ GcList gcListOf(const Args a, Index v) {
   GcList l;
   l.r0 = a.row_ptr[v];
   l.dr = a.row_ptr[v + 1] - l.r0;
@@ -114,7 +117,8 @@ __device__ __forceinline__ GcList gcListOf(const GcArgs a, Index v) {
   return l;
 }
 
-__device__ __forceinline__ Index gcEntry(const GcArgs a, const GcList& l, Index k) {
+template <typename Args>
+__device__ __forceinline__ Index gcEntry(const Args a, const GcList& l, Index k) {
   return k < l.dr ? __ldg(a.row_ind + l.r0 + k) : __ldg(a.col_ind + l.c0 + (k - l.dr));
 }
 

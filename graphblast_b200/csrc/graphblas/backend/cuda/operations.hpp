@@ -39,6 +39,7 @@
 #include "graphblas/backend/cuda/indexed.hpp"
 #include "graphblas/backend/cuda/tri.hpp"
 #include "graphblas/backend/cuda/color.hpp"
+#include "graphblas/backend/cuda/mis.hpp"
 
 namespace graphblas {
 namespace backend {

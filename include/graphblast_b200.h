@@ -306,6 +306,14 @@ int gb200_sssp(gb200_vector_t v, gb200_matrix_t A, int source, gb200_desc_t desc
  * decreasing priority (hash(seed, i), i) order.  include/graphblas/algorithm/gc.hpp */
 int gb200_gc(gb200_vector_t v, gb200_matrix_t A, int seed, gb200_desc_t desc,
              int* ncolors, float* tight_ms);
+/* Maximal independent set of the undirected graph of A's pattern (FP32 or INT32 A; a
+ * non-symmetric A needs its CSC): v[i] = 1 for members, 0 otherwise; *nmembers = the
+ * size of the set.  The set is the greedy MIS in decreasing priority (hash(seed, i), i)
+ * order over the candidates, the priority of gb200_gc.  candidates may be NULL (every
+ * vertex); otherwise i is a candidate when the vector holds a non-zero value for it.
+ * It is never converted and may be v itself.  include/graphblas/algorithm/mis.hpp */
+int gb200_mis(gb200_vector_t v, gb200_matrix_t A, int seed, gb200_vector_t candidates,
+              gb200_desc_t desc, int* nmembers, float* tight_ms);
 int gb200_pr(gb200_vector_t p, gb200_matrix_t A, float alpha, float eps,
              gb200_desc_t desc, float* tight_ms);               /* algorithm/pr.hpp:15-94 */
 int gb200_tc(long long* ntris, gb200_matrix_t A, gb200_matrix_t B,
