@@ -6,6 +6,7 @@
 
 #include <type_traits>
 
+#include "graphblas/backend/cuda/greedy_schedule.hpp"
 #include "graphblas/backend/cuda/kernels/color.cuh"
 
 namespace graphblas {
@@ -22,76 +23,14 @@ Info graphColorRun(Vector<W>* v, const Matrix<a>* A, unsigned int seed, int* nco
                    float* ms = NULL) {
   static_assert(std::is_same<W, int>::value || std::is_same<W, float>::value,
                 "graphColor writes int or float colours");
-  if (!A->isSparse()) {
-    std::cout << "Error: graphColor of a dense matrix is not implemented in this backend\n";
-    return GrB_NOT_IMPLEMENTED;
-  }
-  const SparseMatrix<a>* S = &A->sparse_;
-  const Index n = S->nrows_;
-  if (n != S->ncols_) return GrB_DIMENSION_MISMATCH;
-  Index vsize = 0;
-  CHECK(v->size(&vsize));
-  if (vsize != n) return GrB_DIMENSION_MISMATCH;
-  const bool same_structure = S->symmetric_ || S->d_cscColPtr_ == S->d_csrRowPtr_;
-  const bool stored = n > 0 && S->nvals_ > 0;
-  if (stored && (S->d_csrRowPtr_ == NULL || (!same_structure && S->d_cscColPtr_ == NULL)))
-    return GrB_UNINITIALIZED_OBJECT;
-
-  GpuTimer clock;
-  clock.Start();
-  CHECK(v->setStorage(GrB_DENSE));
-  if (ncolors != NULL) *ncolors = 0;
-  if (!stored) {                       // no edges: every vertex takes colour 1
-    if (n > 0) CHECK(v->fill(static_cast<W>(1)));
-    if (ncolors != NULL && n > 0) *ncolors = 1;
-    clock.Stop();
-    if (ms != NULL) *ms = clock.ElapsedMillis();
-    return GrB_SUCCESS;
-  }
-  CHECK(v->dense_.allocateGpu());
-  cudaStream_t stream = gbStream();
-
-  const size_t words = (static_cast<size_t>(n) + 63)/64*64;     // 256-byte aligned arrays
-  const size_t counters_bytes = 4*sizeof(unsigned long long);     // in the first 256 bytes
-  unsigned char* block = static_cast<unsigned char*>(gbMalloc(
-      256 + 5*words*sizeof(Index)));
-  GcArgs args;
-  args.row_ptr = S->d_csrRowPtr_;  args.row_ind = S->d_csrColInd_;
-  args.col_ptr = same_structure ? NULL : S->d_cscColPtr_;
-  args.col_ind = same_structure ? NULL : S->d_cscRowInd_;
-  args.n = n;
-  args.seed = seed;
-  args.counters   = reinterpret_cast<unsigned long long*>(block);
-  Index* arrays   = reinterpret_cast<Index*>(block + 256);
-  args.colour     = reinterpret_cast<unsigned int*>(arrays);
-  args.waiting_on = arrays + words;
-  args.resume     = arrays + 2*words;
-  args.list[0]    = arrays + 3*words;
-  args.list[1]    = arrays + 4*words;
-  CUDA_CALL(cudaMemsetAsync(block, 0, counters_bytes, stream));
-  CUDA_CALL(cudaMemsetAsync(args.colour, 0, static_cast<size_t>(n)*sizeof(unsigned int),
-                            stream));
-
-  void (*kernel)(GcArgs, W*) = graphColorKernel<W>;
-  static int resident = 0;             // CTAs that fit at once (cooperative launch)
-  if (resident == 0) {
-    int per_sm = 0;
-    CUDA_CALL(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, GB_GC_NT, 0));
-    resident = per_sm*runtime().sm_count;
-    if (resident < 1) { gbFree(block); return GrB_PANIC; }
-  }
-  W* out = v->dense_.d_val_;
-  void* params[] = { &args, &out };
-  CUDA_CALL(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kernel),
-      dim3(resident), dim3(GB_GC_NT), params, 0, stream));
-  GB_KERNEL_CHECK();
-  clock.Stop();
-  v->dense_.touched();
-  if (ncolors != NULL)
-    *ncolors = static_cast<int>(runtime().fetch(args.counters + 3));
-  gbFree(block);
-  if (ms != NULL) *ms = clock.ElapsedMillis();
-  return GrB_SUCCESS;
+  const Info refused = greedyCheck("graphColor", v, A, static_cast<Vector<W>*>(NULL));
+  if (refused != GrB_SUCCESS) return refused;
+  const Index n = A->sparse_.nrows_;
+  return greedyRun<W, graphColorKernel<W>>(v, &A->sparse_, seed, ncolors, ms,
+      [n](unsigned int* colour, cudaStream_t stream) {          // 0 = uncoloured
+        CUDA_CALL(cudaMemsetAsync(colour, 0, static_cast<size_t>(n)*sizeof(unsigned int),
+                                  stream));
+      });
 }
 
 }  // namespace backend

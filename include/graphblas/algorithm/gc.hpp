@@ -4,7 +4,7 @@
 // (i and j conflict when A(i,j) or A(j,i) is stored, i != j; self-loops are ignored).
 // The colouring is sequential greedy first-fit in decreasing priority order, the
 // priority of vertex i being (hash(seed, i), i) with the hash of
-// backend/cuda/kernels/color.cuh, so it depends on seed and A only.  The whole
+// backend/cuda/kernels/greedy_schedule.cuh, so it depends on seed and A only.  The whole
 // colouring is one cooperative kernel (backend/cuda/color.hpp); *ncolors = the
 // largest colour (0 for an empty graph).  A non-symmetric A is read through its CSR
 // and its CSC and needs both on the device.

@@ -4,8 +4,8 @@
 // (i and j conflict when A(i,j) or A(j,i) is stored, i != j; self-loops are ignored).
 // The set is the sequential greedy MIS in decreasing priority order over the
 // candidates: i joins iff no higher-priority candidate neighbour joined, the priority
-// of i being (hash(seed, i), i) with the hash of backend/cuda/kernels/color.cuh, so it
-// depends on A, seed and the candidates only.  With no candidate vector it equals
+// of i being (hash(seed, i), i) with the hash of backend/cuda/kernels/greedy_schedule.cuh,
+// so it depends on A, seed and the candidates only.  With no candidate vector it equals
 // colour class 1 of algorithm::gc with the same seed.  candidates (may be NULL: every
 // vertex) makes vertex i a candidate when it holds a non-zero value for i, in the
 // storage it has; it is never converted and may be v itself.  The whole set is one

@@ -1,6 +1,6 @@
 /* tests/gc_oracle.c — CPU greedy graph colouring, the checker of the device colouring
  * (backend/cuda/kernels/color.cuh).  TEST INFRASTRUCTURE ONLY: tests/, smoke() and
- * tools/bench_gc.py load it (tests/gc_oracle.py); the product never does.
+ * tools/bench_gc.py load it (tests/greedy_oracle.py); the product never does.
  *
  * Ours: the reference's SimpleReferenceGc orders vertices with std::mt19937 and cannot
  * pin a hashed order, so this restatement is pinned by properties instead

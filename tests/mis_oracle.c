@@ -1,6 +1,6 @@
 /* tests/mis_oracle.c — CPU greedy maximal independent set, the checker of the device
  * MIS (backend/cuda/kernels/mis.cuh).  TEST INFRASTRUCTURE ONLY: tests/, smoke() and
- * tools/bench_mis.py load it (tests/mis_oracle.py); the product never does.
+ * tools/bench_mis.py load it (tests/greedy_oracle.py); the product never does.
  *
  * It includes the colouring checker (tests/gc_oracle.c) for its priority hash gc_hash
  * and its decreasing-priority order gc_key_desc, so both checkers sort vertices the

@@ -12,7 +12,7 @@ import os
 import numpy as np
 import pytest
 
-import gc_oracle
+import greedy_oracle
 import oracle_binding as orc
 from test_parity_gpu import make_matrix, path_graph, ragged_graph, star_graph
 
@@ -42,7 +42,7 @@ def check(gb, rp, ci, seeds=(0,), dtype=None):
     A = make_matrix(gb, rp, ci, dtype=dtype)
     for seed in seeds:
         got, ncolors = colour(gb, A, n, seed)
-        want, want_n, _ = gc_oracle.gc(rp, ci, seed)
+        want, want_n, _ = greedy_oracle.gc(rp, ci, seed)
         assert np.array_equal(got, want.astype(np.float32)), seed
         assert ncolors == want_n, seed
     return A
@@ -63,7 +63,7 @@ def test_golden_graphs(gb, name):
     if len(ci) == 0:              # test_sgm holds only self-loops: keep them
         n = len(rp) - 1
         rp, ci = np.arange(n + 1, dtype=np.int32), np.arange(n, dtype=np.int32)
-        assert gc_oracle.gc(rp, ci, 0)[1] == 1
+        assert greedy_oracle.gc(rp, ci, 0)[1] == 1
     check(gb, rp, ci, seeds=(0, 1, 99))
 
 
@@ -95,7 +95,7 @@ def test_clique_with_pendants_needs_several_windows(gb):
         dst.append(k + i)
     rp, ci = symmetric_csr(2*k, src, dst)
     check(gb, rp, ci, seeds=(0, 2))
-    assert gc_oracle.gc(rp, ci, 0)[1] == k
+    assert greedy_oracle.gc(rp, ci, 0)[1] == k
 
 
 def test_complete_bipartite(gb):
@@ -119,10 +119,10 @@ def test_self_loops_are_ignored(gb):
     lrp = np.concatenate([[0], np.cumsum(np.bincount(r, minlength=n))]).astype(np.int32)
     A = make_matrix(gb, lrp, c.astype(np.int32))
     got, ncolors = colour(gb, A, n, 0)
-    want, want_n, _ = gc_oracle.gc(rp, ci, 0)
+    want, want_n, _ = greedy_oracle.gc(rp, ci, 0)
     assert np.array_equal(got, want.astype(np.float32)) and ncolors == want_n
     # the oracle ignores them too
-    assert np.array_equal(gc_oracle.gc(lrp, c, 0)[0], want)
+    assert np.array_equal(greedy_oracle.gc(lrp, c, 0)[0], want)
 
 
 def test_one_vertex(gb):
@@ -137,7 +137,7 @@ def test_one_vertex(gb):
 def test_empty_graph_is_not_constructible_through_the_c_abi(gb):
     """n = 0 colours with 0 colours in C++ (and the oracle); the C ABI has no
     0 x 0 matrix or 0-vector to hand it."""
-    assert gc_oracle.gc(np.zeros(1, np.int32), np.zeros(0, np.int32), 0)[1] == 0
+    assert greedy_oracle.gc(np.zeros(1, np.int32), np.zeros(0, np.int32), 0)[1] == 0
     with pytest.raises(gb.GraphBLASError) as e:
         gb.Matrix(0, 0)
     assert e.value.info == gb.Info.GrB_INVALID_VALUE
@@ -155,10 +155,10 @@ def test_directed_matrix_is_coloured_as_its_symmetrised_pattern(gb):
     A = make_matrix(gb, drp, dci, symmetric=False)
     for seed in (0, 8):
         got, ncolors = colour(gb, A, n, seed)
-        want, want_n, _ = gc_oracle.gc(srp, sci, seed)
+        want, want_n, _ = greedy_oracle.gc(srp, sci, seed)
         assert np.array_equal(got, want.astype(np.float32)) and ncolors == want_n
     # the case tells the two apart: the CSR alone colours differently
-    assert not np.array_equal(gc_oracle.gc(drp, dci, 0)[0], gc_oracle.gc(srp, sci, 0)[0])
+    assert not np.array_equal(greedy_oracle.gc(drp, dci, 0)[0], greedy_oracle.gc(srp, sci, 0)[0])
 
 
 @pytest.mark.parametrize("scale", [16, 18])

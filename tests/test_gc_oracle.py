@@ -15,7 +15,7 @@ import subprocess
 import numpy as np
 import pytest
 
-import gc_oracle
+import greedy_oracle
 import oracle_binding as orc
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -24,7 +24,7 @@ M32 = 0xFFFFFFFF
 
 
 def py_hash(seed, v):
-    """fmix32(v ^ (seed * 0x9E3779B9)), the priority hash of kernels/color.cuh."""
+    """fmix32(v ^ (seed * 0x9E3779B9)), the priority hash of kernels/greedy_schedule.cuh."""
     x = (v ^ (seed*0x9E3779B9)) & M32
     x ^= x >> 16
     x = (x*0x85EBCA6B) & M32
@@ -84,7 +84,7 @@ def graphs():
 @pytest.mark.parametrize("seed", [0, 1, 12345])
 def test_oracle_is_the_greedy_colouring(seed):
     for name, rp, ci in graphs():
-        colors, ncolors, depth = gc_oracle.gc(rp, ci, seed)
+        colors, ncolors, depth = greedy_oracle.gc(rp, ci, seed)
         assert ncolors == colors.max(initial=0), name
         assert 1 <= ncolors <= depth, name         # a colour c needs a chain of c
         check_greedy(rp, ci, colors, seed)
@@ -99,7 +99,7 @@ def test_oracle_equals_the_python_restatement():
         dst = rng.randint(0, n, m).astype(np.int32)
         rp, ci = orc.build_csr(n, src, dst, True)
         seed = int(rng.randint(0, 1 << 31)) if trial % 3 else trial
-        colors, ncolors, _ = gc_oracle.gc(rp, ci, seed)
+        colors, ncolors, _ = greedy_oracle.gc(rp, ci, seed)
         want = py_gc(n, rp.tolist(), ci.tolist(), seed)
         assert colors.tolist() == want, (trial, seed)
         assert ncolors == max(want)
@@ -109,11 +109,11 @@ def test_oracle_ignores_self_loops_and_handles_tiny_graphs():
     # a triangle with a loop on every vertex: colours 1..3, the loops change nothing
     rp = np.array([0, 3, 6, 9], np.int32)
     ci = np.array([0, 1, 2, 0, 1, 2, 0, 1, 2], np.int32)
-    colors, ncolors, depth = gc_oracle.gc(rp, ci, 0)
+    colors, ncolors, depth = greedy_oracle.gc(rp, ci, 0)
     assert sorted(colors.tolist()) == [1, 2, 3] and ncolors == 3 and depth == 3
-    colors, ncolors, depth = gc_oracle.gc(np.zeros(1, np.int32), np.zeros(0, np.int32), 0)
+    colors, ncolors, depth = greedy_oracle.gc(np.zeros(1, np.int32), np.zeros(0, np.int32), 0)
     assert len(colors) == 0 and ncolors == 0 and depth == 0
-    colors, ncolors, depth = gc_oracle.gc(np.zeros(2, np.int32), np.zeros(0, np.int32), 0)
+    colors, ncolors, depth = greedy_oracle.gc(np.zeros(2, np.int32), np.zeros(0, np.int32), 0)
     assert colors.tolist() == [1] and ncolors == 1 and depth == 1
 
 
@@ -122,7 +122,7 @@ def test_oracle_depth_is_the_longest_priority_chain():
     n = 200
     src = np.arange(n - 1, dtype=np.int32)
     rp, ci = orc.build_csr(n, src, src + 1, True)
-    _, ncolors, depth = gc_oracle.gc(rp, ci, 7)
+    _, ncolors, depth = greedy_oracle.gc(rp, ci, 7)
     key = [(py_hash(7, v), v) for v in range(n)]
     rounds = [0]*n
     for v in sorted(range(n), key=lambda v: key[v], reverse=True):

@@ -13,7 +13,7 @@ import os
 import numpy as np
 import pytest
 
-import mis_oracle
+import greedy_oracle
 import oracle_binding as orc
 from test_parity_gpu import make_matrix, path_graph, ragged_graph, star_graph
 
@@ -32,7 +32,7 @@ def gb():
 
 
 def np_hash(seed, v):
-    """The priority hash of kernels/color.cuh over an array of vertices."""
+    """The priority hash of kernels/greedy_schedule.cuh over an array of vertices."""
     x = (np.asarray(v, np.uint64) ^ np.uint64((seed*0x9E3779B9) & 0xFFFFFFFF)) & M32
     x ^= x >> np.uint64(16)
     x = (x*np.uint64(0x85EBCA6B)) & M32
@@ -54,7 +54,7 @@ def check(gb, rp, ci, seeds=(0,), dtype=None):
     A = make_matrix(gb, rp, ci, dtype=dtype)
     for seed in seeds:
         got, k = run_mis(gb, A, n, seed)
-        want, want_k, _ = mis_oracle.mis(rp, ci, seed)
+        want, want_k, _ = greedy_oracle.mis(rp, ci, seed)
         assert np.array_equal(got, want.astype(np.float32)), seed
         assert k == want_k, seed
     return A
@@ -75,7 +75,7 @@ def test_golden_graphs(gb, name):
     if len(ci) == 0:              # test_sgm holds only self-loops: keep them
         n = len(rp) - 1
         rp, ci = np.arange(n + 1, dtype=np.int32), np.arange(n, dtype=np.int32)
-        assert mis_oracle.mis(rp, ci, 0)[1] == n
+        assert greedy_oracle.mis(rp, ci, 0)[1] == n
     check(gb, rp, ci, seeds=(0, 1, 99))
 
 
@@ -85,8 +85,8 @@ def test_star_with_many_leaves(gb):
     150 000 leaves and joins alone."""
     rp, ci = star_graph(150000)
     check(gb, rp, ci, seeds=(0, 5, 845704))
-    assert mis_oracle.mis(rp, ci, 0)[0][0] == 0
-    member, size, _ = mis_oracle.mis(rp, ci, 845704)
+    assert greedy_oracle.mis(rp, ci, 0)[0][0] == 0
+    member, size, _ = greedy_oracle.mis(rp, ci, 845704)
     assert member[0] == 1 and size == 1
 
 
@@ -113,7 +113,7 @@ def test_clique_with_pendants(gb):
         dst.append(k + i)
     rp, ci = symmetric_csr(2*k, src, dst)
     check(gb, rp, ci, seeds=(0, 2))
-    assert mis_oracle.mis(rp, ci, 0)[1] == k
+    assert greedy_oracle.mis(rp, ci, 0)[1] == k
 
 
 def test_complete_bipartite(gb):
@@ -136,9 +136,9 @@ def test_self_loops_are_ignored(gb):
     lrp = np.concatenate([[0], np.cumsum(np.bincount(r, minlength=n))]).astype(np.int32)
     A = make_matrix(gb, lrp, c.astype(np.int32))
     got, k = run_mis(gb, A, n, 0)
-    want, want_k, _ = mis_oracle.mis(rp, ci, 0)
+    want, want_k, _ = greedy_oracle.mis(rp, ci, 0)
     assert np.array_equal(got, want.astype(np.float32)) and k == want_k
-    assert np.array_equal(mis_oracle.mis(lrp, c, 0)[0], want)
+    assert np.array_equal(greedy_oracle.mis(lrp, c, 0)[0], want)
 
 
 def test_one_vertex_and_no_edges(gb):
@@ -171,10 +171,10 @@ def test_directed_matrix_uses_its_symmetrised_pattern(gb):
     A = make_matrix(gb, drp, dci, symmetric=False)
     for seed in (0, 8):
         got, k = run_mis(gb, A, n, seed)
-        want, want_k, _ = mis_oracle.mis(srp, sci, seed)
+        want, want_k, _ = greedy_oracle.mis(srp, sci, seed)
         assert np.array_equal(got, want.astype(np.float32)) and k == want_k
     # the case tells the two apart: the CSR alone gives another set
-    assert not np.array_equal(mis_oracle.mis(drp, dci, 0)[0], mis_oracle.mis(srp, sci, 0)[0])
+    assert not np.array_equal(greedy_oracle.mis(drp, dci, 0)[0], greedy_oracle.mis(srp, sci, 0)[0])
 
 
 @pytest.mark.parametrize("scale", [16, 18])
@@ -195,7 +195,7 @@ def test_path_in_increasing_priority_order(gb):
     n, seed = 20000, 21
     order = np.argsort(np.asarray(np_hash(seed, np.arange(n))), kind="stable")
     rp, ci = symmetric_csr(n, order[:-1], order[1:])
-    _, _, depth = mis_oracle.mis(rp, ci, seed)
+    _, _, depth = greedy_oracle.mis(rp, ci, seed)
     assert depth >= 9000
     check(gb, rp, ci, seeds=(seed,))
 
@@ -214,9 +214,9 @@ def test_dense_candidates(gb):
         c = gb.Vector(n)
         c.build(cand.astype(np.float32))
         got, k = run_mis(gb, A, n, seed, c)
-        want, want_k, _ = mis_oracle.mis(rp, ci, seed, cand)
+        want, want_k, _ = greedy_oracle.mis(rp, ci, seed, cand)
         assert np.array_equal(got, want.astype(np.float32)) and k == want_k, seed
-        assert not np.array_equal(want, mis_oracle.mis(rp, ci, seed)[0])
+        assert not np.array_equal(want, greedy_oracle.mis(rp, ci, seed)[0])
         assert c.getStorage() == gb.Storage.GrB_DENSE
         assert np.array_equal(c.extractTuples(), cand.astype(np.float32))
 
@@ -237,7 +237,7 @@ def test_sparse_candidates(gb):
     cand[ind] = val
     for seed in (0, 2):
         got, k = run_mis(gb, A, n, seed, c)
-        want, want_k, _ = mis_oracle.mis(rp, ci, seed, cand)
+        want, want_k, _ = greedy_oracle.mis(rp, ci, seed, cand)
         assert np.array_equal(got, want.astype(np.float32)) and k == want_k, seed
     assert c.getStorage() == gb.Storage.GrB_SPARSE and c.nvals() == len(ind)
     got_ind, got_val = c.extractTuples(sparse=True)
@@ -273,7 +273,7 @@ def test_candidates_aliased_with_v(gb, storage):
         ind = np.nonzero(cand)[0].astype(np.int32)
         v.build(ind, cand[ind])
     got, k = run_mis(gb, A, n, 5, v, v=v)
-    want, want_k, _ = mis_oracle.mis(rp, ci, 5, cand)
+    want, want_k, _ = greedy_oracle.mis(rp, ci, 5, cand)
     assert np.array_equal(got, want.astype(np.float32)) and k == want_k
 
 

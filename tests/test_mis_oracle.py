@@ -14,8 +14,7 @@ import subprocess
 import numpy as np
 import pytest
 
-import gc_oracle
-import mis_oracle
+import greedy_oracle
 import oracle_binding as orc
 from test_gc_oracle import M32, graphs, py_hash
 
@@ -77,8 +76,8 @@ def random_graph(rng, nmax=60):
 @pytest.mark.parametrize("seed", [0, 1, 12345])
 def test_oracle_is_colour_class_one(seed):
     for name, rp, ci in graphs():
-        member, size, depth = mis_oracle.mis(rp, ci, seed)
-        colors, _, jp_depth = gc_oracle.gc(rp, ci, seed)
+        member, size, depth = greedy_oracle.mis(rp, ci, seed)
+        colors, _, jp_depth = greedy_oracle.gc(rp, ci, seed)
         assert np.array_equal(member, (colors == 1).astype(np.int32)), name
         assert size == int(member.sum()), name
         assert 1 <= depth <= jp_depth, name
@@ -86,8 +85,8 @@ def test_oracle_is_colour_class_one(seed):
     rng = np.random.RandomState(seed & 0xFFFF)
     for _ in range(20):
         _, rp, ci = random_graph(rng)
-        assert np.array_equal(mis_oracle.mis(rp, ci, seed)[0],
-                              (gc_oracle.gc(rp, ci, seed)[0] == 1).astype(np.int32))
+        assert np.array_equal(greedy_oracle.mis(rp, ci, seed)[0],
+                              (greedy_oracle.gc(rp, ci, seed)[0] == 1).astype(np.int32))
 
 
 def test_oracle_equals_the_python_restatement():
@@ -96,7 +95,7 @@ def test_oracle_equals_the_python_restatement():
         n, rp, ci = random_graph(rng)
         seed = int(rng.randint(0, 1 << 31)) if trial % 3 else trial
         cand = None if trial % 2 == 0 else (rng.rand(n) < 0.6).astype(np.int32)
-        member, size, depth = mis_oracle.mis(rp, ci, seed, cand)
+        member, size, depth = greedy_oracle.mis(rp, ci, seed, cand)
         want = py_mis(n, rp.tolist(), ci.tolist(), seed,
                       None if cand is None else cand.tolist())
         assert member.tolist() == want, (trial, seed)
@@ -115,7 +114,7 @@ def test_oracle_depth_is_the_synchronous_luby_round_count():
         n = len(rp) - 1
         seed = trial*7 + 1
         cand = None if trial % 3 else (rng.rand(n) < 0.7).astype(np.int32)
-        member, _, depth = mis_oracle.mis(rp, ci, seed, cand)
+        member, _, depth = greedy_oracle.mis(rp, ci, seed, cand)
         want, rounds = py_luby_rounds(n, rp.tolist(), ci.tolist(), seed,
                                       None if cand is None else cand.tolist())
         assert member.tolist() == want, trial
@@ -125,20 +124,20 @@ def test_oracle_depth_is_the_synchronous_luby_round_count():
 def test_oracle_candidates_and_tiny_graphs():
     rp, ci = graphs()[0][1:]
     n = len(rp) - 1
-    member, size, depth = mis_oracle.mis(rp, ci, 0, np.zeros(n, np.int32))
+    member, size, depth = greedy_oracle.mis(rp, ci, 0, np.zeros(n, np.int32))
     assert size == 0 and depth == 0 and not member.any()
     # every vertex a candidate is the same as no candidate vector
-    assert np.array_equal(mis_oracle.mis(rp, ci, 3, np.full(n, 2.5))[0],
-                          mis_oracle.mis(rp, ci, 3)[0])
+    assert np.array_equal(greedy_oracle.mis(rp, ci, 3, np.full(n, 2.5))[0],
+                          greedy_oracle.mis(rp, ci, 3)[0])
     # a triangle with loops: one member; no edges: every candidate
     rp3 = np.array([0, 3, 6, 9], np.int32)
     ci3 = np.array([0, 1, 2, 0, 1, 2, 0, 1, 2], np.int32)
-    member, size, depth = mis_oracle.mis(rp3, ci3, 0)
+    member, size, depth = greedy_oracle.mis(rp3, ci3, 0)
     assert size == 1 and depth == 1
-    member, size, depth = mis_oracle.mis(np.zeros(6, np.int32), np.zeros(0, np.int32), 0,
+    member, size, depth = greedy_oracle.mis(np.zeros(6, np.int32), np.zeros(0, np.int32), 0,
                                         np.array([1, 0, 1, 1, 0]))
     assert member.tolist() == [1, 0, 1, 1, 0] and size == 3 and depth == 1
-    member, size, depth = mis_oracle.mis(np.zeros(1, np.int32), np.zeros(0, np.int32), 0)
+    member, size, depth = greedy_oracle.mis(np.zeros(1, np.int32), np.zeros(0, np.int32), 0)
     assert len(member) == 0 and size == 0 and depth == 0
 
 

@@ -33,7 +33,7 @@ sys.path.insert(0, os.path.join(os.path.dirname(HERE), "tests"))
 from bench_mxm import card, timed                 # noqa: E402
 import graphblast_b200 as gb                      # noqa: E402
 from graphblast_b200 import algorithm, graphs     # noqa: E402
-import gc_oracle                                  # noqa: E402
+import greedy_oracle                              # noqa: E402
 import oracle_binding as orc                      # noqa: E402
 
 
@@ -108,7 +108,7 @@ def measure(scale, args):
 
     h_rp, h_ci = rp.cpu().numpy(), ci.cpu().numpy()
     t0 = time.perf_counter()
-    want, want_n, depth = gc_oracle.gc(h_rp, h_ci, 0)
+    want, want_n, depth = greedy_oracle.gc(h_rp, h_ci, 0)
     rec["cpu_ms"] = (time.perf_counter() - t0)*1e3
     rec["jp_depth"] = depth
     rec["oracle_ncolors"] = want_n

@@ -32,7 +32,7 @@ sys.path.insert(0, os.path.join(os.path.dirname(HERE), "tests"))
 from bench_mxm import card                        # noqa: E402
 import graphblast_b200 as gb                      # noqa: E402
 from graphblast_b200 import algorithm, graphs     # noqa: E402
-import mis_oracle                                 # noqa: E402
+import greedy_oracle                              # noqa: E402
 
 
 def median_ms(fn, iters, warmup):
@@ -69,7 +69,7 @@ def measure(scale, args):
 
     h_rp, h_ci = rp.cpu().numpy(), ci.cpu().numpy()
     t0 = time.perf_counter()
-    want, want_size, depth = mis_oracle.mis(h_rp, h_ci, 0)
+    want, want_size, depth = greedy_oracle.mis(h_rp, h_ci, 0)
     rec["cpu_ms"] = (time.perf_counter() - t0)*1e3
     rec["luby_depth"] = depth
     rec["oracle_size"] = want_size
