@@ -102,6 +102,7 @@ SIGNATURES = [
     ("gb200_pr", _I, [_P, _P, _F, _F, _P, C.POINTER(_F)]),
     ("gb200_gc", _I, [_P, _P, _I, _P, C.POINTER(_I), C.POINTER(_F)]),
     ("gb200_mis", _I, [_P, _P, _I, _P, _P, C.POINTER(_I), C.POINTER(_F)]),
+    ("gb200_cc", _I, [_P, _P, _P, C.POINTER(_I), C.POINTER(_F)]),
     ("gb200_tc", _I, [C.POINTER(_LL), _P, _P, _P, C.POINTER(_F)]),
     ("gb200_rmat_edges", _I, [_I, _LL, _ULL, _LL, _P, _P]),
     ("gb200_vector_export_bits", _I, [_P, _P, C.POINTER(_LL)]),

@@ -1,9 +1,10 @@
 """graphblas::algorithm — the GraphBLAS algorithm drivers of the reference
 (graphblas/algorithm/{bfs,sssp,pr,tc}.hpp), executed inside the native library as
 loops of backend operations (include/graphblas/algorithm/*.hpp), and the graph
-colouring gc and the maximal independent set mis, one kernel each on the device.
+colouring gc, the maximal independent set mis and the connected components cc, one
+kernel each on the device.
 
-sssp, pr, tc, gc and mis return the device time of the operation loop in milliseconds
+sssp, pr, tc, gc, mis and cc return the device time of the operation loop in milliseconds
 ("tight" in the reference drivers, example/gbfs.cu:110-115).  bfs returns it only
 when called with timed=True; otherwise it returns None and, when the traversal runs
 as the fused kernel, only enqueues it, so that back-to-back traversals keep the GPU
@@ -79,4 +80,19 @@ def mis(v, A, seed, desc, candidates=None):
                                  candidates._h if candidates is not None else None,
                                  desc._h, C.byref(k), C.byref(ms)),
            "algorithm::mis")
+    return k.value, ms.value
+
+
+def cc(v, A, desc):
+    """v[i] = the smallest vertex id in the connected component of i in the undirected
+    graph of A's pattern (i and j joined when A(i,j) or A(j,i) is stored; self-loops
+    ignored), one cooperative union-find kernel (include/graphblas/algorithm/cc.hpp).
+    The result depends only on A's pattern, so there is no seed.  A is FP32 or INT32;
+    only its CSR is read.  v becomes dense and is overwritten.  A float v holds ids
+    exactly only up to 2^24, so nrows(A) > 2^24 + 1 raises GrB_INVALID_VALUE.
+    Returns (ncomponents, tight_ms)."""
+    ms = C.c_float(0)
+    k = C.c_int(0)
+    _check(_lib.load().gb200_cc(v._h, A._h, desc._h, C.byref(k), C.byref(ms)),
+           "algorithm::cc")
     return k.value, ms.value

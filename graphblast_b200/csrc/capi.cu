@@ -26,6 +26,7 @@
 #include "graphblas/algorithm/tc.hpp"
 #include "graphblas/algorithm/gc.hpp"
 #include "graphblas/algorithm/mis.hpp"
+#include "graphblas/algorithm/cc.hpp"
 
 #include "graphblast_b200.h"
 
@@ -1116,6 +1117,23 @@ int gb200_mis(gb200_vector_t v, gb200_matrix_t A, int seed, gb200_vector_t candi
       : graphblas::algorithm::mis(v->f, A->i, seed, &desc->desc, &count, cand);
   if (ms < 0.f) return rc(graphblas::algorithm::lastStatus());
   if (nmembers) *nmembers = count;
+  if (tight_ms) *tight_ms = ms;
+  return 0;
+}
+
+int gb200_cc(gb200_vector_t v, gb200_matrix_t A, gb200_desc_t desc, int* ncomponents,
+             float* tight_ms) {
+  if (v == NULL || A == NULL || desc == NULL)
+    return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
+  if (A->f == NULL && A->i == NULL) return rc(graphblas::GrB_DOMAIN_MISMATCH);
+  GB200_REQUIRE_DEVICE();
+  int count = 0;
+  graphblas::algorithm::lastStatus() = graphblas::GrB_SUCCESS;
+  const float ms = A->f != NULL
+      ? graphblas::algorithm::cc(v->f, A->f, &desc->desc, &count)
+      : graphblas::algorithm::cc(v->f, A->i, &desc->desc, &count);
+  if (ms < 0.f) return rc(graphblas::algorithm::lastStatus());
+  if (ncomponents) *ncomponents = count;
   if (tight_ms) *tight_ms = ms;
   return 0;
 }

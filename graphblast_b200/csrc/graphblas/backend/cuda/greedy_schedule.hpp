@@ -93,13 +93,8 @@ Info greedyRun(Vector<W>* v, const SparseMatrix<a>* S, unsigned int seed, int* c
 
   CHECK(v->setStorage(GrB_DENSE));
   CHECK(v->dense_.allocateGpu());
-  static int resident = 0;             // CTAs of K that fit at once (cooperative launch)
-  if (resident == 0) {
-    int per_sm = 0;
-    CUDA_CALL(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, K, GB_GC_NT, 0));
-    resident = per_sm*runtime().sm_count;
-    if (resident < 1) { gbFree(block); return GrB_PANIC; }
-  }
+  const int resident = cooperativeGrid<K, GB_GC_NT>();
+  if (resident < 1) { gbFree(block); return GrB_PANIC; }
   W* out = v->dense_.d_val_;
   void* params[] = { &args, &out };
   CUDA_CALL(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(K),

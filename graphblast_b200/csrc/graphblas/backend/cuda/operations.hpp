@@ -40,6 +40,7 @@
 #include "graphblas/backend/cuda/tri.hpp"
 #include "graphblas/backend/cuda/color.hpp"
 #include "graphblas/backend/cuda/mis.hpp"
+#include "graphblas/backend/cuda/cc.hpp"
 
 namespace graphblas {
 namespace backend {

@@ -246,6 +246,20 @@ inline void gbFree(void* p) {
   if (p != NULL) (void)cudaFreeAsync(p, runtime().stream);
 }
 
+// CTAs of NT threads of the cooperative kernel K that fit on the device at once: the
+// grid of its cooperative launch.  The occupancy query runs on the first call and is
+// cached per kernel; 0 when no CTA fits.
+template <auto K, int NT>
+int cooperativeGrid() {
+  static int resident = 0;
+  if (resident == 0) {
+    int per_sm = 0;
+    CUDA_CALL(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, K, NT, 0));
+    resident = per_sm*runtime().sm_count;
+  }
+  return resident;
+}
+
 // Grid sizing helper: a grid-stride launch sized in whole waves of the SM count.
 inline int gridFor(size_t work_items, int threads, int ctas_per_sm = 8) {
   size_t want = (work_items + threads - 1) / threads;

@@ -314,6 +314,15 @@ int gb200_gc(gb200_vector_t v, gb200_matrix_t A, int seed, gb200_desc_t desc,
  * It is never converted and may be v itself.  include/graphblas/algorithm/mis.hpp */
 int gb200_mis(gb200_vector_t v, gb200_matrix_t A, int seed, gb200_vector_t candidates,
               gb200_desc_t desc, int* nmembers, float* tight_ms);
+/* Connected components of the undirected graph of A's pattern (FP32 or INT32 A; only
+ * its CSR is read, so a non-symmetric A needs no CSC): v[i] = the smallest vertex id in
+ * the component of i; *ncomponents = the number of components.  i and j are joined
+ * when A(i,j) or A(j,i) is stored; self-loops are ignored.  The result depends only on
+ * A's pattern.  v becomes dense and is overwritten completely.  nrows(A) > 2^24 + 1 is
+ * refused with GrB_INVALID_VALUE: a float holds ids exactly only up to 2^24.
+ * include/graphblas/algorithm/cc.hpp */
+int gb200_cc(gb200_vector_t v, gb200_matrix_t A, gb200_desc_t desc, int* ncomponents,
+             float* tight_ms);
 int gb200_pr(gb200_vector_t p, gb200_matrix_t A, float alpha, float eps,
              gb200_desc_t desc, float* tight_ms);               /* algorithm/pr.hpp:15-94 */
 int gb200_tc(long long* ntris, gb200_matrix_t A, gb200_matrix_t B,
