@@ -74,9 +74,8 @@ Info bfsFused(Vector<float>* v, const Matrix<a>* A, Index s, Descriptor* desc, i
   // in a directed graph one that points somewhere would let the pull discover what
   // it points at.  When the pulled structure is the pushed one, that is the same
   // bitmap; otherwise the pushed structure's empty rows are ANDed in.
-  const bool same_structure = S->symmetric_ || S->d_cscColPtr_ == S->d_csrRowPtr_;
   args.pull_empty = pullEmptyRowBits(probe, n);
-  args.push_empty = same_structure ? NULL : pullEmptyRowBits(
+  args.push_empty = S->sameStructure() ? NULL : pullEmptyRowBits(
       pullFirstNeighbours(S, 0, S->d_csrRowPtr_, S->d_csrColInd_, n), n);
   args.n = n;
   args.source = s;

@@ -66,7 +66,7 @@ Info ccRun(Vector<W>* v, const Matrix<a>* A, int* ncomponents, float* ms = NULL)
   args.n = n;
   args.row_ptr = stored ? S->d_csrRowPtr_ : NULL;
   args.row_ind = stored ? S->d_csrColInd_ : NULL;
-  args.skip = (S->symmetric_ || S->d_cscColPtr_ == S->d_csrRowPtr_) ? 1 : 0;
+  args.skip = S->sameStructure() ? 1 : 0;
   args.counters = reinterpret_cast<unsigned long long*>(block);
   args.parent = reinterpret_cast<Index*>(block + 256);
   args.queued = args.parent + n;

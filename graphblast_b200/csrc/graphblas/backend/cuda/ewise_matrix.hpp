@@ -26,38 +26,6 @@
 namespace graphblas {
 namespace backend {
 
-// C's arrays replaced by (rowptr, colind, val) of nnz entries, stream-ordered
-// after every kernel queued so far (which may still read C's old arrays through
-// an aliased operand).  The CSC, when C's format keeps one, is the one given or,
-// with cscptr == NULL, built here.
-template <typename c>
-void swapInCsr(SparseMatrix<c>* C, Index nnz, Index* rowptr, Index* colind, c* val,
-               Index* cscptr = NULL, Index* cscind = NULL, c* cscval = NULL) {
-  const bool want_csc = C->format_ == GrB_SPARSE_MATRIX_CSRCSC;
-  if (want_csc && cscptr == NULL)
-    ingestCsrToCsc<c>(C->nrows_, C->ncols_, nnz, rowptr, colind, val,
-        &cscptr, &cscind, &cscval);
-  if (!want_csc && cscptr != NULL) { gbFree(cscptr); gbFree(cscind); gbFree(cscval); }
-  C->clear();
-  C->d_csrRowPtr_ = rowptr;
-  C->d_csrColInd_ = colind;
-  C->d_csrVal_ = val;
-  C->csr_ownership_ = true;
-  C->nvals_ = nnz;
-  C->ncapacity_ = nnz;
-  C->symmetric_ = false;
-  if (want_csc) {
-    C->d_cscColPtr_ = cscptr;
-    C->d_cscRowInd_ = cscind;
-    C->d_cscVal_ = cscval;
-    C->csc_ownership_ = true;
-    C->cscval_ownership_ = true;
-    C->csc_initialized_ = true;
-  }
-  C->csr_initialized_ = true;
-  C->need_update_ = true;
-}
-
 template <bool IsAdd, typename c, typename a, typename b, typename SemiringT>
 Info ewiseMatrix(SparseMatrix<c>* C, SemiringT op, const SparseMatrix<a>* A,
                  const SparseMatrix<b>* B, Descriptor* desc) {
@@ -67,21 +35,14 @@ Info ewiseMatrix(SparseMatrix<c>* C, SemiringT op, const SparseMatrix<a>* A,
   const bool use_tran_A = inp0_mode == GrB_TRAN;
   const bool use_tran_B = inp1_mode == GrB_TRAN;
 
-  const Index* A_ptr = use_tran_A ? A->d_cscColPtr_ : A->d_csrRowPtr_;
-  const Index* A_ind = use_tran_A ? A->d_cscRowInd_ : A->d_csrColInd_;
-  const a*     A_val = use_tran_A ? A->d_cscVal_    : A->d_csrVal_;
-  const Index* B_ptr = use_tran_B ? B->d_cscColPtr_ : B->d_csrRowPtr_;
-  const Index* B_ind = use_tran_B ? B->d_cscRowInd_ : B->d_csrColInd_;
-  const b*     B_val = use_tran_B ? B->d_cscVal_    : B->d_csrVal_;
+  const typename SparseMatrix<a>::View Av = A->view(use_tran_A);
+  const typename SparseMatrix<b>::View Bv = B->view(use_tran_B);
   // the frontend checks the shapes of op(A), op(B) and C; they are checked again
   // for callers that reach the backend through the reference's frontend
   const Index m = C->nrows_, n = C->ncols_;
-  if ((use_tran_A ? A->ncols_ : A->nrows_) != m || (use_tran_A ? A->nrows_ : A->ncols_) != n ||
-      (use_tran_B ? B->ncols_ : B->nrows_) != m || (use_tran_B ? B->nrows_ : B->ncols_) != n)
+  if (Av.dim != m || Av.other != n || Bv.dim != m || Bv.other != n)
     return GrB_DIMENSION_MISMATCH;
-  if (A_ptr == NULL || A_ind == NULL || A_val == NULL ||
-      B_ptr == NULL || B_ind == NULL || B_val == NULL)
-    return GrB_UNINITIALIZED_OBJECT;
+  if (!Av.complete() || !Bv.complete()) return GrB_UNINITIALIZED_OBJECT;
 
   cudaStream_t s = gbStream();
   const long long total = static_cast<long long>(A->nvals_) + B->nvals_;
@@ -100,7 +61,7 @@ Info ewiseMatrix(SparseMatrix<c>* C, SemiringT op, const SparseMatrix<a>* A,
   // 1. count: entries of C per tile, per row and in all
   if (ntiles > 0) {
     ewiseMatrixCountKernel<IsAdd><<<static_cast<unsigned int>(ntiles), GB_EWM_NT, 0, s>>>(
-        A_ptr, A_ind, B_ptr, B_ind, m, total, tiles, rowptr, count);
+        Av.ptr, Av.ind, Bv.ptr, Bv.ind, m, total, tiles, rowptr, count);
     GB_KERNEL_CHECK();
   }
   const unsigned long long nnz64 = runtime().fetch(count);
@@ -119,11 +80,11 @@ Info ewiseMatrix(SparseMatrix<c>* C, SemiringT op, const SparseMatrix<a>* A,
   if (ntiles > 0) {
     scanExclusiveAsync(tiles, ntiles, NULL);
     ewiseMatrixFillKernel<IsAdd, c><<<static_cast<unsigned int>(ntiles), GB_EWM_NT, 0, s>>>(
-        A_ptr, A_ind, A_val, B_ptr, B_ind, B_val, m, total, tiles, colind, val,
+        Av.ptr, Av.ind, Av.val, Bv.ptr, Bv.ind, Bv.val, m, total, tiles, colind, val,
         extractMul(op), extractAdd(op));
     GB_KERNEL_CHECK();
   }
-  swapInCsr(C, nnz, rowptr, colind, val);
+  C->replaceDevice(nnz, rowptr, colind, val);
   return GrB_SUCCESS;
 }
 
@@ -176,8 +137,8 @@ Info transposeSparse(SparseMatrix<c>* C, const SparseMatrix<a>* A, bool transpos
             A->d_csrVal_, &csc[0], &csc[1], &csc_val);
       }
     }
-    if (transpose_a) swapInCsr(C, nnz, csr[0], csr[1], csr_val, csc[0], csc[1], csc_val);
-    else             swapInCsr(C, nnz, csc[0], csc[1], csc_val, csr[0], csr[1], csr_val);
+    if (transpose_a) C->replaceDevice(nnz, csr[0], csr[1], csr_val, csc[0], csc[1], csc_val);
+    else             C->replaceDevice(nnz, csc[0], csc[1], csc_val, csr[0], csr[1], csr_val);
     return GrB_SUCCESS;
   }
 }

@@ -31,9 +31,8 @@ Info greedyCheck(const char* what, Vector<W>* v, const Matrix<a>* A, Vector<W>* 
     CHECK(cand->size(&csize));
     if (csize != n) return GrB_DIMENSION_MISMATCH;
   }
-  const bool same_structure = S->symmetric_ || S->d_cscColPtr_ == S->d_csrRowPtr_;
   if (n > 0 && S->nvals_ > 0 &&
-      (S->d_csrRowPtr_ == NULL || (!same_structure && S->d_cscColPtr_ == NULL)))
+      (S->d_csrRowPtr_ == NULL || (!S->sameStructure() && S->d_cscColPtr_ == NULL)))
     return GrB_UNINITIALIZED_OBJECT;
   return GrB_SUCCESS;
 }
@@ -60,7 +59,7 @@ Info greedyRun(Vector<W>* v, const SparseMatrix<a>* S, unsigned int seed, int* c
   }
   cudaStream_t stream = gbStream();
   const bool stored = S->nvals_ > 0;
-  const bool same_structure = S->symmetric_ || S->d_cscColPtr_ == S->d_csrRowPtr_;
+  const bool same_structure = S->sameStructure();
 
   const size_t words = (static_cast<size_t>(n) + 63)/64*64;      // 256-byte aligned arrays
   const size_t rp_words = stored ? 0 : (static_cast<size_t>(n) + 64)/64*64;

@@ -9,56 +9,45 @@
 namespace graphblas {
 namespace backend {
 
-// first[i] as pullFirstNeighbourKernel defines it; the empty-row bitmap follows the
-// array (pullEmptyRowBits).  side: 0 = the CSR arrays are pulled, 1 = the CSC arrays.
+// One summary of nrows + 1 words with the bitmap of empty rows behind it
+// (pullEmptyRowBits), cached in `slot` under the pointer array and entry count it is
+// built from: fill(out) launches the kernel that writes the words.
+template <typename Fill>
+const Index* pullSummary(DerivedArray* slot, const Index* ptr, Index nvals, Index nrows,
+                         Fill fill) {
+  if (!slot->validFor(ptr, nvals)) {
+    const size_t nwords = (static_cast<size_t>(nrows) + 31)/32;
+    Index* out = slot->rebuild(static_cast<size_t>(nrows) + 1 + nwords, ptr, nvals);
+    fill(out);
+    GB_KERNEL_CHECK();
+    pullEmptyRowBitsKernel<<<gridFor(nrows, 256, 8), 256, 0, gbStream()>>>(
+        reinterpret_cast<unsigned int*>(out + nrows + 1), out, nrows);
+    GB_KERNEL_CHECK();
+  }
+  return slot->d;
+}
+
+// first[i] as pullFirstNeighbourKernel defines it.  side: 0 = the CSR arrays are
+// pulled, 1 = the CSC arrays.
 template <typename T>
 const Index* pullFirstNeighbours(SparseMatrix<T>* S, int side, const Index* ptr,
                                  const Index* ind, Index nrows) {
-  if (S->d_pull_first_[side] == NULL || S->pull_first_key_[side] != ptr ||
-      S->pull_first_nvals_[side] != S->nvals_) {
-    if (S->d_pull_first_[side] != NULL) gbFree(S->d_pull_first_[side]);
-    const size_t nwords = (static_cast<size_t>(nrows) + 31)/32;
-    S->d_pull_first_[side] = reinterpret_cast<Index*>(
-        gbMalloc((static_cast<size_t>(nrows) + 1 + nwords)*sizeof(Index)));
-    cudaStream_t s = gbStream();
-    pullFirstNeighbourKernel<<<gridFor(nrows, 256, 8), 256, 0, s>>>(
-        S->d_pull_first_[side], ptr, ind, nrows);
-    GB_KERNEL_CHECK();
-    pullEmptyRowBitsKernel<<<gridFor(nrows, 256, 8), 256, 0, s>>>(
-        reinterpret_cast<unsigned int*>(S->d_pull_first_[side] + nrows + 1),
-        S->d_pull_first_[side], nrows);
-    GB_KERNEL_CHECK();
-    S->pull_first_key_[side] = ptr;
-    S->pull_first_nvals_[side] = S->nvals_;
-  }
-  return S->d_pull_first_[side];
+  return pullSummary(&S->pull_first_[side], ptr, S->nvals_, nrows, [&](Index* out) {
+    pullFirstNeighbourKernel<<<gridFor(nrows, 256, 8), 256, 0, gbStream()>>>(
+        out, ptr, ind, nrows);
+  });
 }
 
 // probe[i] as pullMaxDegreeNeighbourKernel defines it (the fused BFS probes it: the
-// highest-degree neighbour is the one most likely to be visited), the empty-row
-// bitmap following it as above.  Cached beside the first-neighbour summary, under
-// the same key.
+// highest-degree neighbour is the one most likely to be visited).  Cached beside the
+// first-neighbour summary, under the same key.
 template <typename T>
 const Index* pullMaxDegreeNeighbours(SparseMatrix<T>* S, int side, const Index* ptr,
                                      const Index* ind, Index nrows) {
-  if (S->d_pull_maxdeg_[side] == NULL || S->pull_maxdeg_key_[side] != ptr ||
-      S->pull_maxdeg_nvals_[side] != S->nvals_) {
-    if (S->d_pull_maxdeg_[side] != NULL) gbFree(S->d_pull_maxdeg_[side]);
-    const size_t nwords = (static_cast<size_t>(nrows) + 31)/32;
-    S->d_pull_maxdeg_[side] = reinterpret_cast<Index*>(
-        gbMalloc((static_cast<size_t>(nrows) + 1 + nwords)*sizeof(Index)));
-    cudaStream_t s = gbStream();
+  return pullSummary(&S->pull_maxdeg_[side], ptr, S->nvals_, nrows, [&](Index* out) {
     pullMaxDegreeNeighbourKernel<<<gridFor(static_cast<size_t>(nrows)*32, 256, 8), 256, 0,
-                                   s>>>(S->d_pull_maxdeg_[side], ptr, ind, nrows);
-    GB_KERNEL_CHECK();
-    pullEmptyRowBitsKernel<<<gridFor(nrows, 256, 8), 256, 0, s>>>(
-        reinterpret_cast<unsigned int*>(S->d_pull_maxdeg_[side] + nrows + 1),
-        S->d_pull_maxdeg_[side], nrows);
-    GB_KERNEL_CHECK();
-    S->pull_maxdeg_key_[side] = ptr;
-    S->pull_maxdeg_nvals_[side] = S->nvals_;
-  }
-  return S->d_pull_maxdeg_[side];
+                                   gbStream()>>>(out, ptr, ind, nrows);
+  });
 }
 
 inline const unsigned int* pullEmptyRowBits(const Index* first, Index nrows) {

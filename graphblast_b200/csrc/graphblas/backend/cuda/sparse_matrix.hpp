@@ -53,6 +53,30 @@ struct MatrixCacheHeader {
   int32_t  value_bytes;     // sizeof(T) when values follow, 0 for a pattern
 };
 
+// Device words derived from one orientation's arrays, valid for the pointer array
+// and entry count (the merge-path tiles: also the tile count) they were computed
+// from.  Every structural change releases them; the key catches a path that forgot.
+struct DerivedArray {
+  Index*       d = NULL;
+  const Index* key = NULL;
+  Index        nvals = -1;
+  int          count = 0;
+  bool validFor(const Index* k, Index nv, int n = 0) const {
+    return d != NULL && key == k && nvals == nv && count == n;
+  }
+  // Frees what is held, allocates `words` words and stamps the key; the caller fills d.
+  Index* rebuild(size_t words, const Index* k, Index nv, int n = 0) {
+    release();
+    d = reinterpret_cast<Index*>(gbMalloc(words*sizeof(Index)));
+    key = k; nvals = nv; count = n;
+    return d;
+  }
+  void release() {
+    if (d != NULL) gbFree(d);
+    *this = DerivedArray();
+  }
+};
+
 inline bool cacheFileExists(const char* path) {
   FILE* f = fopen(path, "rb");
   if (f == NULL) return false;
@@ -70,6 +94,17 @@ class SparseMatrix {
     Index*& ind;
     T*&     val;
     Index   dim;
+  };
+  // One stored orientation of the device side, read-only: the three arrays an
+  // operation traverses as op(A), with the dimensions that go with them.
+  struct View {
+    const Index* ptr;
+    const Index* ind;
+    const T*     val;
+    Index        dim;       // rows of this orientation (ptr has dim + 1 entries)
+    Index        other;     // its columns
+    int          which;     // 0 = CSR, 1 = CSC: the slot of the derived caches
+    bool complete() const { return ptr != NULL && ind != NULL && val != NULL; }
   };
 
   SparseMatrix() { reset(0, 0); }
@@ -125,7 +160,11 @@ class SparseMatrix {
   Info syncCpu();            // host CSC rebuilt from the host CSR
   Info printCSR(const char* str) { return printSide(str, hostCsr(), ncols_); }
   Info printCSC(const char* str) { return printSide(str, hostCsc(), nrows_); }
-  void dropSpmvTiles();
+  void dropDerived();
+  // The contents replaced by a computed CSR of nnz entries in fresh arrays, which
+  // this object takes (with cscptr != NULL, a ready CSC of the same entries too).
+  void replaceDevice(Index nnz, Index* rowptr, Index* colind, T* val,
+      Index* cscptr = NULL, Index* cscind = NULL, T* cscval = NULL);
   // The entry set stopped being symmetric (tril): from the next upload on the
   // column-major side owns its index arrays instead of borrowing the CSR's.
   void dropSymmetry() { if (symmetric_) { releaseDevice(); symmetric_ = false; } }
@@ -134,6 +173,12 @@ class SparseMatrix {
   Side hostCsc() { return Side{h_cscColPtr_, h_cscRowInd_, h_cscVal_, ncols_}; }
   Side devCsr()  { return Side{d_csrRowPtr_, d_csrColInd_, d_csrVal_, nrows_}; }
   Side devCsc()  { return Side{d_cscColPtr_, d_cscRowInd_, d_cscVal_, ncols_}; }
+  View view(bool csc) const {
+    return csc ? View{d_cscColPtr_, d_cscRowInd_, d_cscVal_, ncols_, nrows_, 1}
+               : View{d_csrRowPtr_, d_csrColInd_, d_csrVal_, nrows_, ncols_, 0};
+  }
+  // Both orientations have the same structure: one pass over either serves for both.
+  bool sameStructure() const { return symmetric_ || d_cscColPtr_ == d_csrRowPtr_; }
 
   Index nrows_;
   Index ncols_;
@@ -171,18 +216,11 @@ class SparseMatrix {
   //   highest-degree-neighbour summary of the fused BFS pull,
   //   hub index of the hub-cached pull SpMV (hub_state_: 0 not built, 1 in use,
   //   2 rejected because too few entries reference the hub columns).
-  Index*       d_spmv_tiles_[2];
-  const Index* spmv_tiles_key_[2];
-  Index        spmv_tiles_nvals_[2];
-  int          spmv_tiles_count_[2];
-  Index*       d_pull_first_[2];
-  const Index* pull_first_key_[2];
-  Index        pull_first_nvals_[2];
-  Index*       d_pull_maxdeg_[2];
-  const Index* pull_maxdeg_key_[2];
-  Index        pull_maxdeg_nvals_[2];
+  DerivedArray tiles_[2];
+  DerivedArray pull_first_[2];
+  DerivedArray pull_maxdeg_[2];
   HubIndex     hub_[2];
-  int          hub_state_[2];
+  int          hub_state_[2] = {0, 0};
 
  private:
   void reset(Index nrows, Index ncols);
@@ -226,27 +264,16 @@ void SparseMatrix<T>::reset(Index nrows, Index ncols) {
   csr_ownership_ = false; csc_ownership_ = false; cscval_ownership_ = false;
   symmetric_ = false;
   format_ = getEnv("GRB_SPARSE_MATRIX_FORMAT", GrB_SPARSE_MATRIX_CSRCSC);
-  for (int k = 0; k < 2; ++k) {
-    d_spmv_tiles_[k] = NULL; spmv_tiles_key_[k] = NULL;
-    spmv_tiles_nvals_[k] = -1; spmv_tiles_count_[k] = 0;
-    d_pull_first_[k] = NULL; pull_first_key_[k] = NULL; pull_first_nvals_[k] = -1;
-    d_pull_maxdeg_[k] = NULL; pull_maxdeg_key_[k] = NULL; pull_maxdeg_nvals_[k] = -1;
-    hub_state_[k] = 0;
-  }
 }
 
 template <typename T>
-void SparseMatrix<T>::dropSpmvTiles() {
+void SparseMatrix<T>::dropDerived() {
   for (int k = 0; k < 2; ++k) {
     hub_[k].release();
     hub_state_[k] = 0;
-    if (d_pull_first_[k] != NULL) gbFree(d_pull_first_[k]);
-    d_pull_first_[k] = NULL; pull_first_key_[k] = NULL; pull_first_nvals_[k] = -1;
-    if (d_pull_maxdeg_[k] != NULL) gbFree(d_pull_maxdeg_[k]);
-    d_pull_maxdeg_[k] = NULL; pull_maxdeg_key_[k] = NULL; pull_maxdeg_nvals_[k] = -1;
-    if (d_spmv_tiles_[k] != NULL) gbFree(d_spmv_tiles_[k]);
-    d_spmv_tiles_[k] = NULL; spmv_tiles_key_[k] = NULL;
-    spmv_tiles_nvals_[k] = -1; spmv_tiles_count_[k] = 0;
+    pull_first_[k].release();
+    pull_maxdeg_[k].release();
+    tiles_[k].release();
   }
 }
 
@@ -261,7 +288,7 @@ void SparseMatrix<T>::releaseHost() {
 
 template <typename T>
 void SparseMatrix<T>::releaseDevice() {
-  dropSpmvTiles();
+  dropDerived();
   if (csc_ownership_) {
     if (d_cscColPtr_ != d_csrRowPtr_) gbFree(d_cscColPtr_);
     if (d_cscRowInd_ != d_csrColInd_) gbFree(d_cscRowInd_);
@@ -293,7 +320,7 @@ Info SparseMatrix<T>::dup(const SparseMatrix* rhs) {
   const bool reusable = csr_ownership_ && nvals_ == rhs->nvals_ &&
                         symmetric_ == rhs->symmetric_ && format_ == rhs->format_;
   if (!reusable) { releaseDevice(); releaseHost(); }
-  dropSpmvTiles();
+  dropDerived();
   nvals_     = rhs->nvals_;
   symmetric_ = rhs->symmetric_;
   format_    = rhs->format_;
@@ -308,6 +335,38 @@ Info SparseMatrix<T>::dup(const SparseMatrix* rhs) {
   need_update_ = true;
   csr_initialized_ = true;
   return GrB_SUCCESS;
+}
+
+// The old arrays, and every cache built on them, go first: stream-ordered after the
+// kernels queued so far, which may still read them through an operand that is this
+// matrix.  Then the CSC, when the format keeps one, is the one given or is built
+// here; a given one is freed when the format is CSR-only.  Nothing is known about
+// the result's symmetry, and the host mirrors follow lazily.
+template <typename T>
+void SparseMatrix<T>::replaceDevice(Index nnz, Index* rowptr, Index* colind, T* val,
+    Index* cscptr, Index* cscind, T* cscval) {
+  clear();
+  d_csrRowPtr_ = rowptr;
+  d_csrColInd_ = colind;
+  d_csrVal_ = val;
+  csr_ownership_ = true;
+  nvals_ = nnz;
+  ncapacity_ = nnz;
+  symmetric_ = false;
+  if (format_ == GrB_SPARSE_MATRIX_CSRCSC) {
+    if (cscptr == NULL)
+      ingestCsrToCsc<T>(nrows_, ncols_, nnz, rowptr, colind, val, &cscptr, &cscind, &cscval);
+    d_cscColPtr_ = cscptr;
+    d_cscRowInd_ = cscind;
+    d_cscVal_ = cscval;
+    csc_ownership_ = true;
+    cscval_ownership_ = true;
+    csc_initialized_ = true;
+  } else if (cscptr != NULL) {
+    gbFree(cscptr); gbFree(cscind); gbFree(cscval);
+  }
+  csr_initialized_ = true;
+  need_update_ = true;
 }
 
 // After the device CSR is in place (owned): the CSC side, then the host mirrors
@@ -500,7 +559,7 @@ template <typename T>
 Info SparseMatrix<T>::adoptCsc(Index* col_ptr, Index* row_ind, T* values,
     bool symmetric) {
   if (d_csrRowPtr_ == NULL) return GrB_UNINITIALIZED_OBJECT;
-  dropSpmvTiles();
+  dropDerived();
   symmetric_ = symmetric;
   const bool alias = symmetric && (col_ptr == NULL || row_ind == NULL);
   d_cscColPtr_ = alias ? d_csrRowPtr_ : col_ptr;
@@ -688,7 +747,7 @@ Info SparseMatrix<T>::cpuToGpu() {
     ncapacity_ = nvals_;
   }
   CHECK(allocateGpu());
-  dropSpmvTiles();
+  dropDerived();
   transfer(devCsr(), hostCsr(), cudaMemcpyHostToDevice, true);
   if (format_ == GrB_SPARSE_MATRIX_CSRCSC) {
     if (symmetric_) {

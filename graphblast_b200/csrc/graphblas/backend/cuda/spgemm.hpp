@@ -91,14 +91,16 @@ Info spgemmMasked(SparseMatrix<c>* C, const Matrix<m>* mask, BinaryOpT accum,
   const bool use_tran_A = inp0_mode == GrB_TRAN;
   const bool use_tran_B = inp1_mode == GrB_TRAN;
 
-  const Index* A_csrRowPtr = (use_tran_A) ? A->d_cscColPtr_ : A->d_csrRowPtr_;
-  const Index* A_csrColInd = (use_tran_A) ? A->d_cscRowInd_ : A->d_csrColInd_;
-  const a*     A_csrVal    = (use_tran_A) ? A->d_cscVal_    : A->d_csrVal_;
-  const Index  A_nrows     = (use_tran_A) ? A->ncols_       : A->nrows_;
-
-  const Index* B_cscColPtr = (use_tran_B) ? B->d_csrRowPtr_ : B->d_cscColPtr_;
-  const Index* B_cscRowInd = (use_tran_B) ? B->d_csrColInd_ : B->d_cscRowInd_;
-  const b*     B_cscVal    = (use_tran_B) ? B->d_csrVal_    : B->d_cscVal_;
+  // rows of op(A) against columns of op(B): B's CSC unless B is transposed
+  const typename SparseMatrix<a>::View Av = A->view(use_tran_A);
+  const typename SparseMatrix<b>::View Bv = B->view(!use_tran_B);
+  const Index* A_csrRowPtr = Av.ptr;
+  const Index* A_csrColInd = Av.ind;
+  const a*     A_csrVal    = Av.val;
+  const Index  A_nrows     = Av.dim;
+  const Index* B_cscColPtr = Bv.ptr;
+  const Index* B_cscRowInd = Bv.ind;
+  const b*     B_cscVal    = Bv.val;
 
   if (A_csrRowPtr == NULL || B_cscColPtr == NULL)
     return GrB_UNINITIALIZED_OBJECT;
@@ -132,7 +134,7 @@ Info spgemmMasked(SparseMatrix<c>* C, const Matrix<m>* mask, BinaryOpT accum,
       const bool mask_by_cols = sparse_mask->format_ == GrB_SPARSE_MATRIX_CSRCSC &&
           sparse_mask->d_cscColPtr_ != NULL && sparse_mask->d_cscRowInd_ != NULL &&
           sparse_mask->d_cscVal_ != NULL;
-      const Index B_ncols = use_tran_B ? B->nrows_ : B->ncols_;
+      const Index B_ncols = Bv.dim;
       const bool hashed = mask_by_cols &&
           sparse_mask->nrows_ == A_nrows && sparse_mask->ncols_ == B_ncols;
       if (hashed) {
@@ -312,23 +314,20 @@ Info spgemmUnmaskedProduct(SparseMatrix<c>* C, SemiringT op,
   const bool use_tran_A = inp0_mode == GrB_TRAN;
   const bool use_tran_B = inp1_mode == GrB_TRAN;
 
-  const Index* A_ptr = use_tran_A ? A->d_cscColPtr_ : A->d_csrRowPtr_;
-  const Index* A_ind = use_tran_A ? A->d_cscRowInd_ : A->d_csrColInd_;
-  const a*     A_val = use_tran_A ? A->d_cscVal_    : A->d_csrVal_;
-  const Index  m     = use_tran_A ? A->ncols_       : A->nrows_;
-  const Index* B_ptr = use_tran_B ? B->d_cscColPtr_ : B->d_csrRowPtr_;
-  const Index* B_ind = use_tran_B ? B->d_cscRowInd_ : B->d_csrColInd_;
-  const b*     B_val = use_tran_B ? B->d_cscVal_    : B->d_csrVal_;
-  const Index  n     = use_tran_B ? B->nrows_       : B->ncols_;
+  const typename SparseMatrix<a>::View Av = A->view(use_tran_A);
+  const typename SparseMatrix<b>::View Bv = B->view(use_tran_B);
+  const Index* A_ptr = Av.ptr;
+  const Index* A_ind = Av.ind;
+  const a*     A_val = Av.val;
+  const Index* B_ptr = Bv.ptr;
+  const Index* B_ind = Bv.ind;
+  const b*     B_val = Bv.val;
   // op(A) is m x k, op(B) k x n: the kernels index B's pointer array with A's
   // columns, and C's arrays with m and n
-  const Index A_ncols = use_tran_A ? A->nrows_ : A->ncols_;
-  const Index B_nrows = use_tran_B ? B->ncols_ : B->nrows_;
-  if (A_ncols != B_nrows || m != C->nrows_ || n != C->ncols_)
+  const Index m = Av.dim, n = Bv.other;
+  if (Av.other != Bv.dim || m != C->nrows_ || n != C->ncols_)
     return GrB_DIMENSION_MISMATCH;
-  if (A_ptr == NULL || A_ind == NULL || A_val == NULL ||
-      B_ptr == NULL || B_ind == NULL || B_val == NULL)
-    return GrB_UNINITIALIZED_OBJECT;
+  if (!Av.complete() || !Bv.complete()) return GrB_UNINITIALIZED_OBJECT;
 
   cudaStream_t s = gbStream();
   const int sms = runtime().sm_count;
@@ -423,25 +422,7 @@ Info spgemmUnmaskedProduct(SparseMatrix<c>* C, SemiringT op,
       A_ind, A_val, B_ptr, B_ind, B_val, n, rowptr, colind, val, extractMul(op),
       extractAdd(op), static_cast<c>(op.identity()), desc, s);
 
-  // swap in: the old arrays (and every cache built on them) go, stream-ordered
-  // after the kernels above that may still read them through A or B
-  CHECK(C->clear());
-  C->d_csrRowPtr_ = rowptr;
-  C->d_csrColInd_ = colind;
-  C->d_csrVal_ = val;
-  C->csr_ownership_ = true;
-  C->nvals_ = nnz;
-  C->ncapacity_ = nnz;
-  C->symmetric_ = false;
-  if (C->format_ == GrB_SPARSE_MATRIX_CSRCSC) {
-    ingestCsrToCsc<c>(C->nrows_, C->ncols_, nnz, rowptr, colind, val,
-        &C->d_cscColPtr_, &C->d_cscRowInd_, &C->d_cscVal_);
-    C->csc_ownership_ = true;
-    C->cscval_ownership_ = true;
-    C->csc_initialized_ = true;
-  }
-  C->csr_initialized_ = true;
-  C->need_update_ = true;
+  C->replaceDevice(nnz, rowptr, colind, val);
   return GrB_SUCCESS;
 }
 }  // namespace backend

@@ -53,11 +53,11 @@ Info spmmProduct(Matrix<c>* C, SemiringT op, const Matrix<a>* A, const Matrix<b>
   const bool tran = inp0_mode == GrB_TRAN;
   SparseMatrix<a>* S = const_cast<SparseMatrix<a>*>(&A->sparse_);
   const DenseMatrix<b>& D = B->dense_;
-  const Index* ptr = tran ? S->d_cscColPtr_ : S->d_csrRowPtr_;
-  const Index* ind = tran ? S->d_cscRowInd_ : S->d_csrColInd_;
-  const a*     val = tran ? S->d_cscVal_    : S->d_csrVal_;
-  const Index  m   = tran ? S->ncols_ : S->nrows_;
-  const Index  k   = tran ? S->nrows_ : S->ncols_;
+  const typename SparseMatrix<a>::View Av = S->view(tran);
+  const Index* ptr = Av.ptr;
+  const Index* ind = Av.ind;
+  const a*     val = Av.val;
+  const Index  m = Av.dim, k = Av.other;
   const long long N = D.ncols_;
   if (D.nrows_ != k || C->nrows_ != m || C->ncols_ != N) return GrB_DIMENSION_MISMATCH;
   // before anything is allocated: C keeps its contents (the kernel indexes columns
@@ -65,7 +65,7 @@ Info spmmProduct(Matrix<c>* C, SemiringT op, const Matrix<a>* A, const Matrix<b>
   if (!DenseMatrix<c>::fits(static_cast<long long>(m)*N) ||
       N > INT32_MAX - GB_SPMM_COL_TILE)
     return GrB_OUT_OF_MEMORY;
-  if (ptr == NULL || ind == NULL || val == NULL || D.d_val_ == NULL)
+  if (!Av.complete() || D.d_val_ == NULL)
     return GrB_UNINITIALIZED_OBJECT;
 
   // The result goes into C's own array when it has one of this shape that B does
@@ -80,7 +80,7 @@ Info spmmProduct(Matrix<c>* C, SemiringT op, const Matrix<a>* A, const Matrix<b>
 
   if (elements > 0) {
     cudaStream_t s = gbStream();
-    const int ntiles = mergeTiles(S, tran ? 1 : 0, ptr, m);
+    const int ntiles = mergeTiles(S, Av.which, ptr, m);
     const Index nnz = S->nvals_;
     Index* carry_row = reinterpret_cast<Index*>(desc->scratch(GB_SCRATCH_CARRY_ROW,
         static_cast<size_t>(ntiles)*sizeof(Index)));
@@ -90,7 +90,7 @@ Info spmmProduct(Matrix<c>* C, SemiringT op, const Matrix<a>* A, const Matrix<b>
     const long long slices = (N + GB_SPMM_COL_TILE - 1)/GB_SPMM_COL_TILE;
     const dim3 grid(ntiles, static_cast<unsigned>(slices < 65535 ? slices : 65535));
     const int nslices = static_cast<int>(slices);
-    const Index* tiles = S->d_spmv_tiles_[tran ? 1 : 0];
+    const Index* tiles = S->tiles_[Av.which].d;
     const double alg_bytes = 4.0*(m + 1) + 8.0*nnz + 4.0*k*N + 4.0*m*N;
     profiler().begin(GB_PROF_SPMM, s);
     if (N % 4 != 0)

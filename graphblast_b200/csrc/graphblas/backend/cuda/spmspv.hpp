@@ -106,11 +106,12 @@ Info spmspvMerge(SparseVector<W>* w, const Vector<M>* mask, BinaryOpT accum,
   }
 
   // Transpose (default is CSC):
-  const Index* A_csrRowPtr = (!use_tran) ? A->d_cscColPtr_ : A->d_csrRowPtr_;
-  const Index* A_csrColInd = (!use_tran) ? A->d_cscRowInd_ : A->d_csrColInd_;
-  const a*     A_csrVal    = (!use_tran) ? A->d_cscVal_    : A->d_csrVal_;
+  const typename SparseMatrix<a>::View Av = A->view(!use_tran);
+  const Index* A_csrRowPtr = Av.ptr;
+  const Index* A_csrColInd = Av.ind;
+  const a*     A_csrVal    = Av.val;
   // Output length = the other dimension of the traversed structure.
-  const Index  out_size    = (!use_tran) ? A->nrows_       : A->ncols_;
+  const Index  out_size    = Av.other;
   if (A_csrRowPtr == NULL) return GrB_UNINITIALIZED_OBJECT;
 
   const Index nf = u->nvals_;

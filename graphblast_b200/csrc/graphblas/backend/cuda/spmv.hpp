@@ -29,19 +29,12 @@ template <typename a>
 int mergeTiles(SparseMatrix<a>* A, int which, const Index* rowptr, Index nrows) {
   const long long merge_total = static_cast<long long>(nrows) + A->nvals_;
   const int ntiles = static_cast<int>((merge_total + GB_SPMV_TILE - 1)/GB_SPMV_TILE);
-  if (A->d_spmv_tiles_[which] == NULL ||
-      A->spmv_tiles_key_[which] != rowptr ||
-      A->spmv_tiles_nvals_[which] != A->nvals_ ||
-      A->spmv_tiles_count_[which] != ntiles) {
-    if (A->d_spmv_tiles_[which] != NULL) gbFree(A->d_spmv_tiles_[which]);
-    A->d_spmv_tiles_[which] = reinterpret_cast<Index*>(
-        gbMalloc((static_cast<size_t>(ntiles) + 1)*sizeof(Index)));
+  DerivedArray& tiles = A->tiles_[which];
+  if (!tiles.validFor(rowptr, A->nvals_, ntiles)) {
+    tiles.rebuild(static_cast<size_t>(ntiles) + 1, rowptr, A->nvals_, ntiles);
     spmvMergePartitionKernel<<<(ntiles + 256)/256, 256, 0, gbStream()>>>(
-        A->d_spmv_tiles_[which], rowptr, nrows, A->nvals_, ntiles, GB_SPMV_TILE);
+        tiles.d, rowptr, nrows, A->nvals_, ntiles, GB_SPMV_TILE);
     GB_KERNEL_CHECK();
-    A->spmv_tiles_key_[which]   = rowptr;
-    A->spmv_tiles_nvals_[which] = A->nvals_;
-    A->spmv_tiles_count_[which] = ntiles;
   }
   return ntiles;
 }
@@ -135,10 +128,11 @@ Info spmv(DenseVector<W>* w, const Vector<M>* mask, BinaryOpT accum, SemiringT o
   }
 
   // Transpose (default is CSR):
-  const Index* A_csrRowPtr = (use_tran) ? A->d_cscColPtr_ : A->d_csrRowPtr_;
-  const Index* A_csrColInd = (use_tran) ? A->d_cscRowInd_ : A->d_csrColInd_;
-  const a*     A_csrVal    = (use_tran) ? A->d_cscVal_    : A->d_csrVal_;
-  const Index  A_nrows     = (use_tran) ? A->ncols_       : A->nrows_;
+  const typename SparseMatrix<a>::View Av = A->view(use_tran);
+  const Index* A_csrRowPtr = Av.ptr;
+  const Index* A_csrColInd = Av.ind;
+  const a*     A_csrVal    = Av.val;
+  const Index  A_nrows     = Av.dim;
   if (A_csrRowPtr == NULL) return GrB_UNINITIALIZED_OBJECT;
 
   DenseVector<U>* u_t = const_cast<DenseVector<U>*>(u);
@@ -192,9 +186,8 @@ Info spmv(DenseVector<W>* w, const Vector<M>* mask, BinaryOpT accum, SemiringT o
         const int grid = gridFor(A_nrows, GB_PULL_NT, 8);
         // First-neighbour summary of this structure, computed once per matrix.
         SparseMatrix<a>* A_f = const_cast<SparseMatrix<a>*>(A);
-        const int fw = use_tran ? 1 : 0;
-        const Index* A_first = pullFirstNeighbours(A_f, fw, A_csrRowPtr, A_csrColInd,
-                                                   A_nrows);
+        const Index* A_first = pullFirstNeighbours(A_f, Av.which, A_csrRowPtr,
+                                                   A_csrColInd, A_nrows);
         mail_ticket = runtime().mailTicket();
         unsigned long long* mail = runtime().mailSlot(1);
         unsigned long long* done = desc->counters() + 4;
@@ -290,7 +283,7 @@ Info spmv(DenseVector<W>* w, const Vector<M>* mask, BinaryOpT accum, SemiringT o
       w_val = w->d_val_;
 
     SparseMatrix<a>* A_t = const_cast<SparseMatrix<a>*>(A);
-    const int which = use_tran ? 1 : 0;
+    const int which = Av.which;
     mergeTiles(A_t, which, A_csrRowPtr, A_nrows);
     // Large matrices whose entries mostly reference a few columns (power-law
     // graphs) take the hub-cached kernel (kernels/spmv_hub.cuh): hub columns are
@@ -306,11 +299,10 @@ Info spmv(DenseVector<W>* w, const Vector<M>* mask, BinaryOpT accum, SemiringT o
           (reinterpret_cast<uintptr_t>(A_csrColInd) % 32 == 0) &&
           (reinterpret_cast<uintptr_t>(A_csrVal) % 32 == 0);
       if (hub_mode != 0 && A->nvals_ >= hub_min_nnz && aligned32) {
-        const Index ncols_t = use_tran ? A->nrows_ : A->ncols_;
         HubIndex& h = A_t->hub_[which];
         if (A_t->hub_state_[which] == 0 || h.key != A_csrColInd ||
             h.key_nvals != A->nvals_) {
-          buildHubIndex(&h, A_csrRowPtr, A_csrColInd, A_nrows, ncols_t, A->nvals_,
+          buildHubIndex(&h, A_csrRowPtr, A_csrColInd, A_nrows, Av.other, A->nvals_,
               GB_HUB_CAPACITY);
           A_t->hub_state_[which] = (100.0*h.coverage >= hub_min_pct) ? 1 : 2;
           if (A_t->hub_state_[which] == 2) {   // keep only the verdict
@@ -327,7 +319,7 @@ Info spmv(DenseVector<W>* w, const Vector<M>* mask, BinaryOpT accum, SemiringT o
       }
     }
     if (!done)
-    CHECK(spmvMergeLaunch(w_val, A_t->d_spmv_tiles_[which], op, A_csrRowPtr, A_csrColInd,
+    CHECK(spmvMergeLaunch(w_val, A_t->tiles_[which].d, op, A_csrRowPtr, A_csrColInd,
         A_csrVal, u_t->d_val_, A_nrows, A->nvals_, desc));
 
     if (use_mask) {
