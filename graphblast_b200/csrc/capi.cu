@@ -38,14 +38,13 @@ struct gb200_desc_s {
 };
 
 struct gb200_vector_s {
-  int dtype;
   graphblas::Vector<float>* f;
 };
 
+// Exactly one of f and i is set: it names the handle's element type.
 struct gb200_matrix_s {
-  int dtype;
-  graphblas::Matrix<float>* f;
-  graphblas::Matrix<int>*   i;
+  graphblas::Matrix<float>* f = NULL;
+  graphblas::Matrix<int>*   i = NULL;
 };
 
 // Result of gb200_ingest_coo: a CSR in pool memory until exported / freed.
@@ -63,69 +62,6 @@ using graphblas::Info;
 using graphblas::GrB_SUCCESS;
 
 inline int rc(Info info) { return static_cast<int>(info); }
-
-// Semiring id -> instantiation.  BODY uses `op`.
-#define GB200_SEMIRING_DISPATCH(ID, ...)                                       \
-  switch (ID) {                                                                \
-    case GB200_LOGICAL_OR_AND:                                                 \
-      { graphblas::LogicalOrAndSemiring<float> op; __VA_ARGS__; } break;              \
-    case GB200_PLUS_MULTIPLIES:                                                \
-      { graphblas::PlusMultipliesSemiring<float> op; __VA_ARGS__; } break;            \
-    case GB200_MINIMUM_PLUS:                                                   \
-      { graphblas::MinimumPlusSemiring<float> op; __VA_ARGS__; } break;               \
-    case GB200_MAXIMUM_MULTIPLIES:                                             \
-      { graphblas::MaximumMultipliesSemiring<float> op; __VA_ARGS__; } break;         \
-    case GB200_PLUS_DIVIDES:                                                   \
-      { graphblas::PlusDividesSemiring<float> op; __VA_ARGS__; } break;               \
-    case GB200_PLUS_GREATER:                                                   \
-      { graphblas::PlusGreaterSemiring<float> op; __VA_ARGS__; } break;               \
-    case GB200_GREATER_PLUS:                                                   \
-      { graphblas::GreaterPlusSemiring<float> op; __VA_ARGS__; } break;               \
-    case GB200_PLUS_MINUS:                                                     \
-      { graphblas::PlusMinusSemiring<float> op; __VA_ARGS__; } break;                 \
-    case GB200_PLUS_LESS:                                                      \
-      { graphblas::PlusLessSemiring<float> op; __VA_ARGS__; } break;                  \
-    case GB200_CUSTOM_LESS_PLUS:                                               \
-      { graphblas::CustomLessPlusSemiring<float> op; __VA_ARGS__; } break;            \
-    case GB200_MINIMUM_MULTIPLIES:                                             \
-      { graphblas::MinimumMultipliesSemiring<float> op; __VA_ARGS__; } break;         \
-    case GB200_MULTIPLIES_MULTIPLIES:                                          \
-      { graphblas::MultipliesMultipliesSemiring<float> op; __VA_ARGS__; } break;      \
-    case GB200_NOT_EQUAL_TO_PLUS:                                              \
-      { graphblas::NotEqualToPlusSemiring<float> op; __VA_ARGS__; } break;            \
-    case GB200_MINIMUM_SELECT_SECOND:                                          \
-      { graphblas::MinimumSelectSecondSemiring<float> op; __VA_ARGS__; } break;       \
-    case GB200_PLUS_NOT_EQUAL_TO:                                              \
-      { graphblas::PlusNotEqualToSemiring<float> op; __VA_ARGS__; } break;            \
-    case GB200_CUSTOM_LESS_LESS:                                               \
-      { graphblas::CustomLessLessSemiring<float> op; __VA_ARGS__; } break;            \
-    case GB200_MINIMUM_NOT_EQUAL_TO:                                           \
-      { graphblas::MinimumNotEqualToSemiring<float> op; __VA_ARGS__; } break;         \
-    default: return rc(graphblas::GrB_INVALID_VALUE);                          \
-  }
-
-#define GB200_MONOID_DISPATCH(ID, TYPE, ...)                                   \
-  switch (ID) {                                                                \
-    case GB200_PLUS_MONOID:                                                    \
-      { graphblas::PlusMonoid<TYPE> op; __VA_ARGS__; } break;                         \
-    case GB200_MULTIPLIES_MONOID:                                              \
-      { graphblas::MultipliesMonoid<TYPE> op; __VA_ARGS__; } break;                   \
-    case GB200_MINIMUM_MONOID:                                                 \
-      { graphblas::MinimumMonoid<TYPE> op; __VA_ARGS__; } break;                      \
-    case GB200_MAXIMUM_MONOID:                                                 \
-      { graphblas::MaximumMonoid<TYPE> op; __VA_ARGS__; } break;                      \
-    case GB200_LOGICAL_OR_MONOID:                                              \
-      { graphblas::LogicalOrMonoid<TYPE> op; __VA_ARGS__; } break;                    \
-    case GB200_LOGICAL_AND_MONOID:                                             \
-      { graphblas::LogicalAndMonoid<TYPE> op; __VA_ARGS__; } break;                   \
-    case GB200_GREATER_MONOID:                                                 \
-      { graphblas::GreaterMonoid<TYPE> op; __VA_ARGS__; } break;                      \
-    case GB200_CUSTOM_LESS_MONOID:                                             \
-      { graphblas::CustomLessMonoid<TYPE> op; __VA_ARGS__; } break;                   \
-    case GB200_NOT_EQUAL_TO_MONOID:                                            \
-      { graphblas::NotEqualToMonoid<TYPE> op; __VA_ARGS__; } break;                   \
-    default: return rc(graphblas::GrB_INVALID_VALUE);                          \
-  }
 
 inline bool cudaOk() {
   int count = 0;
@@ -147,7 +83,163 @@ inline bool cudaOk() {
     }                                                                          \
   } while (0)
 
+// body(op) with the FP32 semiring of a GB200_* semiring id; GrB_INVALID_VALUE for
+// an unknown id.
+template <typename Body>
+int withSemiring(int id, Body&& body) {
+  using namespace graphblas;  // NOLINT(build/namespaces)
+  switch (id) {
+    case GB200_LOGICAL_OR_AND:        return body(LogicalOrAndSemiring<float>());
+    case GB200_PLUS_MULTIPLIES:       return body(PlusMultipliesSemiring<float>());
+    case GB200_MINIMUM_PLUS:          return body(MinimumPlusSemiring<float>());
+    case GB200_MAXIMUM_MULTIPLIES:    return body(MaximumMultipliesSemiring<float>());
+    case GB200_PLUS_DIVIDES:          return body(PlusDividesSemiring<float>());
+    case GB200_PLUS_GREATER:          return body(PlusGreaterSemiring<float>());
+    case GB200_GREATER_PLUS:          return body(GreaterPlusSemiring<float>());
+    case GB200_PLUS_MINUS:            return body(PlusMinusSemiring<float>());
+    case GB200_PLUS_LESS:             return body(PlusLessSemiring<float>());
+    case GB200_CUSTOM_LESS_PLUS:      return body(CustomLessPlusSemiring<float>());
+    case GB200_MINIMUM_MULTIPLIES:    return body(MinimumMultipliesSemiring<float>());
+    case GB200_MULTIPLIES_MULTIPLIES: return body(MultipliesMultipliesSemiring<float>());
+    case GB200_NOT_EQUAL_TO_PLUS:     return body(NotEqualToPlusSemiring<float>());
+    case GB200_MINIMUM_SELECT_SECOND: return body(MinimumSelectSecondSemiring<float>());
+    case GB200_PLUS_NOT_EQUAL_TO:     return body(PlusNotEqualToSemiring<float>());
+    case GB200_CUSTOM_LESS_LESS:      return body(CustomLessLessSemiring<float>());
+    case GB200_MINIMUM_NOT_EQUAL_TO:  return body(MinimumNotEqualToSemiring<float>());
+    default: return rc(GrB_INVALID_VALUE);
+  }
+}
+
+// body(op) with the monoid over T of a GB200_*_MONOID id; GrB_INVALID_VALUE for an
+// unknown id.
+template <typename T, typename Body>
+int withMonoid(int id, Body&& body) {
+  using namespace graphblas;  // NOLINT(build/namespaces)
+  switch (id) {
+    case GB200_PLUS_MONOID:         return body(PlusMonoid<T>());
+    case GB200_MULTIPLIES_MONOID:   return body(MultipliesMonoid<T>());
+    case GB200_MINIMUM_MONOID:      return body(MinimumMonoid<T>());
+    case GB200_MAXIMUM_MONOID:      return body(MaximumMonoid<T>());
+    case GB200_LOGICAL_OR_MONOID:   return body(LogicalOrMonoid<T>());
+    case GB200_LOGICAL_AND_MONOID:  return body(LogicalAndMonoid<T>());
+    case GB200_GREATER_MONOID:      return body(GreaterMonoid<T>());
+    case GB200_CUSTOM_LESS_MONOID:  return body(CustomLessMonoid<T>());
+    case GB200_NOT_EQUAL_TO_MONOID: return body(NotEqualToMonoid<T>());
+    default: return rc(GrB_INVALID_VALUE);
+  }
+}
+
 graphblas::Vector<float>* vec(gb200_vector_t v) { return v ? v->f : NULL; }
+
+// The element type T of a graphblas::Matrix<T>* M: decltype(elementOf(M)).
+template <typename T> T elementOf(const graphblas::Matrix<T>*);
+
+// f(M) with A's typed matrix M, a graphblas::Matrix<float>* or Matrix<int>*.
+template <typename F>
+auto onMatrix(gb200_matrix_t A, F&& f) { return A->f != NULL ? f(A->f) : f(A->i); }
+
+// Every given handle holds FP32 (allFp32) or INT32 (allInt32) values; NULL, an
+// absent mask, matches either.
+template <typename... M>
+bool allFp32(M... m) { return ((m == NULL || m->f != NULL) && ...); }
+template <typename... M>
+bool allInt32(M... m) { return ((m == NULL || m->i != NULL) && ...); }
+
+// *out = a new handle of element type dtype, its matrix M (a Matrix<float>*& or
+// Matrix<int>*&) set by make(M); GrB_DOMAIN_MISMATCH for an unknown dtype.
+template <typename Make>
+int newMatrix(gb200_matrix_t* out, int dtype, Make&& make) {
+  gb200_matrix_s* m = new gb200_matrix_s();
+  const Info info = dtype == GB200_FP32  ? make(m->f)
+                  : dtype == GB200_INT32 ? make(m->i) : graphblas::GrB_DOMAIN_MISMATCH;
+  if (info != GrB_SUCCESS) {
+    delete m;
+    return rc(info);
+  }
+  *out = m;
+  return 0;
+}
+
+// An algorithm driver run(): it returns the device time of its loop in ms, or a
+// negative time with the failing status left in algorithm::lastStatus().  The time
+// goes to *tight_ms when asked for.
+template <typename Run>
+int runAlgorithm(float* tight_ms, Run&& run) {
+  graphblas::algorithm::lastStatus() = GrB_SUCCESS;
+  const float ms = run();
+  if (ms < 0.f) return rc(graphblas::algorithm::lastStatus());
+  if (tight_ms) *tight_ms = ms;
+  return 0;
+}
+
+template <typename T>
+Info buildCoo(graphblas::Matrix<T>* M, const int* rows, const int* cols,
+              const void* vals, int nvals, int undirected) {
+  std::vector<graphblas::Index> r(rows, rows + nvals);
+  std::vector<graphblas::Index> c(cols, cols + nvals);
+  std::vector<T> v(nvals, static_cast<T>(1));
+  if (vals != NULL) {
+    const T* tv = static_cast<const T*>(vals);
+    v.assign(tv, tv + nvals);
+  }
+  // The backend keys CSR/CSC aliasing on the ".ud." marker of the cache name
+  // (reference sparse_matrix.hpp:300-306); pass the marker without a cache file.
+  M->matrix_.sparse_.symmetric_ = (undirected != 0);
+  Info info = M->build(&r, &c, &v, nvals, GrB_NULL);
+  return info;
+}
+
+// Matrix Market file -> matrix: the text is parsed on the host (MtxFile), the raw
+// tuples go to the device, and symmetrising, ordering and the removal of
+// self-loops / repeated pairs run there (backend/cuda/ingest.hpp) with the
+// semantics of the reference's readMtx (graphblas/util.hpp:264-329, 364-430).
+template <typename T>
+Info loadMtx(graphblas::Matrix<T>** out, const char* path, int directed) {
+  using namespace graphblas::backend;
+  MtxFile file(path);
+  if (!file.ok) return graphblas::GrB_INVALID_VALUE;
+  std::vector<graphblas::Index> rows, cols;
+  std::vector<T> vals;
+  file.tuples<T>(&rows, &cols, &vals);
+  const bool undirected = directed != 1 && (file.symmetric() || directed == 2);
+  const bool drop_loops = getEnv("GRB_UTIL_REMOVE_SELFLOOP", true);
+  graphblas::Matrix<T>* M = new graphblas::Matrix<T>(file.nrows, file.ncols);
+  const size_t m = rows.size();
+  const size_t alloc = m > 0 ? m : 1;
+  graphblas::Index* d_r = reinterpret_cast<graphblas::Index*>(gbMalloc(alloc*sizeof(graphblas::Index)));
+  graphblas::Index* d_c = reinterpret_cast<graphblas::Index*>(gbMalloc(alloc*sizeof(graphblas::Index)));
+  T* d_v = reinterpret_cast<T*>(gbMalloc(alloc*sizeof(T)));
+  if (m > 0) {
+    CUDA_CALL(cudaMemcpyAsync(d_r, rows.data(), m*sizeof(graphblas::Index), cudaMemcpyHostToDevice, gbStream()));
+    CUDA_CALL(cudaMemcpyAsync(d_c, cols.data(), m*sizeof(graphblas::Index), cudaMemcpyHostToDevice, gbStream()));
+    CUDA_CALL(cudaMemcpyAsync(d_v, vals.data(), m*sizeof(T), cudaMemcpyHostToDevice, gbStream()));
+    runtime().sync();
+  }
+  const int mode = (undirected ? GB_INGEST_SYMMETRIZE : 0) |
+                   (drop_loops ? GB_INGEST_DROP_LOOPS : 0) | GB_INGEST_DEDUP;
+  M->matrix_.mat_type_ = graphblas::GrB_SPARSE;
+  Info info = M->matrix_.sparse_.buildFromDeviceTuples(d_r, d_c, d_v,
+      static_cast<long long>(m), mode, undirected);
+  gbFree(d_v); gbFree(d_c); gbFree(d_r);
+  if (info != GrB_SUCCESS) {
+    delete M;
+    return info;
+  }
+  *out = M;
+  return GrB_SUCCESS;
+}
+
+template <typename T>
+Info extractCsr(graphblas::Matrix<T>* M, int* rowptr, int* colind, void* val) {
+  if (!M->matrix_.isSparse()) return graphblas::GrB_UNINITIALIZED_OBJECT;
+  graphblas::backend::SparseMatrix<T>& S = M->matrix_.sparse_;
+  CHECK(S.gpuToCpu());
+  memcpy(rowptr, S.h_csrRowPtr_, (S.nrows_ + 1)*sizeof(int));
+  memcpy(colind, S.h_csrColInd_, static_cast<size_t>(S.nvals_)*sizeof(int));
+  if (val != NULL)
+    memcpy(val, S.h_csrVal_, static_cast<size_t>(S.nvals_)*sizeof(T));
+  return GrB_SUCCESS;
+}
 
 // C = A (+) B (IsAdd) or A (x) B of two matrices: FP32 over every semiring,
 // INT32 over PlusMultiplies only, no mixing.
@@ -156,9 +248,9 @@ int ewiseMatrix(gb200_matrix_t C, gb200_matrix_t mask, int semiring, gb200_matri
                 gb200_matrix_t B, gb200_desc_t desc) {
   if (C == NULL || A == NULL || B == NULL || desc == NULL)
     return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
-  if (C->f != NULL && A->f != NULL && B->f != NULL && (mask == NULL || mask->f != NULL)) {
+  if (allFp32(C, A, B, mask)) {
     GB200_REQUIRE_DEVICE();
-    GB200_SEMIRING_DISPATCH(semiring, {
+    return withSemiring(semiring, [&](auto op) {
       if constexpr (IsAdd)
         return rc((graphblas::eWiseAdd<float, float, float, float>(C->f,
             mask != NULL ? mask->f : NULL, GrB_NULL, op, A->f, B->f, &desc->desc)));
@@ -166,10 +258,8 @@ int ewiseMatrix(gb200_matrix_t C, gb200_matrix_t mask, int semiring, gb200_matri
         return rc((graphblas::eWiseMult<float, float, float, float>(C->f,
             mask != NULL ? mask->f : NULL, GrB_NULL, op, A->f, B->f, &desc->desc)));
     });
-    return 0;
   }
-  if (C->i == NULL || A->i == NULL || B->i == NULL || (mask != NULL && mask->i == NULL))
-    return rc(graphblas::GrB_DOMAIN_MISMATCH);
+  if (!allInt32(C, A, B, mask)) return rc(graphblas::GrB_DOMAIN_MISMATCH);
   if (semiring != GB200_PLUS_MULTIPLIES) return rc(graphblas::GrB_NOT_IMPLEMENTED);
   GB200_REQUIRE_DEVICE();
   if constexpr (IsAdd)
@@ -178,6 +268,32 @@ int ewiseMatrix(gb200_matrix_t C, gb200_matrix_t mask, int semiring, gb200_matri
   else
     return rc((graphblas::eWiseMult<int, int, int, int>(C->i, mask ? mask->i : NULL,
         GrB_NULL, graphblas::PlusMultipliesSemiring<int>(), A->i, B->i, &desc->desc)));
+}
+
+__global__ void rmatEdgesKernel(int scale, long long nedges,
+                                unsigned long long seed, long long first_edge,
+                                int* __restrict__ src, int* __restrict__ dst) {
+  const unsigned int T1 = 2448131358u, T2 = 3264175144u, T3 = 4080218930u;
+  long long e = static_cast<long long>(blockIdx.x)*blockDim.x + threadIdx.x;
+  const long long stride = static_cast<long long>(gridDim.x)*blockDim.x;
+  for (; e < nedges; e += stride) {
+    const unsigned long long ge = static_cast<unsigned long long>(first_edge + e);
+    unsigned int s = 0, d = 0;
+    for (int l = 0; l < scale; ++l) {
+      unsigned long long z = ((seed << 48) ^ (ge << 6) ^
+          static_cast<unsigned long long>(l)) + 0x9E3779B97F4A7C15ull;
+      z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+      z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+      z = z ^ (z >> 31);
+      const unsigned int r = static_cast<unsigned int>(z >> 32);
+      const unsigned int sb = (r >= T2) ? 1u : 0u;
+      const unsigned int db = ((r >= T1 && r < T2) || r >= T3) ? 1u : 0u;
+      s = (s << 1) | sb;
+      d = (d << 1) | db;
+    }
+    src[e] = static_cast<int>(s);
+    dst[e] = static_cast<int>(d);
+  }
 }
 
 }  // namespace
@@ -286,15 +402,10 @@ int gb200_matrix_new(gb200_matrix_t* out, int dtype, int nrows, int ncols) {
   if (out == NULL) return rc(graphblas::GrB_NULL_POINTER);
   if (nrows <= 0 || ncols <= 0) return rc(graphblas::GrB_INVALID_VALUE);
   GB200_REQUIRE_DEVICE();
-  gb200_matrix_s* m = new gb200_matrix_s();
-  m->dtype = dtype;
-  m->f = NULL;
-  m->i = NULL;
-  if (dtype == GB200_FP32)       m->f = new graphblas::Matrix<float>(nrows, ncols);
-  else if (dtype == GB200_INT32) m->i = new graphblas::Matrix<int>(nrows, ncols);
-  else { delete m; return rc(graphblas::GrB_DOMAIN_MISMATCH); }
-  *out = m;
-  return 0;
+  return newMatrix(out, dtype, [&](auto& M) {
+    M = new graphblas::Matrix<decltype(elementOf(M))>(nrows, ncols);
+    return GrB_SUCCESS;
+  });
 }
 
 int gb200_matrix_free(gb200_matrix_t A) {
@@ -305,29 +416,6 @@ int gb200_matrix_free(gb200_matrix_t A) {
   return 0;
 }
 
-}  // extern "C"
-
-namespace {
-template <typename T>
-Info buildCoo(graphblas::Matrix<T>* M, const int* rows, const int* cols,
-              const void* vals, int nvals, int undirected) {
-  std::vector<graphblas::Index> r(rows, rows + nvals);
-  std::vector<graphblas::Index> c(cols, cols + nvals);
-  std::vector<T> v(nvals, static_cast<T>(1));
-  if (vals != NULL) {
-    const T* tv = static_cast<const T*>(vals);
-    v.assign(tv, tv + nvals);
-  }
-  // The backend keys CSR/CSC aliasing on the ".ud." marker of the cache name
-  // (reference sparse_matrix.hpp:300-306); pass the marker without a cache file.
-  M->matrix_.sparse_.symmetric_ = (undirected != 0);
-  Info info = M->build(&r, &c, &v, nvals, GrB_NULL);
-  return info;
-}
-}  // namespace
-
-extern "C" {
-
 int gb200_matrix_build_coo(gb200_matrix_t A, const int* h_rows,
                            const int* h_cols, const void* h_vals, int nvals,
                            int undirected) {
@@ -335,55 +423,10 @@ int gb200_matrix_build_coo(gb200_matrix_t A, const int* h_rows,
     return rc(graphblas::GrB_NULL_POINTER);
   if (nvals <= 0) return rc(graphblas::GrB_NO_VALUE);
   GB200_REQUIRE_DEVICE();
-  if (A->f) return rc(buildCoo(A->f, h_rows, h_cols, h_vals, nvals, undirected));
-  return rc(buildCoo(A->i, h_rows, h_cols, h_vals, nvals, undirected));
+  return rc(onMatrix(A, [&](auto M) {
+    return buildCoo(M, h_rows, h_cols, h_vals, nvals, undirected);
+  }));
 }
-
-}  // extern "C"
-
-namespace {
-// Matrix Market file -> matrix: the text is parsed on the host (MtxFile), the raw
-// tuples go to the device, and symmetrising, ordering and the removal of
-// self-loops / repeated pairs run there (backend/cuda/ingest.hpp) with the
-// semantics of the reference's readMtx (graphblas/util.hpp:264-329, 364-430).
-template <typename T>
-Info loadMtx(graphblas::Matrix<T>** out, const char* path, int directed) {
-  using namespace graphblas::backend;
-  MtxFile file(path);
-  if (!file.ok) return graphblas::GrB_INVALID_VALUE;
-  std::vector<graphblas::Index> rows, cols;
-  std::vector<T> vals;
-  file.tuples<T>(&rows, &cols, &vals);
-  const bool undirected = directed != 1 && (file.symmetric() || directed == 2);
-  const bool drop_loops = getEnv("GRB_UTIL_REMOVE_SELFLOOP", true);
-  graphblas::Matrix<T>* M = new graphblas::Matrix<T>(file.nrows, file.ncols);
-  const size_t m = rows.size();
-  const size_t alloc = m > 0 ? m : 1;
-  graphblas::Index* d_r = reinterpret_cast<graphblas::Index*>(gbMalloc(alloc*sizeof(graphblas::Index)));
-  graphblas::Index* d_c = reinterpret_cast<graphblas::Index*>(gbMalloc(alloc*sizeof(graphblas::Index)));
-  T* d_v = reinterpret_cast<T*>(gbMalloc(alloc*sizeof(T)));
-  if (m > 0) {
-    CUDA_CALL(cudaMemcpyAsync(d_r, rows.data(), m*sizeof(graphblas::Index), cudaMemcpyHostToDevice, gbStream()));
-    CUDA_CALL(cudaMemcpyAsync(d_c, cols.data(), m*sizeof(graphblas::Index), cudaMemcpyHostToDevice, gbStream()));
-    CUDA_CALL(cudaMemcpyAsync(d_v, vals.data(), m*sizeof(T), cudaMemcpyHostToDevice, gbStream()));
-    runtime().sync();
-  }
-  const int mode = (undirected ? GB_INGEST_SYMMETRIZE : 0) |
-                   (drop_loops ? GB_INGEST_DROP_LOOPS : 0) | GB_INGEST_DEDUP;
-  M->matrix_.mat_type_ = graphblas::GrB_SPARSE;
-  Info info = M->matrix_.sparse_.buildFromDeviceTuples(d_r, d_c, d_v,
-      static_cast<long long>(m), mode, undirected);
-  gbFree(d_v); gbFree(d_c); gbFree(d_r);
-  if (info != GrB_SUCCESS) {
-    delete M;
-    return info;
-  }
-  *out = M;
-  return GrB_SUCCESS;
-}
-}  // namespace
-
-extern "C" {
 
 int gb200_matrix_load_mtx(gb200_matrix_t* out, int dtype, const char* path,
                           int directed) {
@@ -392,20 +435,7 @@ int gb200_matrix_load_mtx(gb200_matrix_t* out, int dtype, const char* path,
   FILE* probe = fopen(path, "r");
   if (probe == NULL) return rc(graphblas::GrB_INVALID_VALUE);
   fclose(probe);
-  gb200_matrix_s* m = new gb200_matrix_s();
-  m->dtype = dtype;
-  m->f = NULL;
-  m->i = NULL;
-  Info info;
-  if (dtype == GB200_FP32)       info = loadMtx(&m->f, path, directed);
-  else if (dtype == GB200_INT32) info = loadMtx(&m->i, path, directed);
-  else info = graphblas::GrB_DOMAIN_MISMATCH;
-  if (info != GrB_SUCCESS) {
-    delete m;
-    return rc(info);
-  }
-  *out = m;
-  return 0;
+  return newMatrix(out, dtype, [&](auto& M) { return loadMtx(&M, path, directed); });
 }
 
 int gb200_matrix_build_coo_device(gb200_matrix_t A, const int* d_rows,
@@ -417,14 +447,12 @@ int gb200_matrix_build_coo_device(gb200_matrix_t A, const int* d_rows,
   GB200_REQUIRE_DEVICE();
   const int mode = flags & 7;
   const bool symmetric = (flags & GB200_INGEST_SYMMETRIC_STRUCTURE) != 0;
-  if (A->f) {
-    CHECK(A->f->matrix_.setStorage(graphblas::GrB_SPARSE));
-    return rc(A->f->matrix_.sparse_.buildFromDeviceTuples(d_rows, d_cols,
-        static_cast<const float*>(d_vals), ntuples, mode, symmetric));
-  }
-  CHECK(A->i->matrix_.setStorage(graphblas::GrB_SPARSE));
-  return rc(A->i->matrix_.sparse_.buildFromDeviceTuples(d_rows, d_cols,
-      static_cast<const int*>(d_vals), ntuples, mode, symmetric));
+  return rc(onMatrix(A, [&](auto M) {
+    using T = decltype(elementOf(M));
+    CHECK(M->matrix_.setStorage(graphblas::GrB_SPARSE));
+    return M->matrix_.sparse_.buildFromDeviceTuples(d_rows, d_cols,
+        static_cast<const T*>(d_vals), ntuples, mode, symmetric);
+  }));
 }
 
 int gb200_ingest_coo(int nrows, int ncols, const int* d_rows, const int* d_cols,
@@ -446,17 +474,11 @@ int gb200_ingest_coo(int nrows, int ncols, const int* d_rows, const int* d_cols,
 int gb200_ingest_export(gb200_ingest_t h, int* d_rowptr, int* d_colind, float* d_val) {
   if (h == NULL) return rc(graphblas::GrB_NULL_POINTER);
   GB200_REQUIRE_DEVICE();
-  cudaStream_t s = graphblas::backend::gbStream();
-  if (d_rowptr != NULL)
-    CUDA_CALL(cudaMemcpyAsync(d_rowptr, h->rowptr, (static_cast<size_t>(h->nrows) + 1)*sizeof(int),
-        cudaMemcpyDeviceToDevice, s));
-  if (d_colind != NULL && h->nnz > 0)
-    CUDA_CALL(cudaMemcpyAsync(d_colind, h->colind, static_cast<size_t>(h->nnz)*sizeof(int),
-        cudaMemcpyDeviceToDevice, s));
-  if (d_val != NULL && h->nnz > 0)
-    CUDA_CALL(cudaMemcpyAsync(d_val, h->val, static_cast<size_t>(h->nnz)*sizeof(float),
-        cudaMemcpyDeviceToDevice, s));
-  graphblas::backend::runtime().sync();
+  using namespace graphblas::backend;
+  copyAsync(d_rowptr, h->rowptr, static_cast<size_t>(h->nrows) + 1, cudaMemcpyDeviceToDevice);
+  copyAsync(d_colind, h->colind, static_cast<size_t>(h->nnz), cudaMemcpyDeviceToDevice);
+  copyAsync(d_val, h->val, static_cast<size_t>(h->nnz), cudaMemcpyDeviceToDevice);
+  runtime().sync();
   return 0;
 }
 
@@ -481,19 +503,11 @@ int gb200_csr_transpose_values(int nrows, int ncols, int nnz, const int* d_rowpt
   ingestCsrToCsc<float>(nrows, ncols, nnz, d_rowptr, d_colind, d_val,
       d_colptr_out != NULL ? &colptr : NULL, d_rowind_out != NULL ? &rowind : NULL,
       d_cscval_out != NULL ? &cval : NULL);
-  cudaStream_t s = gbStream();
-  if (colptr != NULL) {
-    CUDA_CALL(cudaMemcpyAsync(d_colptr_out, colptr, (static_cast<size_t>(ncols) + 1)*sizeof(int), cudaMemcpyDeviceToDevice, s));
-    gbFree(colptr);
-  }
-  if (rowind != NULL) {
-    if (nnz > 0) CUDA_CALL(cudaMemcpyAsync(d_rowind_out, rowind, static_cast<size_t>(nnz)*sizeof(int), cudaMemcpyDeviceToDevice, s));
-    gbFree(rowind);
-  }
-  if (cval != NULL) {
-    if (nnz > 0) CUDA_CALL(cudaMemcpyAsync(d_cscval_out, cval, static_cast<size_t>(nnz)*sizeof(float), cudaMemcpyDeviceToDevice, s));
-    gbFree(cval);
-  }
+  const size_t nvals = nnz > 0 ? static_cast<size_t>(nnz) : 0;
+  copyAsync(d_colptr_out, colptr, static_cast<size_t>(ncols) + 1, cudaMemcpyDeviceToDevice);
+  copyAsync(d_rowind_out, rowind, nvals, cudaMemcpyDeviceToDevice);
+  copyAsync(d_cscval_out, cval, nvals, cudaMemcpyDeviceToDevice);
+  gbFree(colptr); gbFree(rowind); gbFree(cval);
   runtime().sync();
   return 0;
 }
@@ -512,11 +526,9 @@ int gb200_sort_pairs_u64(unsigned long long* d_keys, unsigned int* d_payload,
       ? reinterpret_cast<unsigned int*>(gbMalloc(alloc*4)) : NULL;
   radixSortPairs(&keys, d_payload != NULL ? &pay : NULL, &keys_tmp,
       d_payload != NULL ? &pay_tmp : NULL, n, bits);
-  cudaStream_t s = gbStream();
   if (keys != d_keys) {              // an odd number of passes left the result in the temporaries
-    CUDA_CALL(cudaMemcpyAsync(d_keys, keys, alloc*8, cudaMemcpyDeviceToDevice, s));
-    if (d_payload != NULL)
-      CUDA_CALL(cudaMemcpyAsync(d_payload, pay, alloc*4, cudaMemcpyDeviceToDevice, s));
+    copyAsync(d_keys, keys, alloc, cudaMemcpyDeviceToDevice);
+    copyAsync(d_payload, pay, alloc, cudaMemcpyDeviceToDevice);
     runtime().sync();
     gbFree(keys);
     if (pay != NULL && pay != d_payload) gbFree(pay);
@@ -532,61 +544,44 @@ int gb200_matrix_adopt_csr(gb200_matrix_t A, int* d_rowptr, int* d_colind,
                            void* d_val, int nvals) {
   if (A == NULL) return rc(graphblas::GrB_NULL_POINTER);
   GB200_REQUIRE_DEVICE();
-  if (A->f) return rc(A->f->build(d_rowptr, d_colind,
-                                  static_cast<float*>(d_val), nvals));
-  return rc(A->i->build(d_rowptr, d_colind, static_cast<int*>(d_val), nvals));
+  return rc(onMatrix(A, [&](auto M) {
+    using T = decltype(elementOf(M));
+    return M->build(d_rowptr, d_colind, static_cast<T*>(d_val), nvals);
+  }));
 }
 
 int gb200_matrix_adopt_csc(gb200_matrix_t A, int* d_colptr, int* d_rowind,
                            void* d_val, int symmetric) {
   if (A == NULL) return rc(graphblas::GrB_NULL_POINTER);
   GB200_REQUIRE_DEVICE();
-  if (A->f) return rc(A->f->matrix_.sparse_.adoptCsc(d_colptr, d_rowind,
-                      static_cast<float*>(d_val), symmetric != 0));
-  return rc(A->i->matrix_.sparse_.adoptCsc(d_colptr, d_rowind,
-            static_cast<int*>(d_val), symmetric != 0));
+  return rc(onMatrix(A, [&](auto M) {
+    using T = decltype(elementOf(M));
+    return M->matrix_.sparse_.adoptCsc(d_colptr, d_rowind, static_cast<T*>(d_val),
+                                       symmetric != 0);
+  }));
 }
 
 int gb200_matrix_nrows(gb200_matrix_t A, int* out) {
   if (A == NULL || out == NULL) return rc(graphblas::GrB_NULL_POINTER);
-  return A->f ? rc(A->f->nrows(out)) : rc(A->i->nrows(out));
+  return rc(onMatrix(A, [&](auto M) { return M->nrows(out); }));
 }
 
 int gb200_matrix_ncols(gb200_matrix_t A, int* out) {
   if (A == NULL || out == NULL) return rc(graphblas::GrB_NULL_POINTER);
-  return A->f ? rc(A->f->ncols(out)) : rc(A->i->ncols(out));
+  return rc(onMatrix(A, [&](auto M) { return M->ncols(out); }));
 }
 
 int gb200_matrix_nvals(gb200_matrix_t A, int* out) {
   if (A == NULL || out == NULL) return rc(graphblas::GrB_NULL_POINTER);
-  return A->f ? rc(A->f->nvals(out)) : rc(A->i->nvals(out));
+  return rc(onMatrix(A, [&](auto M) { return M->nvals(out); }));
 }
-
-}  // extern "C"
-
-namespace {
-template <typename T>
-Info extractCsr(graphblas::Matrix<T>* M, int* rowptr, int* colind, void* val) {
-  if (!M->matrix_.isSparse()) return graphblas::GrB_UNINITIALIZED_OBJECT;
-  graphblas::backend::SparseMatrix<T>& S = M->matrix_.sparse_;
-  CHECK(S.gpuToCpu());
-  memcpy(rowptr, S.h_csrRowPtr_, (S.nrows_ + 1)*sizeof(int));
-  memcpy(colind, S.h_csrColInd_, static_cast<size_t>(S.nvals_)*sizeof(int));
-  if (val != NULL)
-    memcpy(val, S.h_csrVal_, static_cast<size_t>(S.nvals_)*sizeof(T));
-  return GrB_SUCCESS;
-}
-}  // namespace
-
-extern "C" {
 
 int gb200_matrix_extract_csr(gb200_matrix_t A, int* h_rowptr, int* h_colind,
                              void* h_val) {
   if (A == NULL || h_rowptr == NULL || h_colind == NULL)
     return rc(graphblas::GrB_NULL_POINTER);
   GB200_REQUIRE_DEVICE();
-  if (A->f) return rc(extractCsr(A->f, h_rowptr, h_colind, h_val));
-  return rc(extractCsr(A->i, h_rowptr, h_colind, h_val));
+  return rc(onMatrix(A, [&](auto M) { return extractCsr(M, h_rowptr, h_colind, h_val); }));
 }
 
 int gb200_matrix_build_dense(gb200_matrix_t A, const void* h_vals, long long nvals) {
@@ -622,7 +617,7 @@ int gb200_matrix_dense_ptr(gb200_matrix_t A, void** d_vals) {
 int gb200_matrix_storage(gb200_matrix_t A, int* out) {
   if (A == NULL || out == NULL) return rc(graphblas::GrB_NULL_POINTER);
   graphblas::Storage s;
-  Info info = A->f ? A->f->getStorage(&s) : A->i->getStorage(&s);
+  Info info = onMatrix(A, [&](auto M) { return M->getStorage(&s); });
   *out = static_cast<int>(s);
   return rc(info);
 }
@@ -632,8 +627,10 @@ int gb200_matrix_tril(gb200_matrix_t A, gb200_desc_t desc) {
   GB200_REQUIRE_DEVICE();
   Info info = desc->desc.set(graphblas::GrB_BACKEND, graphblas::GrB_SEQUENTIAL);
   if (info == GrB_SUCCESS) {
-    if (A->f) info = graphblas::tril<float, float>(A->f, A->f, &desc->desc);
-    else      info = graphblas::tril<int, int>(A->i, A->i, &desc->desc);
+    info = onMatrix(A, [&](auto M) {
+      using T = decltype(elementOf(M));
+      return graphblas::tril<T, T>(M, M, &desc->desc);
+    });
   }
   desc->desc.set(graphblas::GrB_BACKEND, graphblas::GrB_CUDA);
   return rc(info);
@@ -674,7 +671,6 @@ int gb200_vector_new(gb200_vector_t* out, int dtype, int size) {
   if (size <= 0) return rc(graphblas::GrB_INVALID_VALUE);
   GB200_REQUIRE_DEVICE();
   gb200_vector_s* v = new gb200_vector_s();
-  v->dtype = dtype;
   v->f = new graphblas::Vector<float>(size);
   *out = v;
   return 0;
@@ -836,14 +832,13 @@ int gb200_vxm(gb200_vector_t w, gb200_vector_t mask, int use_accum,
     return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
   if (A->f == NULL) return rc(graphblas::GrB_DOMAIN_MISMATCH);
   GB200_REQUIRE_DEVICE();
-  GB200_SEMIRING_DISPATCH(semiring, {
+  return withSemiring(semiring, [&](auto op) {
     if (use_accum)
       return rc((graphblas::vxm<float, float, float, float>(vec(w), vec(mask),
           graphblas::plus<float>(), op, vec(u), A->f, &desc->desc)));
     return rc((graphblas::vxm<float, float, float, float>(vec(w), vec(mask),
         GrB_NULL, op, vec(u), A->f, &desc->desc)));
   });
-  return 0;
 }
 
 int gb200_mxv(gb200_vector_t w, gb200_vector_t mask, int use_accum,
@@ -853,35 +848,29 @@ int gb200_mxv(gb200_vector_t w, gb200_vector_t mask, int use_accum,
     return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
   if (A->f == NULL) return rc(graphblas::GrB_DOMAIN_MISMATCH);
   GB200_REQUIRE_DEVICE();
-  GB200_SEMIRING_DISPATCH(semiring, {
+  return withSemiring(semiring, [&](auto op) {
     if (use_accum)
       return rc((graphblas::mxv<float, float, float, float>(vec(w), vec(mask),
           graphblas::plus<float>(), op, A->f, vec(u), &desc->desc)));
     return rc((graphblas::mxv<float, float, float, float>(vec(w), vec(mask),
         GrB_NULL, op, A->f, vec(u), &desc->desc)));
   });
-  return 0;
 }
 
 int gb200_mxm(gb200_matrix_t C, gb200_matrix_t mask, int semiring,
               gb200_matrix_t A, gb200_matrix_t B, gb200_desc_t desc) {
   if (C == NULL || A == NULL || B == NULL || desc == NULL)
     return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
-  const bool fp32 = C->f != NULL && A->f != NULL && B->f != NULL;
   // a float mask only reaches the backend beside a dense operand, which refuses it
-  const bool dense_operand = fp32 &&
-      (A->f->matrix_.isDense() || B->f->matrix_.isDense());
-  if (fp32 && (mask == NULL || (dense_operand && mask->f != NULL))) {
+  if (allFp32(C, A, B, mask) &&
+      (mask == NULL || A->f->matrix_.isDense() || B->f->matrix_.isDense())) {
     GB200_REQUIRE_DEVICE();
-    GB200_SEMIRING_DISPATCH(semiring, {
+    return withSemiring(semiring, [&](auto op) {
       return rc((graphblas::mxm<float, float, float, float>(C->f,
           mask != NULL ? mask->f : NULL, GrB_NULL, op, A->f, B->f, &desc->desc)));
     });
-    return 0;
   }
-  if (C->i == NULL || A->i == NULL || B->i == NULL ||
-      (mask != NULL && mask->i == NULL))
-    return rc(graphblas::GrB_DOMAIN_MISMATCH);
+  if (!allInt32(C, A, B, mask)) return rc(graphblas::GrB_DOMAIN_MISMATCH);
   if (semiring != GB200_PLUS_MULTIPLIES)
     return rc(graphblas::GrB_NOT_IMPLEMENTED);
   GB200_REQUIRE_DEVICE();
@@ -904,13 +893,12 @@ int gb200_transpose(gb200_matrix_t C, gb200_matrix_t mask, gb200_matrix_t A,
                     gb200_desc_t desc) {
   if (C == NULL || A == NULL || desc == NULL)
     return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
-  if (C->f != NULL && A->f != NULL && (mask == NULL || mask->f != NULL)) {
+  if (allFp32(C, A, mask)) {
     GB200_REQUIRE_DEVICE();
     return rc((graphblas::transpose<float, float, float>(C->f,
         mask != NULL ? mask->f : NULL, GrB_NULL, A->f, &desc->desc)));
   }
-  if (C->i == NULL || A->i == NULL || (mask != NULL && mask->i == NULL))
-    return rc(graphblas::GrB_DOMAIN_MISMATCH);
+  if (!allInt32(C, A, mask)) return rc(graphblas::GrB_DOMAIN_MISMATCH);
   GB200_REQUIRE_DEVICE();
   return rc((graphblas::transpose<int, int, int>(C->i, mask ? mask->i : NULL, GrB_NULL,
       A->i, &desc->desc)));
@@ -921,11 +909,10 @@ int gb200_ewise_add(gb200_vector_t w, gb200_vector_t mask, int semiring,
   if (w == NULL || u == NULL || v == NULL || desc == NULL)
     return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
   GB200_REQUIRE_DEVICE();
-  GB200_SEMIRING_DISPATCH(semiring, {
+  return withSemiring(semiring, [&](auto op) {
     return rc((graphblas::eWiseAdd<float, float, float, float>(vec(w),
         vec(mask), GrB_NULL, op, vec(u), vec(v), &desc->desc)));
   });
-  return 0;
 }
 
 int gb200_ewise_add_scalar(gb200_vector_t w, gb200_vector_t mask, int semiring,
@@ -933,12 +920,11 @@ int gb200_ewise_add_scalar(gb200_vector_t w, gb200_vector_t mask, int semiring,
   if (w == NULL || u == NULL || desc == NULL)
     return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
   GB200_REQUIRE_DEVICE();
-  GB200_SEMIRING_DISPATCH(semiring, {
+  return withSemiring(semiring, [&](auto op) {
     return rc((graphblas::eWiseAdd<float, float, float, float>(vec(w),
         vec(mask), GrB_NULL, op, vec(u), static_cast<float>(val),
         &desc->desc)));
   });
-  return 0;
 }
 
 int gb200_ewise_mult(gb200_vector_t w, gb200_vector_t mask, int semiring,
@@ -946,11 +932,10 @@ int gb200_ewise_mult(gb200_vector_t w, gb200_vector_t mask, int semiring,
   if (w == NULL || u == NULL || v == NULL || desc == NULL)
     return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
   GB200_REQUIRE_DEVICE();
-  GB200_SEMIRING_DISPATCH(semiring, {
+  return withSemiring(semiring, [&](auto op) {
     return rc((graphblas::eWiseMult<float, float, float, float>(vec(w),
         vec(mask), GrB_NULL, op, vec(u), vec(v), &desc->desc)));
   });
-  return 0;
 }
 
 int gb200_assign_scalar(gb200_vector_t w, gb200_vector_t mask, double val,
@@ -969,14 +954,13 @@ int gb200_reduce_vector(double* out, int monoid, gb200_vector_t u,
   if (out == NULL || u == NULL || desc == NULL)
     return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
   GB200_REQUIRE_DEVICE();
-  float val = 0.f;
-  GB200_MONOID_DISPATCH(monoid, float, {
+  return withMonoid<float>(monoid, [&](auto op) {
+    float val = 0.f;
     Info info = graphblas::reduce<float, float>(&val, GrB_NULL, op, vec(u),
         &desc->desc);
     *out = val;
     return rc(info);
   });
-  return 0;
 }
 
 int gb200_reduce_matrix(double* out, int monoid, gb200_matrix_t A,
@@ -984,23 +968,21 @@ int gb200_reduce_matrix(double* out, int monoid, gb200_matrix_t A,
   if (out == NULL || A == NULL || desc == NULL)
     return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
   GB200_REQUIRE_DEVICE();
-  if (A->f) {
-    float val = 0.f;
-    GB200_MONOID_DISPATCH(monoid, float, {
+  if (A->f != NULL) {
+    return withMonoid<float>(monoid, [&](auto op) {
+      float val = 0.f;
       Info info = graphblas::reduce<float, float>(&val, GrB_NULL, op, A->f,
           &desc->desc);
       *out = val;
       return rc(info);
     });
-  } else {
-    if (monoid != GB200_PLUS_MONOID) return rc(graphblas::GrB_NOT_IMPLEMENTED);
-    int val = 0;
-    Info info = graphblas::reduce<int, int>(&val, GrB_NULL,
-        graphblas::PlusMonoid<int>(), A->i, &desc->desc);
-    *out = val;
-    return rc(info);
   }
-  return 0;
+  if (monoid != GB200_PLUS_MONOID) return rc(graphblas::GrB_NOT_IMPLEMENTED);
+  int val = 0;
+  Info info = graphblas::reduce<int, int>(&val, GrB_NULL,
+      graphblas::PlusMonoid<int>(), A->i, &desc->desc);
+  *out = val;
+  return rc(info);
 }
 
 int gb200_reduce_matrix_rows(gb200_vector_t w, int monoid, gb200_matrix_t A,
@@ -1009,11 +991,10 @@ int gb200_reduce_matrix_rows(gb200_vector_t w, int monoid, gb200_matrix_t A,
     return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
   if (A->f == NULL) return rc(graphblas::GrB_DOMAIN_MISMATCH);
   GB200_REQUIRE_DEVICE();
-  GB200_MONOID_DISPATCH(monoid, float, {
+  return withMonoid<float>(monoid, [&](auto op) {
     return rc((graphblas::reduce<float, float, float>(vec(w), GrB_NULL,
         GrB_NULL, op, A->f, &desc->desc)));
   });
-  return 0;
 }
 
 // ---- Algorithms ---------------------------------------------------------------
@@ -1027,12 +1008,9 @@ int gb200_bfs(gb200_vector_t v, gb200_matrix_t A, int source, gb200_desc_t desc,
   A->f->nrows(&n);
   if (source < 0 || source >= n) return rc(graphblas::GrB_INVALID_INDEX);
   GB200_REQUIRE_DEVICE();
-  graphblas::algorithm::lastStatus() = graphblas::GrB_SUCCESS;
-  const float ms = graphblas::algorithm::bfs(v->f, A->f, source, &desc->desc,
-                                             tight_ms != NULL);
-  if (ms < 0.f) return rc(graphblas::algorithm::lastStatus());
-  if (tight_ms) *tight_ms = ms;
-  return 0;
+  return runAlgorithm(tight_ms, [&] {
+    return graphblas::algorithm::bfs(v->f, A->f, source, &desc->desc, tight_ms != NULL);
+  });
 }
 
 // scatter / assignScatter / extractGather (reference graphblas/operations.hpp:
@@ -1079,11 +1057,9 @@ int gb200_sssp(gb200_vector_t v, gb200_matrix_t A, int source,
   A->f->nrows(&n);
   if (source < 0 || source >= n) return rc(graphblas::GrB_INVALID_INDEX);
   GB200_REQUIRE_DEVICE();
-  graphblas::algorithm::lastStatus() = graphblas::GrB_SUCCESS;
-  float ms = graphblas::algorithm::sssp(v->f, A->f, source, &desc->desc);
-  if (ms < 0.f) return rc(graphblas::algorithm::lastStatus());
-  if (tight_ms) *tight_ms = ms;
-  return 0;
+  return runAlgorithm(tight_ms, [&] {
+    return graphblas::algorithm::sssp(v->f, A->f, source, &desc->desc);
+  });
 }
 
 int gb200_gc(gb200_vector_t v, gb200_matrix_t A, int seed, gb200_desc_t desc,
@@ -1093,14 +1069,13 @@ int gb200_gc(gb200_vector_t v, gb200_matrix_t A, int seed, gb200_desc_t desc,
   if (A->f == NULL && A->i == NULL) return rc(graphblas::GrB_DOMAIN_MISMATCH);
   GB200_REQUIRE_DEVICE();
   int count = 0;
-  graphblas::algorithm::lastStatus() = graphblas::GrB_SUCCESS;
-  const float ms = A->f != NULL
-      ? graphblas::algorithm::gc(v->f, A->f, seed, &desc->desc, &count)
-      : graphblas::algorithm::gc(v->f, A->i, seed, &desc->desc, &count);
-  if (ms < 0.f) return rc(graphblas::algorithm::lastStatus());
-  if (ncolors) *ncolors = count;
-  if (tight_ms) *tight_ms = ms;
-  return 0;
+  const int info = runAlgorithm(tight_ms, [&] {
+    return onMatrix(A, [&](auto M) {
+      return graphblas::algorithm::gc(v->f, M, seed, &desc->desc, &count);
+    });
+  });
+  if (info == 0 && ncolors) *ncolors = count;
+  return info;
 }
 
 int gb200_mis(gb200_vector_t v, gb200_matrix_t A, int seed, gb200_vector_t candidates,
@@ -1111,14 +1086,13 @@ int gb200_mis(gb200_vector_t v, gb200_matrix_t A, int seed, gb200_vector_t candi
   GB200_REQUIRE_DEVICE();
   int count = 0;
   const graphblas::Vector<float>* cand = candidates != NULL ? candidates->f : NULL;
-  graphblas::algorithm::lastStatus() = graphblas::GrB_SUCCESS;
-  const float ms = A->f != NULL
-      ? graphblas::algorithm::mis(v->f, A->f, seed, &desc->desc, &count, cand)
-      : graphblas::algorithm::mis(v->f, A->i, seed, &desc->desc, &count, cand);
-  if (ms < 0.f) return rc(graphblas::algorithm::lastStatus());
-  if (nmembers) *nmembers = count;
-  if (tight_ms) *tight_ms = ms;
-  return 0;
+  const int info = runAlgorithm(tight_ms, [&] {
+    return onMatrix(A, [&](auto M) {
+      return graphblas::algorithm::mis(v->f, M, seed, &desc->desc, &count, cand);
+    });
+  });
+  if (info == 0 && nmembers) *nmembers = count;
+  return info;
 }
 
 int gb200_cc(gb200_vector_t v, gb200_matrix_t A, gb200_desc_t desc, int* ncomponents,
@@ -1128,14 +1102,13 @@ int gb200_cc(gb200_vector_t v, gb200_matrix_t A, gb200_desc_t desc, int* ncompon
   if (A->f == NULL && A->i == NULL) return rc(graphblas::GrB_DOMAIN_MISMATCH);
   GB200_REQUIRE_DEVICE();
   int count = 0;
-  graphblas::algorithm::lastStatus() = graphblas::GrB_SUCCESS;
-  const float ms = A->f != NULL
-      ? graphblas::algorithm::cc(v->f, A->f, &desc->desc, &count)
-      : graphblas::algorithm::cc(v->f, A->i, &desc->desc, &count);
-  if (ms < 0.f) return rc(graphblas::algorithm::lastStatus());
-  if (ncomponents) *ncomponents = count;
-  if (tight_ms) *tight_ms = ms;
-  return 0;
+  const int info = runAlgorithm(tight_ms, [&] {
+    return onMatrix(A, [&](auto M) {
+      return graphblas::algorithm::cc(v->f, M, &desc->desc, &count);
+    });
+  });
+  if (info == 0 && ncomponents) *ncomponents = count;
+  return info;
 }
 
 int gb200_pr(gb200_vector_t p, gb200_matrix_t A, float alpha, float eps,
@@ -1144,26 +1117,23 @@ int gb200_pr(gb200_vector_t p, gb200_matrix_t A, float alpha, float eps,
     return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
   if (A->f == NULL) return rc(graphblas::GrB_DOMAIN_MISMATCH);
   GB200_REQUIRE_DEVICE();
-  graphblas::algorithm::lastStatus() = graphblas::GrB_SUCCESS;
-  float ms = graphblas::algorithm::pr(p->f, A->f, alpha, eps, &desc->desc);
-  if (ms < 0.f) return rc(graphblas::algorithm::lastStatus());
-  if (tight_ms) *tight_ms = ms;
-  return 0;
+  return runAlgorithm(tight_ms, [&] {
+    return graphblas::algorithm::pr(p->f, A->f, alpha, eps, &desc->desc);
+  });
 }
 
 int gb200_tc(long long* ntris, gb200_matrix_t A, gb200_matrix_t B,
              gb200_desc_t desc, float* tight_ms) {
   if (ntris == NULL || A == NULL || B == NULL || desc == NULL)
     return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
-  if (A->i == NULL || B->i == NULL) return rc(graphblas::GrB_DOMAIN_MISMATCH);
+  if (!allInt32(A, B)) return rc(graphblas::GrB_DOMAIN_MISMATCH);
   GB200_REQUIRE_DEVICE();
   int count = 0;
-  graphblas::algorithm::lastStatus() = graphblas::GrB_SUCCESS;
-  float ms = graphblas::algorithm::tc(&count, A->i, B->i, &desc->desc);
-  if (ms < 0.f) return rc(graphblas::algorithm::lastStatus());
-  *ntris = count;
-  if (tight_ms) *tight_ms = ms;
-  return 0;
+  const int info = runAlgorithm(tight_ms, [&] {
+    return graphblas::algorithm::tc(&count, A->i, B->i, &desc->desc);
+  });
+  if (info == 0) *ntris = count;
+  return info;
 }
 
 // ---- Vector as a bitmap ---------------------------------------------------------
@@ -1240,32 +1210,6 @@ int gb200_launch_count(unsigned long long* out) {
 }
 
 // ---- Graph ingest -------------------------------------------------------------
-
-__global__ void rmatEdgesKernel(int scale, long long nedges,
-                                unsigned long long seed, long long first_edge,
-                                int* __restrict__ src, int* __restrict__ dst) {
-  const unsigned int T1 = 2448131358u, T2 = 3264175144u, T3 = 4080218930u;
-  long long e = static_cast<long long>(blockIdx.x)*blockDim.x + threadIdx.x;
-  const long long stride = static_cast<long long>(gridDim.x)*blockDim.x;
-  for (; e < nedges; e += stride) {
-    const unsigned long long ge = static_cast<unsigned long long>(first_edge + e);
-    unsigned int s = 0, d = 0;
-    for (int l = 0; l < scale; ++l) {
-      unsigned long long z = ((seed << 48) ^ (ge << 6) ^
-          static_cast<unsigned long long>(l)) + 0x9E3779B97F4A7C15ull;
-      z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-      z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-      z = z ^ (z >> 31);
-      const unsigned int r = static_cast<unsigned int>(z >> 32);
-      const unsigned int sb = (r >= T2) ? 1u : 0u;
-      const unsigned int db = ((r >= T1 && r < T2) || r >= T3) ? 1u : 0u;
-      s = (s << 1) | sb;
-      d = (d << 1) | db;
-    }
-    src[e] = static_cast<int>(s);
-    dst[e] = static_cast<int>(d);
-  }
-}
 
 int gb200_rmat_edges(int scale, long long nedges, unsigned long long seed,
                      long long first_edge, int* d_src, int* d_dst) {

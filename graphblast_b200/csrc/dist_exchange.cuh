@@ -382,7 +382,7 @@ int gb200_dist_sssp(gb200_xchg_t x, gb200_vector_t v, gb200_matrix_t M,
   Vector<float>* frontier = x->ss_vec[0];
   Vector<float>* relaxed  = x->ss_vec[1];
   Vector<float>* improved = x->ss_vec[2];
-  gb200_vector_s relaxed_h = {GB200_FP32, relaxed};
+  gb200_vector_s relaxed_h = {relaxed};
 
   const bool own_src = source >= static_cast<long long>(lo) &&
                        source < static_cast<long long>(lo) + nl;

@@ -232,11 +232,6 @@ class SparseMatrix {
   static X* hostArray(size_t count) { return reinterpret_cast<X*>(malloc(count*sizeof(X))); }
   template <typename X>
   static X* devArray(size_t count) { return reinterpret_cast<X*>(gbMalloc(count*sizeof(X))); }
-  template <typename X>
-  static void copyAsync(X* dst, const X* src, size_t count, cudaMemcpyKind kind) {
-    if (count > 0 && dst != NULL && src != NULL && dst != src)
-      CUDA_CALL(cudaMemcpyAsync(dst, src, count*sizeof(X), kind, gbStream()));
-  }
   void transfer(Side dst, Side src, cudaMemcpyKind kind, bool with_indices) {
     if (with_indices) {
       copyAsync(dst.ptr, src.ptr, static_cast<size_t>(dst.dim) + 1, kind);

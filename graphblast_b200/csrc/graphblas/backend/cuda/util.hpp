@@ -246,6 +246,14 @@ inline void gbFree(void* p) {
   if (p != NULL) (void)cudaFreeAsync(p, runtime().stream);
 }
 
+// Copy of count elements on the backend stream; none for an empty count, a NULL
+// end or a copy of an array onto itself.
+template <typename X>
+void copyAsync(X* dst, const X* src, size_t count, cudaMemcpyKind kind) {
+  if (count > 0 && dst != NULL && src != NULL && dst != src)
+    CUDA_CALL(cudaMemcpyAsync(dst, src, count*sizeof(X), kind, gbStream()));
+}
+
 // CTAs of NT threads of the cooperative kernel K that fit on the device at once: the
 // grid of its cooperative launch.  The occupancy query runs on the first call and is
 // cached per kernel; 0 when no CTA fits.
