@@ -57,14 +57,15 @@ Info assignDense(DenseVector<W>* w, Vector<M>* mask, BinaryOpT accum, T val,
   bool bits_kept = false;
   if (mask_vec_type == GrB_DENSE) {
     const int grid = gridFor(w->nvals_, 256);
-    if (mask->dense_.bits_valid_) {
-      unsigned int* w_bits = w->bits_valid_ ? w->d_bits_ : NULL;
+    const unsigned int* mask_bits = mask->dense_.exactBits();
+    if (mask_bits != NULL) {
+      unsigned int* w_bits = w->exactBits();
       if (use_scmp)
         assignDenseBitsMaskKernel<true><<<grid, 256, 0, s>>>(w->d_val_, w_bits,
-            w->nvals_, mask->dense_.d_bits_, static_cast<W>(val));
+            w->nvals_, mask_bits, static_cast<W>(val));
       else
         assignDenseBitsMaskKernel<false><<<grid, 256, 0, s>>>(w->d_val_, w_bits,
-            w->nvals_, mask->dense_.d_bits_, static_cast<W>(val));
+            w->nvals_, mask_bits, static_cast<W>(val));
       bits_kept = (w_bits != NULL);
     } else if (use_scmp) {
       assignDenseDenseMaskKernel<true><<<grid, 256, 0, s>>>(w->d_val_,
@@ -80,9 +81,10 @@ Info assignDense(DenseVector<W>* w, Vector<M>* mask, BinaryOpT accum, T val,
       std::cout << "Error: Feature not implemented yet!\n";
     } else if (mask->sparse_.nvals_ > 0) {
       const int grid = gridFor(mask->sparse_.nvals_, 256);
-      if (w->bits_valid_) {
+      unsigned int* w_bits = w->exactBits();
+      if (w_bits != NULL) {
         assignDenseSparseMaskBitsKernel<<<grid, 256, 0, s>>>(w->d_val_,
-            w->d_bits_, mask->sparse_.d_ind_, mask->sparse_.nvals_,
+            w_bits, mask->sparse_.d_ind_, mask->sparse_.nvals_,
             static_cast<W>(val));
         bits_kept = true;
       } else {
@@ -91,13 +93,12 @@ Info assignDense(DenseVector<W>* w, Vector<M>* mask, BinaryOpT accum, T val,
       }
       GB_KERNEL_CHECK();
     } else {
-      bits_kept = w->bits_valid_;
+      bits_kept = (w->exactBits() != NULL);
     }
   } else {
     return GrB_UNINITIALIZED_OBJECT;
   }
-  w->touched();
-  w->bits_valid_ = bits_kept;
+  w->wroteUnderMask(bits_kept);
   return GrB_SUCCESS;
 }
 
@@ -158,8 +159,7 @@ Info assignSparse(SparseVector<W>* w, Vector<M>* mask, BinaryOpT accum, T val,
     CUDA_CALL(cudaMemcpyAsync(w->d_val_, tmp_val, kept*sizeof(W),
         cudaMemcpyDeviceToDevice, s));
   }
-  w->nvals_ = kept;
-  w->need_update_ = true;
+  w->computed(kept);
   return GrB_SUCCESS;
 }
 }  // namespace backend

@@ -33,7 +33,9 @@ Index compactOrdered(Source src, Index nitems, Descriptor* desc) {
   compactEmitKernel<<<nblocks, GB_COMPACT_NT, 0, s>>>(src, nitems,
       block_counts);
   GB_KERNEL_CHECK();
-  return static_cast<Index>(runtime().mailWait(0, ticket, ctr));
+  unsigned long long total;
+  if (!runtime().mailWait(0, ticket, &total)) total = runtime().fetch(ctr);
+  return static_cast<Index>(total);
 }
 
 }  // namespace backend

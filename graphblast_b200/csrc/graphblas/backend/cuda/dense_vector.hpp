@@ -12,8 +12,9 @@
 //  * the vector carries facts ABOUT its contents that the traversal kernels leave
 //    behind or consume: the count of non-identity entries (nnz_valid_, or still on
 //    the device: count_pending_), "contents are exactly 0/1" (zero_one_), a bitmap
-//    shadow (bits_valid_), and "only the bitmap is current" (vals_stale_).  Every
-//    write to the values goes through contentChanged(), which forgets them.
+//    shadow (bits_valid_), and "only the bitmap is current" (vals_stale_).  They are
+//    private: a write reports itself through touched(), wroteBooleanPull(),
+//    wroteUnderMask() or scattered(); exactBits(), valuesStale(), holdsZeroOne() read.
 #ifndef GRAPHBLAS_BACKEND_CUDA_DENSE_VECTOR_HPP_
 #define GRAPHBLAS_BACKEND_CUDA_DENSE_VECTOR_HPP_
 
@@ -90,9 +91,10 @@ class DenseVector {
     if (!(nnz_valid_ && same_identity)) {
       if (count_pending_ && same_identity && d_count_ != NULL) {
         // posted to the host mailbox by the producing kernel, or read from its cell
-        nnz_ = (count_ticket_ != 0ull)
-            ? static_cast<Index>(runtime().mailWait(1, count_ticket_, d_count_))
-            : static_cast<Index>(runtime().fetch(d_count_));
+        unsigned long long posted;
+        nnz_ = static_cast<Index>(
+            (count_ticket_ != 0ull && runtime().mailWait(1, count_ticket_, &posted))
+                ? posted : runtime().fetch(d_count_));
       } else {
         CHECK(allocateGpu());
         CHECK(materialize());
@@ -318,6 +320,34 @@ class DenseVector {
   // ---- facts about the contents -----------------------------------------------------------
   // A kernel wrote the values.
   void touched() { contentChanged(); }
+  // The fused Boolean pull wrote 0/1 (with `bits_only`: the bitmap shadow alone) and
+  // counted the ones into countCell() and, unless `ticket` is 0, the mailbox.
+  void wroteBooleanPull(bool bits_only, unsigned long long ticket) {
+    contentChanged();
+    bits_valid_    = bits_only;
+    vals_stale_    = bits_only;
+    count_pending_ = true;
+    count_ticket_  = ticket;
+    zero_one_      = true;
+    nnz_identity_  = T(0);
+  }
+  // A masked constant assign wrote the values; `bits_exact`: it kept the shadow in step.
+  void wroteUnderMask(bool bits_exact) {
+    contentChanged();
+    bits_valid_ = bits_exact;
+  }
+  // A sparse vector of nnz entries was scattered into these values.  Under --opreuse
+  // nothing was written, so the pending count, zero_one_ and vals_stale_ stay as they are.
+  void scattered(Index nnz, bool bits_exact) {
+    need_update_ = true;
+    nnz_         = nnz;
+    nnz_valid_   = false;
+    bits_valid_  = bits_exact;
+  }
+  // The bitmap shadow when it is exact, else NULL.
+  unsigned int* exactBits() const { return bits_valid_ ? d_bits_ : NULL; }
+  bool valuesStale() const  { return vals_stale_; }
+  bool holdsZeroOne() const { return zero_one_; }
 
   // Lazy values.  The fused Boolean pull publishes its 0/1 result through the
   // bitmap shadow only and sets vals_stale_; every consumer inside a traversal
@@ -369,8 +399,9 @@ class DenseVector {
   T*    h_val_ = NULL;
   T*    d_val_ = NULL;
   bool  need_update_ = false;    // device copy newer than host copy
-  bool  owns_device_ = true;
 
+ private:
+  bool  owns_device_ = true;
   bool  nnz_valid_ = false;      // nnz_ counts entries != nnz_identity_ of the current data
   T     nnz_identity_ = T();
   // Count left on the device by the kernel that produced the current contents
@@ -388,7 +419,6 @@ class DenseVector {
   size_t bits_alloc_words_ = 0;
   bool   vals_stale_ = false;    // only the bitmap is current
 
- private:
   static size_t bytes(Index count) { return static_cast<size_t>(count)*sizeof(T); }
   // The values were (or are about to be) overwritten: the host mirror is behind and
   // nothing derived from the old contents holds any more.

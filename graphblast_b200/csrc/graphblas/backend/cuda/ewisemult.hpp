@@ -65,8 +65,7 @@ Info eWiseMultInner(SparseVector<W>* w, const SparseVector<M>* mask, BinaryOpT a
         extractMul(op), u->d_val_, v->d_val_);
     GB_KERNEL_CHECK();
   }
-  w->nvals_ = mask_nvals;
-  w->need_update_ = true;
+  w->computed(mask_nvals);
   return GrB_SUCCESS;
 }
 
@@ -91,8 +90,7 @@ Info eWiseMultInner(SparseVector<W>* w, const Vector<M>* mask, BinaryOpT accum,
           op.identity(), extractMul(op), u->d_ind_, u->d_val_, nu, v->d_val_, reverse);
       GB_KERNEL_CHECK();
     }
-    w->nvals_ = mask_nvals;
-    w->need_update_ = true;
+    w->computed(mask_nvals);
     return GrB_SUCCESS;
   }
   Index u_nvals;
@@ -111,8 +109,7 @@ Info eWiseMultInner(SparseVector<W>* w, const Vector<M>* mask, BinaryOpT accum,
       GB_KERNEL_CHECK();
     }
   }
-  w->nvals_ = u_nvals;
-  w->need_update_ = true;
+  w->computed(u_nvals);
   return GrB_SUCCESS;
 }
 

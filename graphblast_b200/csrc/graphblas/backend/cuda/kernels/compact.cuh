@@ -14,6 +14,7 @@
 #define GRAPHBLAS_BACKEND_CUDA_KERNELS_COMPACT_CUH_
 
 #include "graphblas/backend/cuda/kernels/common.cuh"
+#include "graphblas/backend/cuda/kernels/util.cuh"
 
 namespace graphblas {
 namespace backend {
@@ -66,10 +67,7 @@ compactCountScanKernel(Source src, Index nitems, int* __restrict__ block_counts,
   if (threadIdx.x == 0) {
     *total_out = static_cast<unsigned long long>(s_carry);
     *done = 0ull;
-    // post the total to the host (util.hpp mailbox)
-    *reinterpret_cast<volatile unsigned long long*>(mail) =
-        (ticket << 40) | static_cast<unsigned long long>(s_carry);
-    __threadfence_system();
+    mailPost(mail, ticket, static_cast<unsigned long long>(s_carry));   // total to the host
   }
 }
 

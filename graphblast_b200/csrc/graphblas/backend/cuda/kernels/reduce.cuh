@@ -6,6 +6,7 @@
 #define GRAPHBLAS_BACKEND_CUDA_KERNELS_REDUCE_CUH_
 
 #include "graphblas/backend/cuda/kernels/common.cuh"
+#include "graphblas/backend/cuda/kernels/util.cuh"
 
 namespace graphblas {
 namespace backend {
@@ -59,9 +60,7 @@ reduceFinalKernel(T* __restrict__ out, const T* __restrict__ partials,
     if (mail != NULL && sizeof(T) == 4) {   // post to the host (util.hpp mailbox)
       unsigned int bits;
       memcpy(&bits, &total, 4);
-      *reinterpret_cast<volatile unsigned long long*>(mail) =
-          (ticket << 40) | static_cast<unsigned long long>(bits);
-      __threadfence_system();
+      mailPost(mail, ticket, bits);
     }
   }
 }

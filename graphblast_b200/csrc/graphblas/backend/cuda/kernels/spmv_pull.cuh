@@ -24,6 +24,7 @@
 #define GRAPHBLAS_BACKEND_CUDA_KERNELS_SPMV_PULL_CUH_
 
 #include "graphblas/backend/cuda/kernels/common.cuh"
+#include "graphblas/backend/cuda/kernels/util.cuh"
 
 namespace graphblas {
 namespace backend {
@@ -564,9 +565,7 @@ spmvMaskedOrPullBitsKernel(unsigned int* __restrict__       w_bits,
       const unsigned long long count =
           *reinterpret_cast<volatile unsigned long long*>(discovered);
       *done = 0ull;
-      *reinterpret_cast<volatile unsigned long long*>(mail) =
-          (ticket << 40) | count;
-      __threadfence_system();
+      mailPost(mail, ticket, count);
     }
   }
 }

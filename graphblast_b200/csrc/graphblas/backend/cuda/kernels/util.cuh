@@ -170,14 +170,18 @@ frontierDegreeScanKernel(Index* __restrict__ offs,
   }
 }
 
-// Posts one device-side Index to the host mailbox (backend/cuda/util.hpp).
+// Posts a value of at most 40 bits to a host mailbox slot (backend/cuda/util.hpp).
+__device__ __forceinline__ void mailPost(unsigned long long* mail, unsigned long long ticket,
+                                         unsigned long long value) {
+  *reinterpret_cast<volatile unsigned long long*>(mail) = (ticket << 40) | value;
+  __threadfence_system();
+}
+
+// Posts one device-side Index to the host mailbox.
 __global__ void postIndexKernel(const Index* __restrict__ value,
                                 unsigned long long* mail,
                                 unsigned long long ticket) {
-  *reinterpret_cast<volatile unsigned long long*>(mail) =
-      (ticket << 40) | static_cast<unsigned long long>(
-          static_cast<unsigned int>(*value));
-  __threadfence_system();
+  mailPost(mail, ticket, static_cast<unsigned int>(*value));
 }
 
 // Binary search helper kept for API parity with reference kernels/util.hpp:8-24.

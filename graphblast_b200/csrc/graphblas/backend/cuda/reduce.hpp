@@ -27,23 +27,13 @@ Info reduceFold(T* val, MonoidT op, T* partials, int grid) {
   reduceFinalKernel<<<1, GB_REDUCE_NT, 0, s>>>(d_out, partials, grid, op,
       static_cast<T>(op.identity()), mail ? runtime().mailSlot(2) : NULL, ticket);
   GB_KERNEL_CHECK();
-  if (mail) {
-    // fallback cell holds a T; read it as such if the post is lost
-    volatile unsigned long long* slot = runtime().h_mail + 2;
-    const auto t0 = std::chrono::steady_clock::now();
-    for (unsigned long long spin = 0;; ++spin) {
-      const unsigned long long v = *slot;
-      if ((v >> 40) == ticket) {
-        const unsigned int bits = static_cast<unsigned int>(v & 0xffffffffull);
-        memcpy(val, &bits, 4);
-        return GrB_SUCCESS;
-      }
-      if ((spin & 0x3ff) == 0x3ff &&
-          std::chrono::steady_clock::now() - t0 > std::chrono::seconds(2))
-        break;
-    }
+  unsigned long long posted;
+  if (mail && runtime().mailWait(2, ticket, &posted)) {
+    const unsigned int bits = static_cast<unsigned int>(posted & 0xffffffffull);
+    memcpy(val, &bits, 4);
+    return GrB_SUCCESS;
   }
-  *val = runtime().fetch(d_out);
+  *val = runtime().fetch(d_out);              // the cell holds a T: read it as such
   return GrB_SUCCESS;
 }
 
@@ -98,7 +88,7 @@ Info reduceStored(T* val, BinaryOpT accum, MonoidT op, const Container* x,
 template <typename T, typename U, typename BinaryOpT, typename MonoidT>
 Info reduceDense(T* val, BinaryOpT accum, MonoidT op, DenseVector<U>* u,
                  Descriptor* desc) {
-  const bool counts_ones = u->zero_one_ && op(3, 5) == 8 &&
+  const bool counts_ones = u->holdsZeroOne() && op(3, 5) == 8 &&
                            op.identity() == static_cast<T>(0);
   if (counts_ones) {
     Index ones;

@@ -77,9 +77,8 @@ class SparseVector {
     dropDevice();
     d_ind_ = indices;
     d_val_ = values;
-    nvals_ = nvals;
     owns_device_ = false;
-    need_update_ = true;
+    computed(nvals);
     return GrB_SUCCESS;
   }
 
@@ -169,6 +168,11 @@ class SparseVector {
     std::swap(owns_device_, rhs->owns_device_);
     return GrB_SUCCESS;
   }
+  // The device lists hold nvals entries (from a kernel, or adopted) the host lacks.
+  void computed(Index nvals) {
+    nvals_ = nvals;
+    need_update_ = true;
+  }
 
   // ---- storage --------------------------------------------------------------------------
   Info allocateCpu() {
@@ -222,9 +226,10 @@ class SparseVector {
   Index* d_ind_ = NULL;
   T*     d_val_ = NULL;
   bool   need_update_ = false;   // device copy newer than host copy
-  bool   owns_device_ = true;
 
  private:
+  bool   owns_device_ = true;
+
   static void copyLists(Index* ind_to, T* val_to, const Index* ind_from, const T* val_from,
                         Index count, cudaMemcpyKind kind) {
     if (count <= 0) return;

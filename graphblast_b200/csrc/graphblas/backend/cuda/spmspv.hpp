@@ -117,8 +117,7 @@ Info spmspvMerge(SparseVector<W>* w, const Vector<M>* mask, BinaryOpT accum,
   const Index nf = u->nvals_;
   CHECK(w->allocateGpu());
   if (nf == 0) {
-    w->nvals_       = 0;
-    w->need_update_ = true;
+    w->computed(0);
     return GrB_SUCCESS;
   }
 
@@ -129,7 +128,7 @@ Info spmspvMerge(SparseVector<W>* w, const Vector<M>* mask, BinaryOpT accum,
     CHECK(mask->getStorage(&mask_vec_type));
     if (mask_vec_type == GrB_DENSE) {
       mask_val = mask->dense_.d_val_;
-      if (mask->dense_.bits_valid_) mask_bits = mask->dense_.d_bits_;
+      mask_bits = mask->dense_.exactBits();
     } else if (mask_vec_type == GrB_SPARSE) {
       std::cout << "Spmspv Sparse Mask\n";
       std::cout << "Error: Feature not implemented yet!\n";
@@ -167,17 +166,9 @@ Info spmspvMerge(SparseVector<W>* w, const Vector<M>* mask, BinaryOpT accum,
     const unsigned long long ticket = runtime().mailTicket();
     postIndexKernel<<<1, 1, 0, s>>>(offs + nf, runtime().mailSlot(4), ticket);
     GB_KERNEL_CHECK();
-    long long ef = -1;
-    volatile unsigned long long* slot = runtime().h_mail + 4;
-    const auto t0 = std::chrono::steady_clock::now();
-    for (unsigned long long spin = 0;; ++spin) {
-      const unsigned long long v = *slot;
-      if ((v >> 40) == ticket) { ef = static_cast<long long>(v & 0xffffffffull); break; }
-      if ((spin & 0x3ff) == 0x3ff &&
-          std::chrono::steady_clock::now() - t0 > std::chrono::seconds(2))
-        break;
-    }
-    if (ef < 0) ef = runtime().fetch(offs + nf);
+    unsigned long long posted;
+    const long long ef = runtime().mailWait(4, ticket, &posted)
+        ? static_cast<long long>(posted & 0xffffffffull) : runtime().fetch(offs + nf);
     if (static_cast<double>(ef) > static_cast<double>(edge_switch)*A->nvals_) {
       if (desc->dirinfo())
         std::cout << "Frontier owns " << ef << " of " << A->nvals_
@@ -241,8 +232,7 @@ Info spmspvMerge(SparseVector<W>* w, const Vector<M>* mask, BinaryOpT accum,
     src.out_ind = w->d_ind_; src.out_val = w->d_val_;
     count = compactOrdered(src, nwords, desc);
   }
-  w->nvals_       = count;
-  w->need_update_ = true;
+  w->computed(count);
   if (profiler().enabled)
     profiler().host_bytes[GB_PROF_PUSH] += 8.0*count;   // (ind, val) written
 

@@ -241,17 +241,7 @@ Info spmv(DenseVector<W>* w, const Vector<M>* mask, BinaryOpT accum, SemiringT o
       GB_KERNEL_CHECK();
       // the inspected colind bytes are added on the device
       profiler().end(GB_PROF_PULL_BOOL, s, fixed_bytes);
-      w->touched();
-      w->bits_valid_ = bits_form;
-      // The bitmap form publishes its 0/1 result through the bitmap shadow only;
-      // the value array is written when somebody asks for it (materialize()).
-      w->vals_stale_ = bits_form;
-      // The kernel wrote 0/1 and counted the ones: the next convert() or
-      // a PlusMonoid reduce can reuse the count (one 8-byte read, no pass).
-      w->count_pending_ = true;
-      w->count_ticket_  = mail_ticket;     // 0: not posted to the mailbox
-      w->zero_one_      = true;
-      w->nnz_identity_  = static_cast<W>(0);
+      w->wroteBooleanPull(bits_form, mail_ticket);
       if (desc->debug())
         { w->materialize(); printDevice("w_val", w->d_val_, A_nrows); }
     } else if (mask_vec_type == GrB_SPARSE) {

@@ -177,8 +177,9 @@ struct Runtime {
   // launches next.  Reading it with cudaMemcpyAsync + cudaStreamSynchronize
   // waits for EVERYTHING queued on the stream and costs ~10 us of idle GPU per
   // level; instead the kernel that knows the value stores (ticket << 40 | value)
-  // into mapped pinned memory and the host polls that word, so it can go on as
-  // soon as the producing kernel is done, while later kernels still run.
+  // into mapped pinned memory (mailPost, kernels/util.cuh) and the host polls that
+  // word (mailWait), so it goes on once the producing kernel is done, while later
+  // kernels still run.  Slots: 0 compaction, 1 Boolean pull, 2 reduce, 4 push edges.
   unsigned long long* h_mail;     // pinned + mapped, 8 slots
   unsigned long long* d_mail;
   unsigned long long  mail_seq;
@@ -193,23 +194,21 @@ struct Runtime {
   // Ticket for the next post (24 bits, never 0) and where the kernel writes it.
   unsigned long long mailTicket() { mailInit(); mail_seq = (mail_seq % 0xfffffeull) + 1; return mail_seq; }
   unsigned long long* mailSlot(int slot) { mailInit(); return d_mail + slot; }
-  // Value posted under `ticket`; falls back to a stream-ordered read of
-  // d_fallback if the slot was reused by a later post or nothing arrives.
-  unsigned long long mailWait(int slot, unsigned long long ticket,
-      const unsigned long long* d_fallback) {
+  // The 40-bit value posted under `ticket`; false if the slot was reused by a later
+  // post or nothing arrives (the caller then reads its own cell stream-ordered).
+  bool mailWait(int slot, unsigned long long ticket, unsigned long long* value) {
     volatile unsigned long long* p = h_mail + slot;
     const auto t0 = std::chrono::steady_clock::now();
     for (unsigned long long spin = 0;; ++spin) {
       const unsigned long long v = *p;
       const unsigned long long got = v >> 40;
-      if (got == ticket) return v & ((1ull << 40) - 1ull);
+      if (got == ticket) { *value = v & ((1ull << 40) - 1ull); return true; }
       if (got != 0 && ((got - ticket) & 0xffffffull) < 0x800000ull)
-        break;                                  // overwritten by a later post
+        return false;                           // overwritten by a later post
       if ((spin & 0x3ff) == 0x3ff &&
           std::chrono::steady_clock::now() - t0 > std::chrono::seconds(2))
-        break;
+        return false;
     }
-    return fetch(d_fallback);
   }
 };
 

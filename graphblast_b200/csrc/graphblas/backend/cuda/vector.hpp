@@ -218,10 +218,10 @@ Info Vector<T>::sparse2dense(T identity, Descriptor* desc) {
       if (desc != NULL && desc->struconly()) {
         scatterConstKernel<<<gridFor(nvals, nt), nt, 0, gbStream()>>>(
             dense_.d_val_, sparse_.d_ind_, (T)1, nvals);
-        if (identity == static_cast<T>(0) && dense_.bits_valid_) {
+        if (identity == static_cast<T>(0) && dense_.exactBits() != NULL) {
           GB_KERNEL_CHECK();
           scatterBitsKernel<<<gridFor(nvals, nt), nt, 0, gbStream()>>>(
-              dense_.d_bits_, sparse_.d_ind_, nvals);
+              dense_.exactBits(), sparse_.d_ind_, nvals);
           keep_bits = true;
         }
       } else
@@ -231,11 +231,8 @@ Info Vector<T>::sparse2dense(T identity, Descriptor* desc) {
     }
   }
 
-  vec_type_            = GrB_DENSE;
-  dense_.need_update_  = true;
-  dense_.nnz_          = nvals;
-  dense_.nnz_valid_    = false;
-  dense_.bits_valid_   = keep_bits;
+  vec_type_ = GrB_DENSE;
+  dense_.scattered(nvals, keep_bits);
   return GrB_SUCCESS;
 }
 
@@ -255,23 +252,24 @@ Info Vector<T>::dense2sparse(T identity, Descriptor* desc) {
       GrB_LOAD_BALANCE_MERGE);
 
   // Lazy values are only tolerable on the structure-only bitmap path below.
-  if (dense_.vals_stale_ &&
+  if (dense_.valuesStale() &&
       !(identity == static_cast<T>(0) && desc->struconly() &&
         mxv_mode == GrB_LOAD_BALANCE_MERGE))
     CHECK(dense_.materialize());
 
   Index count;
-  if (dense_.bits_valid_ && identity == static_cast<T>(0)) {
+  const unsigned int* bits = dense_.exactBits();
+  if (bits != NULL && identity == static_cast<T>(0)) {
     // Compact the bitmap shadow: n/32 words instead of n values.
     const Index nwords = (n + 31)/32;
     if (desc->struconly() && mxv_mode == GrB_LOAD_BALANCE_MERGE) {
       DenseBitsCompactSource<T, true> src;
-      src.bits = dense_.d_bits_; src.u = dense_.d_val_;
+      src.bits = bits; src.u = dense_.d_val_;
       src.out_ind = sparse_.d_ind_; src.out_val = sparse_.d_val_;
       count = compactOrdered(src, nwords, desc);
     } else {
       DenseBitsCompactSource<T, false> src;
-      src.bits = dense_.d_bits_; src.u = dense_.d_val_;
+      src.bits = bits; src.u = dense_.d_val_;
       src.out_ind = sparse_.d_ind_; src.out_val = sparse_.d_val_;
       count = compactOrdered(src, nwords, desc);
     }
@@ -286,7 +284,7 @@ Info Vector<T>::dense2sparse(T identity, Descriptor* desc) {
     src.out_ind = sparse_.d_ind_; src.out_val = sparse_.d_val_;
     count = compactOrdered(src, nitems, desc);
   }
-  sparse_.nvals_ = count;
+  sparse_.computed(count);
 
   if (desc->debug()) {
     std::cout << "Dense frontier size: " << n << std::endl;
@@ -294,7 +292,6 @@ Info Vector<T>::dense2sparse(T identity, Descriptor* desc) {
   }
 
   vec_type_ = GrB_SPARSE;
-  sparse_.need_update_ = true;
   return GrB_SUCCESS;
 }
 
