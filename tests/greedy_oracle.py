@@ -1,8 +1,9 @@
 """ctypes binding of the CPU greedy graph colouring (tests/gc_oracle.c orc_gc) and the
 CPU greedy maximal independent set (tests/mis_oracle.c orc_mis), the checkers of the
 device colouring and MIS.  mis_oracle.c includes gc_oracle.c for its priority order,
-so one library built from it exports both.  Test infrastructure only: tests/, smoke()
-and tools/bench_gc.py / bench_mis.py import it.
+so one library built from it exports both.  priority_hash restates their priority
+order in numpy.  Test infrastructure only: tests/, smoke() and tools/bench_gc.py /
+bench_mis.py import it.
 
 build() compiles the library into build/libgreedyoracle.so; where that file is missing
 or older than either source, it is compiled into a temporary directory instead, so
@@ -19,8 +20,21 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SOURCE = os.path.join(ROOT, "tests", "mis_oracle.c")
 SOURCES = [SOURCE, os.path.join(ROOT, "tests", "gc_oracle.c")]
 LIB_PATH = os.path.join(ROOT, "build", "libgreedyoracle.so")
+M32 = 0xFFFFFFFF
 
 _lib = None
+
+
+def priority_hash(seed, v):
+    """fmix32(v ^ (seed * 0x9E3779B9)), the priority hash of
+    kernels/greedy_schedule.cuh, of one vertex or an array of vertices (uint64)."""
+    m32 = np.uint64(M32)
+    x = (np.asarray(v, np.uint64) ^ np.uint64((seed*0x9E3779B9) & M32)) & m32
+    x ^= x >> np.uint64(16)
+    x = (x*np.uint64(0x85EBCA6B)) & m32
+    x ^= x >> np.uint64(13)
+    x = (x*np.uint64(0xC2B2AE35)) & m32
+    return x ^ (x >> np.uint64(16))
 
 
 def compile_to(path):

@@ -8,48 +8,11 @@ import numpy as np
 import pytest
 
 import oracle_binding as orc
+from support import fused_stats, gb, make_matrix
 
 pytestmark = pytest.mark.gpu
 
 FUSED = dict(struconly=1, opreuse=1, earlyexit=1)
-
-
-@pytest.fixture(scope="module")
-def gb():
-    import graphblast_b200 as g
-    g.init(0)
-    return g
-
-
-def transpose(rp, ci):
-    n = len(rp) - 1
-    rows = np.repeat(np.arange(n, dtype=np.int32), np.diff(rp))
-    order = np.lexsort((rows, ci))
-    t_rp = np.concatenate([[0], np.cumsum(np.bincount(ci, minlength=n))]).astype(np.int32)
-    return t_rp, rows[order].astype(np.int32)
-
-
-def device_matrix(gb, rp, ci, directed=False):
-    import torch
-    from graphblast_b200 import graphs
-    n = len(rp) - 1
-    d_rp = torch.from_numpy(rp.astype(np.int32)).cuda()
-    d_ci = torch.from_numpy(ci.astype(np.int32)).cuda()
-    if not directed:
-        return graphs.matrix_from_csr(n, d_rp, d_ci)
-    t_rp, t_ci = transpose(rp, ci)
-    A = gb.Matrix(n, n)
-    ones = torch.ones(len(ci), dtype=torch.float32, device="cuda")
-    A.build_device_csr(d_rp, d_ci, ones, len(ci), torch.from_numpy(t_rp).cuda(),
-                       torch.from_numpy(t_ci).cuda(), ones.clone(), symmetric=False)
-    return A
-
-
-def fused_stats(desc, n):
-    from graphblast_b200 import _lib
-    st = (C.c_ulonglong * 6)()
-    _lib.load().gb200_bfs_stats(desc._h, n, st)
-    return [int(x) for x in st]
 
 
 @pytest.fixture(scope="module")
@@ -76,7 +39,7 @@ def test_two_traversals_queued_on_one_descriptor(gb, graphs, name, mode):
     from graphblast_b200 import algorithm
     rp, ci, directed = graphs[name]
     n = len(rp) - 1
-    A = device_matrix(gb, rp, ci, directed)
+    A = make_matrix(gb, rp, ci, symmetric=not directed)
     deg = np.diff(rp)
     s1, s2 = int(np.argmax(deg)), int(np.nonzero(deg)[0][-1])
     desc = gb.Descriptor(mxvmode=mode, **FUSED)
@@ -94,7 +57,7 @@ def test_timed_returns_the_device_time(gb, graphs, mode):
     rp, ci, _ = graphs["rmat12-cut"]
     n = len(rp) - 1
     assert n % 32 != 0
-    A = device_matrix(gb, rp, ci)
+    A = make_matrix(gb, rp, ci)
     s = int(np.argmax(np.diff(rp)))
     v = gb.Vector(n)
     ms = algorithm.bfs(v, A, s, gb.Descriptor(mxvmode=mode, **FUSED), timed=True)
@@ -112,7 +75,7 @@ def test_profiled_traversal_is_one_launch_and_counts_its_bytes(gb, graphs, mode)
     lib = _lib.load()
     rp, ci, directed = graphs["directed-rmat11"]
     n = len(rp) - 1
-    A = device_matrix(gb, rp, ci, directed)
+    A = make_matrix(gb, rp, ci, symmetric=not directed)
     s = int(np.argmax(np.diff(rp)))
     desc = gb.Descriptor(mxvmode=mode, **FUSED)
     v = gb.Vector(n)

@@ -2,62 +2,15 @@
 graph: state carried from one traversal to the next, directed graphs (the pushed
 CSR and the pulled CSC differ), and the overflow of the push level's heavy-vertex
 list.  Levels are compared bit-exactly with the oracle's BFS."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
 import oracle_binding as orc
+from support import bfs_levels, fused_stats, gb, make_matrix
 
 pytestmark = pytest.mark.gpu
 
 FUSED = dict(struconly=1, opreuse=1, earlyexit=1)
-
-
-@pytest.fixture(scope="module")
-def gb():
-    import graphblast_b200 as g
-    g.init(0)
-    return g
-
-
-def fused_stats(gb, desc, n):
-    """levels, entries inspected pulling, pull levels, vertices pushed, edges
-    pushed, vertices discovered pushing — of the last fused traversal."""
-    from graphblast_b200 import _lib
-    st = (C.c_ulonglong * 6)()
-    _lib.load().gb200_bfs_stats(desc._h, n, st)
-    return [int(x) for x in st]
-
-
-def device_matrix(gb, rp, ci, directed=False):
-    """Device CSR (+ CSC: the transpose for a directed graph) through graphs."""
-    import torch
-    from graphblast_b200 import graphs
-    n = len(rp) - 1
-    d_rp = torch.from_numpy(rp.astype(np.int32)).cuda()
-    d_ci = torch.from_numpy(ci.astype(np.int32)).cuda()
-    if not directed:
-        return graphs.matrix_from_csr(n, d_rp, d_ci)
-    rows = np.repeat(np.arange(n, dtype=np.int32), np.diff(rp))
-    order = np.lexsort((rows, ci))
-    t_rp = np.concatenate([[0], np.cumsum(np.bincount(ci, minlength=n))]).astype(np.int32)
-    t_ci = rows[order].astype(np.int32)
-    A = gb.Matrix(n, n)
-    ones = torch.ones(len(ci), dtype=torch.float32, device="cuda")
-    A.build_device_csr(d_rp, d_ci, ones, len(ci), torch.from_numpy(t_rp).cuda(),
-                       torch.from_numpy(t_ci).cuda(), ones.clone(), symmetric=False)
-    return A
-
-
-def expected(rp, ci, s, max_niter=None):
-    """The oracle's levels; with a cut-off after max_niter iterations only levels
-    1..max_niter are assigned (reference algorithm/bfs.hpp: the frontier found in
-    the last iteration is not), the rest are unreached."""
-    want = orc.bfs(rp, ci, s)
-    if max_niter is not None:
-        want = np.where(want <= max_niter, want, 0).astype(want.dtype)
-    return want
 
 
 def two_components(scale):
@@ -81,20 +34,20 @@ def test_vector_and_descriptor_reused_across_traversals(gb, mode):
         deg = np.diff(rp)
         hub_a = int(np.argmax(deg[:n // 2]))
         hub_b = n // 2 + int(np.argmax(deg[n // 2:]))
-        A = device_matrix(gb, rp, ci)
+        A = make_matrix(gb, rp, ci)
         v = gb.Vector(n)
         for s in (hub_a, hub_b, hub_a, int(np.argmin(deg))):
             algorithm.bfs(v, A, s, desc)
-            assert fused_stats(gb, desc, n)[0] > 0
+            assert fused_stats(desc, n)[0] > 0
             got = v.extractTuples().astype(np.int32)
-            assert np.array_equal(got, expected(rp, ci, s)), (mode, n, s)
+            assert np.array_equal(got, bfs_levels(rp, ci, s)), (mode, n, s)
         # a cut-off traversal after a full one from the same source, checked
         # against the operation-by-operation loop too
         for cut in (3, 2, 1):
             cdesc = gb.Descriptor(mxvmode=mode, max_niter=cut, **FUSED)
             algorithm.bfs(v, A, hub_b, cdesc)
             got = v.extractTuples().astype(np.int32)
-            assert np.array_equal(got, expected(rp, ci, hub_b, cut)), (mode, n, cut)
+            assert np.array_equal(got, bfs_levels(rp, ci, hub_b, cut)), (mode, n, cut)
             w = gb.Vector(n)
             algorithm.bfs(w, A, hub_b, gb.Descriptor(mxvmode=mode, max_niter=cut))
             assert np.array_equal(got, w.extractTuples().astype(np.int32)), (mode, n, cut)
@@ -108,15 +61,15 @@ def test_directed_graph(gb, mode):
     src, dst = orc.rmat_edges(scale, 8, seed=3)
     rp, ci = orc.build_csr(n, src, dst, False)
     assert not np.array_equal(rp, orc.build_csr(n, dst, src, False)[0])
-    A = device_matrix(gb, rp, ci, directed=True)
+    A = make_matrix(gb, rp, ci, symmetric=False)
     desc = gb.Descriptor(mxvmode=mode, **FUSED)
     deg = np.diff(rp)
     for s in (int(np.argmax(deg)), 0, int(np.argmin(deg))):
         v = gb.Vector(n)
         algorithm.bfs(v, A, s, desc)
         got = v.extractTuples().astype(np.int32)
-        assert np.array_equal(got, expected(rp, ci, s)), (mode, s)
-    stats = fused_stats(gb, desc, n)
+        assert np.array_equal(got, bfs_levels(rp, ci, s)), (mode, s)
+    stats = fused_stats(desc, n)
     assert stats[0] > 0
     if mode == 2:
         assert stats[2] == stats[0]
@@ -135,15 +88,15 @@ def test_heavy_list_overflow(gb, mode):
     dst = np.concatenate([hub_ids, np.tile(leaf_ids, hubs)])
     n = hubs + leaves + 8                       # a few isolated vertices at the end
     rp, ci = orc.build_csr(n, src, dst, True)
-    A = device_matrix(gb, rp, ci)
+    A = make_matrix(gb, rp, ci)
     desc = gb.Descriptor(mxvmode=mode, **FUSED)
     v = gb.Vector(n)
     for s in (0, int(leaf_ids[0])):
         algorithm.bfs(v, A, s, desc)
         got = v.extractTuples().astype(np.int32)
-        assert np.array_equal(got, expected(rp, ci, s)), (mode, s)
+        assert np.array_equal(got, bfs_levels(rp, ci, s)), (mode, s)
     if mode == 1:
         # from source 0: one vertex pushed at level 1, the hubs at level 2
         algorithm.bfs(v, A, 0, desc)
-        stats = fused_stats(gb, desc, n)
+        stats = fused_stats(desc, n)
         assert stats[3] >= 1 + hubs and stats[4] >= hubs * (leaves + 1)

@@ -9,19 +9,13 @@ import numpy as np
 import pytest
 
 import oracle_binding as orc
-from test_bfs_fused_gpu import FUSED, device_matrix, expected
+from support import bfs_levels, gb, make_matrix
 
 pytestmark = pytest.mark.gpu
 
+FUSED = dict(struconly=1, opreuse=1, earlyexit=1)
 PATH = 330                      # path vertices: a traversal from vertex 0 is deeper
 STAR = 2100                     # leaves of a star: more than GB_BFS_HEAVY (2048)
-
-
-@pytest.fixture(scope="module")
-def gb():
-    import graphblast_b200 as g
-    g.init(0)
-    return g
 
 
 def csr_edges(rp, ci):
@@ -58,9 +52,9 @@ def levels(v):
 def test_deeper_than_a_byte(gb, mode):
     from graphblast_b200 import algorithm
     rp, ci, _ = deep_graph()
-    want = expected(rp, ci, 0)
+    want = bfs_levels(rp, ci, 0)
     assert want.max() > 300 and want[-1] == PATH + 2        # a leaf of the star
-    A = device_matrix(gb, rp, ci)
+    A = make_matrix(gb, rp, ci)
     v = gb.Vector(len(rp) - 1)
     algorithm.bfs(v, A, 0, gb.Descriptor(mxvmode=mode, max_niter=1000, **FUSED))
     assert np.array_equal(levels(v), want)
@@ -71,10 +65,10 @@ def test_deeper_than_a_byte(gb, mode):
 def test_deep_traversal_cut_off(gb, mode, cut):
     from graphblast_b200 import algorithm
     rp, ci, _ = deep_graph()
-    A = device_matrix(gb, rp, ci)
+    A = make_matrix(gb, rp, ci)
     v = gb.Vector(len(rp) - 1)
     algorithm.bfs(v, A, 0, gb.Descriptor(mxvmode=mode, max_niter=cut, **FUSED))
-    assert np.array_equal(levels(v), expected(rp, ci, 0, cut)), (mode, cut)
+    assert np.array_equal(levels(v), bfs_levels(rp, ci, 0, cut)), (mode, cut)
 
 
 @pytest.mark.parametrize("mode", [0, 1, 2])
@@ -83,12 +77,12 @@ def test_deep_and_shallow_share_vector_and_descriptor(gb, mode):
     traversal may show through in the next."""
     from graphblast_b200 import algorithm
     rp, ci, shallow = deep_graph()
-    A = device_matrix(gb, rp, ci)
+    A = make_matrix(gb, rp, ci)
     v = gb.Vector(len(rp) - 1)
     desc = gb.Descriptor(mxvmode=mode, max_niter=1000, **FUSED)
     for s in (0, shallow, 0, shallow, PATH - 1, 0):
         algorithm.bfs(v, A, s, desc)
-        assert np.array_equal(levels(v), expected(rp, ci, s)), (mode, s)
+        assert np.array_equal(levels(v), bfs_levels(rp, ci, s)), (mode, s)
 
 
 def small_graph(n, seed):
@@ -110,13 +104,13 @@ def small_graph(n, seed):
 def test_sizes_not_a_multiple_of_16(gb, mode, n):
     from graphblast_b200 import algorithm
     rp, ci = small_graph(n, seed=n)
-    A = device_matrix(gb, rp, ci)
+    A = make_matrix(gb, rp, ci)
     desc = gb.Descriptor(mxvmode=mode, **FUSED)
     deg = np.diff(rp)
     v = gb.Vector(n)
     for s in sorted({int(np.argmax(deg)), n - 1, 0}):
         algorithm.bfs(v, A, s, desc)
-        assert np.array_equal(levels(v), expected(rp, ci, s)), (mode, n, s)
+        assert np.array_equal(levels(v), bfs_levels(rp, ci, s)), (mode, n, s)
 
 
 @pytest.mark.parametrize("mode", [0, 2])
@@ -127,12 +121,12 @@ def test_result_array_not_16_byte_aligned(gb, mode):
     from graphblast_b200 import algorithm
     rp, ci = orc.rmat_csr(12)
     n = len(rp) - 1
-    A = device_matrix(gb, rp, ci)
+    A = make_matrix(gb, rp, ci)
     buf = torch.full((n + 8,), -7.0, dtype=torch.float32, device="cuda")
     v = gb.Vector(n)
     v.build_device(buf[1:n + 1])
     s = int(np.argmax(np.diff(rp)))
     algorithm.bfs(v, A, s, gb.Descriptor(mxvmode=mode, **FUSED))
     got = buf.cpu().numpy()
-    assert np.array_equal(got[1:n + 1].astype(np.int32), expected(rp, ci, s))
+    assert np.array_equal(got[1:n + 1].astype(np.int32), bfs_levels(rp, ci, s))
     assert got[0] == -7.0 and np.all(got[n + 1:] == -7.0)

@@ -4,68 +4,16 @@ at entry 0, and the scan that takes a chunk's open rows 32 at a time.  Levels ar
 compared bit-exactly with the oracle's BFS in all three mxvmodes; in pull-only
 traversals the kernel's count of inspected entries must equal the CPU model of
 tools/bfs_pull_model.py."""
-import ctypes as C
-import importlib.util
-import os
-
 import numpy as np
 import pytest
 
 import oracle_binding as orc
+from support import bfs_pull_model, fused_stats, gb, make_matrix, symmetric_csr, transpose
 
 pytestmark = pytest.mark.gpu
 
 FUSED = dict(struconly=1, opreuse=1, earlyexit=1)
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _model():
-    spec = importlib.util.spec_from_file_location(
-        "bfs_pull_model", os.path.join(ROOT, "tools", "bfs_pull_model.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-model = _model()
-
-
-@pytest.fixture(scope="module")
-def gb():
-    import graphblast_b200 as g
-    g.init(0)
-    return g
-
-
-def fused_stats(desc, n):
-    from graphblast_b200 import _lib
-    st = (C.c_ulonglong * 6)()
-    _lib.load().gb200_bfs_stats(desc._h, n, st)
-    return [int(x) for x in st]
-
-
-def transpose(rp, ci):
-    n = len(rp) - 1
-    rows = np.repeat(np.arange(n, dtype=np.int32), np.diff(rp))
-    order = np.lexsort((rows, ci))
-    t_rp = np.concatenate([[0], np.cumsum(np.bincount(ci, minlength=n))]).astype(np.int32)
-    return t_rp, rows[order].astype(np.int32)
-
-
-def device_matrix(gb, rp, ci, directed=False):
-    import torch
-    from graphblast_b200 import graphs
-    n = len(rp) - 1
-    d_rp = torch.from_numpy(rp.astype(np.int32)).cuda()
-    d_ci = torch.from_numpy(ci.astype(np.int32)).cuda()
-    if not directed:
-        return graphs.matrix_from_csr(n, d_rp, d_ci)
-    t_rp, t_ci = transpose(rp, ci)
-    A = gb.Matrix(n, n)
-    ones = torch.ones(len(ci), dtype=torch.float32, device="cuda")
-    A.build_device_csr(d_rp, d_ci, ones, len(ci), torch.from_numpy(t_rp).cuda(),
-                       torch.from_numpy(t_ci).cuda(), ones.clone(), symmetric=False)
-    return A
+model = bfs_pull_model()
 
 
 def model_inspected(rp, ci, s, directed=False):
@@ -73,7 +21,7 @@ def model_inspected(rp, ci, s, directed=False):
     if not directed:
         _, insp = model.replay(rp.astype(np.int64), ci, s, mode=2)
         return insp["maxdeg"]
-    t_rp, t_ci = transpose(rp, ci)
+    t_rp, t_ci, _ = transpose(rp, ci)
     isolated = (np.diff(t_rp) == 0) & (np.diff(rp) == 0)
     _, insp = model.replay(t_rp.astype(np.int64), t_ci, s, mode=2, isolated=isolated)
     return insp["maxdeg"]
@@ -84,7 +32,7 @@ def check(gb, rp, ci, sources, directed=False, count=True):
     inspected entries against the model."""
     from graphblast_b200 import algorithm
     n = len(rp) - 1
-    A = device_matrix(gb, rp, ci, directed)
+    A = make_matrix(gb, rp, ci, symmetric=not directed)
     for mode in (0, 1, 2):
         desc = gb.Descriptor(mxvmode=mode, **FUSED)
         for s in sources:
@@ -99,15 +47,11 @@ def check(gb, rp, ci, sources, directed=False, count=True):
                 assert stats[1] == model_inspected(rp, ci, s, directed), s
 
 
-def symmetric(n, src, dst):
-    return orc.build_csr(n, np.asarray(src, np.int32), np.asarray(dst, np.int32), True)
-
-
 def test_summary_is_the_highest_degree_neighbour():
     """The CPU model's summary on a hand-checked graph: ties take the earliest
     entry, empty rows are -1."""
     # 0: {1, 2, 3}; 1: {0}; 2: {0, 4, 5}; 3: {0, 6, 7}; 4..7 leaves of 2 and 3; 8 alone
-    rp, ci = symmetric(9, [0, 0, 0, 2, 2, 3, 3], [1, 2, 3, 4, 5, 6, 7])
+    rp, ci = symmetric_csr(9, [0, 0, 0, 2, 2, 3, 3], [1, 2, 3, 4, 5, 6, 7])
     probe = model.probe_summary(rp.astype(np.int64), ci, "maxdeg")
     assert list(probe) == [2, 0, 0, 0, 2, 2, 3, 3, -1]
     assert list(model.probe_summary(rp.astype(np.int64), ci, "first")) == \
@@ -126,7 +70,7 @@ def test_highest_degree_neighbour_not_first(gb):
         src.append(r); dst.append(r - 10)
         src.append(r); dst.append(hubs[r % 10])
     n = 1500
-    rp, ci = symmetric(n, src, dst)
+    rp, ci = symmetric_csr(n, src, dst)
     check(gb, rp, ci, [100, 0, 15, 1005])
 
 
@@ -138,7 +82,7 @@ def test_degree_ties(gb):
     v = np.arange(n)
     src = np.concatenate([v, v])
     dst = np.concatenate([(v + 1) % n, (v + 7) % n])
-    rp, ci = symmetric(n, src, dst)
+    rp, ci = symmetric_csr(n, src, dst)
     check(gb, rp, ci, [0, int(rng.integers(n))])
 
 
@@ -146,7 +90,7 @@ def test_single_entry_rows(gb):
     """Stars and chains: most rows have one entry (bit 31 of the summary)."""
     src = [0] * 300 + list(range(300, 2000))
     dst = list(range(1, 301)) + list(range(301, 2001))
-    rp, ci = symmetric(2100, src, dst)
+    rp, ci = symmetric_csr(2100, src, dst)
     check(gb, rp, ci, [0, 5, 2000, 1200])
 
 
@@ -157,11 +101,11 @@ def test_only_visited_neighbour_is_entry_zero(gb):
     src = [1, 1] + [2] * 50 + [10] * 60
     dst = [0, 2] + list(range(100, 150)) + list(range(200, 260))
     n = 300
-    rp, ci = symmetric(n, src, dst)
+    rp, ci = symmetric_csr(n, src, dst)
     assert list(ci[rp[1]:rp[2]]) == [0, 2]
     assert model.probe_summary(rp.astype(np.int64), ci, "maxdeg")[1] == 2
     from graphblast_b200 import algorithm
-    A = device_matrix(gb, rp, ci)
+    A = make_matrix(gb, rp, ci)
     desc = gb.Descriptor(mxvmode=2, **FUSED)
     v = gb.Vector(n)
     algorithm.bfs(v, A, 0, desc)
@@ -185,7 +129,7 @@ def test_directed_in_and_out_degree_rank_differently(gb):
     src += [0, 0, 1]; dst += [a, 1, 200]            # 0 -> a, 0 -> 1 -> 200 -> b
     n = 400
     rp, ci = orc.build_csr(n, np.asarray(src, np.int32), np.asarray(dst, np.int32), False)
-    t_rp, t_ci = transpose(rp, ci)
+    t_rp, t_ci, _ = transpose(rp, ci)
     probe = model.probe_summary(t_rp.astype(np.int64), t_ci, "maxdeg")
     assert probe[100] == b
     check(gb, rp, ci, [0, a, 1, 250], directed=True)
@@ -228,7 +172,7 @@ def test_chunks_with_few_and_many_open_rows(gb):
     src = np.concatenate([live[1:], live[rng.integers(len(live), size=len(live))]])
     dst = np.concatenate([parent, live[rng.integers(len(live), size=len(live))]])
     keep = src != dst
-    rp, ci = symmetric(n, src[keep], dst[keep])
+    rp, ci = symmetric_csr(n, src[keep], dst[keep])
     assert (np.diff(rp)[:1024] == 0).all() and np.diff(rp)[n - 1] > 0
     deg = np.diff(rp)
     check(gb, rp, ci, [int(live[0]), int(np.argmax(deg)), n - 1, int(rows[1][0])])

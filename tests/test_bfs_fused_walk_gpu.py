@@ -7,29 +7,17 @@ the scan's, a long inline walk through the warp-wide loop and a partial last chu
 Levels are compared bit-exactly with the oracle's BFS in all three mxvmodes, and in
 modes 0 and 2 the kernel's count of inspected entries with the CPU model of
 tools/bfs_pull_model.py."""
-import ctypes as C
-import importlib.util
-import os
-
 import numpy as np
 import pytest
 
 import oracle_binding as orc
+from support import bfs_pull_model, fused_stats, gb, make_matrix, transpose
 
 FUSED = dict(struconly=1, opreuse=1, earlyexit=1, switchpoint=0.01)
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 WALK_INLINE = 64          # GB_BFS_WALK_INLINE
 
 
-def _model():
-    spec = importlib.util.spec_from_file_location(
-        "bfs_pull_model", os.path.join(ROOT, "tools", "bfs_pull_model.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-model = _model()
+model = bfs_pull_model()
 
 # The designed graphs share one skeleton.  S reaches the mid rows at the first level;
 # H has the highest degree (its leaves), so a row whose entries are a mid row and H
@@ -107,20 +95,12 @@ def model_levels(rp, ci, s, mode, directed=False):
         iters, insp = model.replay(rp.astype(np.int64), ci, s, mode=mode,
                                    switchpoint=np.float32(0.01), walk_inline=WALK_INLINE)
         return iters, insp["maxdeg"]
-    t_rp, t_ci = transpose(rp, ci)
+    t_rp, t_ci, _ = transpose(rp, ci)
     isolated = (np.diff(t_rp) == 0) & (np.diff(rp) == 0)
     iters, insp = model.replay(t_rp.astype(np.int64), t_ci, s, mode=mode,
                                switchpoint=np.float32(0.01), isolated=isolated,
                                walk_inline=WALK_INLINE)
     return iters, insp["maxdeg"]
-
-
-def transpose(rp, ci):
-    n = len(rp) - 1
-    rows = np.repeat(np.arange(n, dtype=np.int32), np.diff(rp))
-    order = np.lexsort((rows, ci))
-    t_rp = np.concatenate([[0], np.cumsum(np.bincount(ci, minlength=n))]).astype(np.int32)
-    return t_rp, rows[order].astype(np.int32)
 
 
 # ---- the designs do what they say (CPU) -----------------------------------------------
@@ -159,43 +139,13 @@ def test_designs_put_chunks_on_both_sides(mode):
 
 # ---- the kernel (GPU) ---------------------------------------------------------------
 
-@pytest.fixture(scope="module")
-def gb():
-    import graphblast_b200 as g
-    g.init(0)
-    return g
-
-
-def fused_stats(desc, n):
-    from graphblast_b200 import _lib
-    st = (C.c_ulonglong * 6)()
-    _lib.load().gb200_bfs_stats(desc._h, n, st)
-    return [int(x) for x in st]
-
-
-def device_matrix(gb, rp, ci, directed=False):
-    import torch
-    from graphblast_b200 import graphs
-    n = len(rp) - 1
-    d_rp = torch.from_numpy(rp.astype(np.int32)).cuda()
-    d_ci = torch.from_numpy(ci.astype(np.int32)).cuda()
-    if not directed:
-        return graphs.matrix_from_csr(n, d_rp, d_ci)
-    t_rp, t_ci = transpose(rp, ci)
-    A = gb.Matrix(n, n)
-    ones = torch.ones(len(ci), dtype=torch.float32, device="cuda")
-    A.build_device_csr(d_rp, d_ci, ones, len(ci), torch.from_numpy(t_rp).cuda(),
-                       torch.from_numpy(t_ci).cuda(), ones.clone(), symmetric=False)
-    return A
-
-
 def check(gb, rp, ci, sources, directed=False):
     """Levels in all three modes against the oracle, one descriptor per mode for
     all the sources (traversals back to back); in modes 0 and 2 the inspected
     entries against the model."""
     from graphblast_b200 import algorithm
     n = len(rp) - 1
-    A = device_matrix(gb, rp, ci, directed)
+    A = make_matrix(gb, rp, ci, symmetric=not directed)
     for mode in (0, 1, 2):
         desc = gb.Descriptor(mxvmode=mode, **FUSED)
         for s in sources:

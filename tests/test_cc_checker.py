@@ -1,4 +1,4 @@
-"""CPU tests of the connected-components checker (test_cc_gpu.components) and a
+"""CPU tests of the connected-components checker (support.components) and a
 compile-only check of backend::ccRun.
 
 The checker is pinned against a pure-Python union-find on small random directed
@@ -12,7 +12,7 @@ import subprocess
 import numpy as np
 import pytest
 
-from test_cc_gpu import check_structure, components
+from support import check_structure, components
 
 
 def py_components(n, edges):

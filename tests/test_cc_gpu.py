@@ -20,7 +20,8 @@ import numpy as np
 import pytest
 
 import oracle_binding as orc
-from test_parity_gpu import make_matrix
+from support import (check_structure, components, directed_csr, gb, make_matrix, mtx_graph,
+                     symmetric_csr)
 
 pytestmark = pytest.mark.gpu
 
@@ -30,45 +31,8 @@ GOLDEN = os.path.join(HERE, "golden")
 
 
 # ---------------------------------------------------------------------------
-# the checker
-# ---------------------------------------------------------------------------
-
-def components(n, rp, ci):
-    """(label, count): scipy's weakly connected components of the pattern (rp, ci),
-    each label mapped to its component's minimum vertex id."""
-    import scipy.sparse as sp
-    from scipy.sparse.csgraph import connected_components
-    if n == 0:
-        return np.zeros(0, np.int64), 0
-    A = sp.csr_matrix((np.ones(len(ci), np.int8), np.asarray(ci, np.int64),
-                       np.asarray(rp, np.int64)), shape=(n, n))
-    k, lab = connected_components(A, directed=True, connection="weak")
-    low = np.full(k, n, np.int64)
-    np.minimum.at(low, lab, np.arange(n, dtype=np.int64))
-    return low[lab], int(k)
-
-
-def check_structure(rp, ci, label):
-    """Without scipy: every stored entry joins equal labels, and each label is a
-    vertex no larger than i that labels itself."""
-    n = len(rp) - 1
-    label = np.asarray(label, np.int64)
-    rows = np.repeat(np.arange(n, dtype=np.int64), np.diff(rp))
-    assert np.array_equal(label[rows], label[np.asarray(ci, np.int64)]), "an edge spans two labels"
-    assert np.all((label >= 0) & (label <= np.arange(n))), "a label above its vertex"
-    assert np.array_equal(label[label], label), "a label that does not label itself"
-
-
-# ---------------------------------------------------------------------------
 # helpers
 # ---------------------------------------------------------------------------
-
-@pytest.fixture(scope="module")
-def gb():
-    import graphblast_b200 as g
-    g.init(0)
-    return g
-
 
 def run_cc(gb, A, n, v=None):
     from graphblast_b200 import algorithm
@@ -92,33 +56,6 @@ def check(gb, A, rp, ci):
     return got, k
 
 
-def csr_only(gb, rp, ci, dtype=None):
-    """A matrix adopted with its CSR alone, not marked symmetric: no CSC, no skip."""
-    import torch
-    dtype = gb.api.FP32 if dtype is None else dtype
-    n = len(rp) - 1
-    tdt = torch.float32 if dtype == gb.api.FP32 else torch.int32
-    A = gb.Matrix(n, n, dtype=dtype)
-    A.build_device_csr(torch.from_numpy(np.asarray(rp, np.int32)).cuda(),
-                       torch.from_numpy(np.asarray(ci, np.int32)).cuda(),
-                       torch.ones(len(ci), dtype=tdt, device="cuda"), len(ci),
-                       symmetric=False)
-    return A
-
-
-def symmetric_csr(n, src, dst):
-    return orc.build_csr(n, np.asarray(src, np.int32), np.asarray(dst, np.int32), True)
-
-
-def directed_csr(n, src, dst):
-    return orc.build_csr(n, np.asarray(src, np.int32), np.asarray(dst, np.int32), False)
-
-
-def mtx_graph(name):
-    n, src, dst, _ = orc.read_mtx_edges(os.path.join(GOLDEN, name + ".mtx"))
-    return orc.build_csr(n, src, dst, True)
-
-
 # ---------------------------------------------------------------------------
 # golden graphs and small cases
 # ---------------------------------------------------------------------------
@@ -133,7 +70,7 @@ def test_golden_graphs(gb, name):
         assert k == n and np.array_equal(got, np.arange(n))
         return
     check(gb, make_matrix(gb, rp, ci), rp, ci)
-    check(gb, csr_only(gb, rp, ci), rp, ci)
+    check(gb, make_matrix(gb, rp, ci, symmetric=False, csc=False), rp, ci)
 
 
 @pytest.mark.parametrize("directed", [0, 1, 2])
@@ -244,7 +181,7 @@ def test_long_path(gb, kind):
     got, k = check(gb, make_matrix(gb, rp, ci), rp, ci)
     assert k == 1 and not got.any()
     drp, dci = directed_csr(n, p[:-1], p[1:])
-    got, k = check(gb, csr_only(gb, drp, dci), drp, dci)
+    got, k = check(gb, make_matrix(gb, drp, dci, symmetric=False, csc=False), drp, dci)
     assert k == 1 and not got.any()
 
 
@@ -259,10 +196,10 @@ def test_star_with_the_hub_last(gb):
     got, k = check(gb, make_matrix(gb, rp, ci), rp, ci)
     assert k == 1 and not got.any()
     drp, dci = directed_csr(n, leaf, hub)              # one way, leaf -> hub
-    got, k = check(gb, csr_only(gb, drp, dci), drp, dci)
+    got, k = check(gb, make_matrix(gb, drp, dci, symmetric=False, csc=False), drp, dci)
     assert k == 1 and not got.any()
     drp, dci = directed_csr(n, hub, leaf)              # one way, hub -> leaf: one warp list
-    check(gb, csr_only(gb, drp, dci), drp, dci)
+    check(gb, make_matrix(gb, drp, dci, symmetric=False, csc=False), drp, dci)
 
 
 def test_disjoint_edges_and_triangles(gb):
@@ -279,7 +216,7 @@ def test_disjoint_edges_and_triangles(gb):
     _, k = check(gb, make_matrix(gb, rp, ci), rp, ci)
     assert k == ne + nt
     drp, dci = directed_csr(n, src, dst)
-    check(gb, csr_only(gb, drp, dci), drp, dci)
+    check(gb, make_matrix(gb, drp, dci, symmetric=False, csc=False), drp, dci)
 
 
 def random_component(rng, ids, extra):
@@ -325,7 +262,8 @@ def test_rmat(gb, scale):
     assert np.diff(rp).max() > 5000 and np.count_nonzero(np.diff(rp) == 0) > 0
     got, k = check(gb, make_matrix(gb, rp, ci), rp, ci)
     assert k > 1 and np.count_nonzero(got == 0) > n//2
-    got2, k2 = check(gb, csr_only(gb, rp, ci), rp, ci)         # the same graph, no skip
+    got2, k2 = check(gb, make_matrix(gb, rp, ci, symmetric=False, csc=False),
+                     rp, ci)                                    # the same graph, no skip
     assert np.array_equal(got, got2) and k == k2
 
 
@@ -357,7 +295,8 @@ def test_non_symmetric_matrix_never_skips(gb):
         first += m
     assert drp[N + 1] - drp[N] == 0
     want = np.concatenate([np.zeros(first, np.int64), np.arange(first, n)])
-    for A in (make_matrix(gb, drp, dci, symmetric=False), csr_only(gb, drp, dci)):
+    for A in (make_matrix(gb, drp, dci, symmetric=False),
+              make_matrix(gb, drp, dci, symmetric=False, csc=False)):
         got, k = check(gb, A, drp, dci)
         assert np.array_equal(got, want) and k == 6
     # the same pattern made symmetric may skip, and gives the same components
@@ -371,7 +310,8 @@ def test_directed_one_way_matrix(gb):
     n = 5000
     src = np.arange(n - 1, dtype=np.int32)
     drp, dci = directed_csr(n, src, src + 1)
-    for A in (make_matrix(gb, drp, dci, symmetric=False), csr_only(gb, drp, dci)):
+    for A in (make_matrix(gb, drp, dci, symmetric=False),
+              make_matrix(gb, drp, dci, symmetric=False, csc=False)):
         got, k = check(gb, A, drp, dci)
         assert k == 1 and not got.any()
     # 50..99 join the path 100..4999 only through 100 -> 50, an entry of row 100 alone
@@ -380,18 +320,18 @@ def test_directed_one_way_matrix(gb):
     src2 = np.concatenate([src2, np.arange(50, 99)]).astype(np.int32)
     dst2 = np.concatenate([dst2, np.arange(51, 100)]).astype(np.int32)
     drp, dci = directed_csr(n, src2, dst2)
-    got, k = check(gb, csr_only(gb, drp, dci), drp, dci)
+    got, k = check(gb, make_matrix(gb, drp, dci, symmetric=False, csc=False), drp, dci)
     assert k == 51 and np.all(got[50:] == 50)
 
 
 def test_int32_matrix_and_stored_zeros(gb):
     rp, ci = orc.rmat_csr(12)
-    check(gb, make_matrix(gb, rp, ci, dtype=gb.api.INT32), rp, ci)
-    check(gb, csr_only(gb, rp, ci, dtype=gb.api.INT32), rp, ci)
+    check(gb, make_matrix(gb, rp, ci, integer=True), rp, ci)
+    check(gb, make_matrix(gb, rp, ci, symmetric=False, csc=False, integer=True), rp, ci)
     zeros = np.zeros(len(ci), np.float32)
-    got, _ = check(gb, make_matrix(gb, rp, ci, zeros), rp, ci)
+    got, _ = check(gb, make_matrix(gb, rp, ci, zeros, symmetric=False), rp, ci)
     got_i, _ = check(gb, make_matrix(gb, rp, ci, zeros.astype(np.int32),
-                                     dtype=gb.api.INT32), rp, ci)
+                                     symmetric=False, integer=True), rp, ci)
     assert np.array_equal(got, got_i)
 
 

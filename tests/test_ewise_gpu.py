@@ -32,6 +32,7 @@ if __name__ == "__main__":
 
 import ewise_reference as ref  # noqa: E402
 import mxm_reference as mref  # noqa: E402
+from support import device_matrix, gb, make_matrix, ragged_graph, same  # noqa: E402
 
 COMPACT_NT = 256
 VALUE_CTA = COMPACT_NT*8
@@ -73,11 +74,6 @@ def values(rng, regime, n):
     return x
 
 
-def same(x, y):
-    x, y = np.asarray(x, np.float32), np.asarray(y, np.float32)
-    return x.shape == y.shape and bool(np.all((x == y) | (np.isnan(x) & np.isnan(y))))
-
-
 def pattern(rng, n, kind):
     """Sorted indices: empty, one entry, all, the last partial word, random."""
     if kind == "empty":
@@ -89,13 +85,6 @@ def pattern(rng, n, kind):
     if kind == "tail":
         return np.arange(n - (n % 32 or 32), n, dtype=np.int32)[::2].copy()
     return np.sort(rng.choice(n, max(1, n//3), replace=False)).astype(np.int32)
-
-
-@pytest.fixture(scope="module")
-def gb():
-    import graphblast_b200 as g
-    g.init(0)
-    return g
 
 
 def dense(gb, x):
@@ -344,8 +333,8 @@ def test_matrix_scale_and_broadcast_through_pr_normalize(gb):
     rng = np.random.RandomState(3)
     S = mx.structure(rng, ROW_LENGTHS, 6000)
     vals = rng.randint(1, 9, S.nnz).astype(np.float32)
-    S = mx.with_values(S, vals)
-    M = mx.device_matrix(gb, S)
+    S = S.with_values(vals)
+    M = device_matrix(gb, S)
     alpha = np.float32(0.85)
     M.pr_normalize(float(alpha), gb.Descriptor())
     outdeg, _ = ref.reduce_rows(0, S.ptr, S.val)
@@ -420,13 +409,13 @@ def test_reduce_matrix_to_scalar(gb):
     import test_mxv_gpu as mx
     rng = np.random.RandomState(11)
     S = mx.structure(rng, ROW_LENGTHS*20, 6000)
-    M = mx.device_matrix(gb, S)
+    M = device_matrix(gb, S)
     desc = gb.Descriptor()
     for m in (0, 2, 3, 4, 5):
         want, _ = ref.reduce(m, S.val)
         assert reduce_val(gb, m, M, desc) == want, m
-    F = mx.with_values(S, values(rng, "float", S.nnz))
-    MF = mx.device_matrix(gb, F)
+    F = S.with_values(values(rng, "float", S.nnz))
+    MF = device_matrix(gb, F)
     want, bound = ref.reduce(0, F.val)
     assert abs(float(reduce_val(gb, 0, MF, desc)) - want) <= bound
     assert reduce_val(gb, 0, MF, gb.Descriptor(struconly=1)) == S.nnz
@@ -443,7 +432,7 @@ def test_reduce_rows(gb, regime):
     import test_mxv_gpu as mx
     rng = np.random.RandomState(12)
     S = mx.structure(rng, ROW_LENGTHS, 6000)
-    M = mx.device_matrix(gb, S)
+    M = device_matrix(gb, S)
     desc = gb.Descriptor()
     monoids = [0] if regime == "float" else [0, 1, 2, 3, 4, 5]
     for m in monoids:
@@ -452,7 +441,7 @@ def test_reduce_rows(gb, regime):
         else:
             val = np.concatenate([monoid_values(rng, m, S.ptr[i + 1] - S.ptr[i])
                                   for i in range(S.nrows)]).astype(np.float32)
-        M = mx.device_matrix(gb, mx.with_values(S, val))
+        M = device_matrix(gb, S.with_values(val))
         w = gb.Vector(S.nrows)
         gb.reduce(None, m, M, desc, out=w)
         want, bound = ref.reduce_rows(m, S.ptr, val)
@@ -574,7 +563,7 @@ def test_assign_dense_target_every_mask(gb, scmp):
             check_shadow(gb, w)
             # mask from a fused Boolean pull (lazily held 0/1 values)
             S = mx.square(rng, n)
-            M = mx.device_matrix(gb, S)
+            M = device_matrix(gb, S)
             u = rng.choice(np.float32([0, 1]), n)
             pm = rng.choice(np.float32([0, 1]), n)
             f = mx.bool_pull(gb, M, "mxv", 0, u, mx.dense_vector(gb, pm), False, False, False)
@@ -647,7 +636,7 @@ def test_count_of_a_zero_one_vector_follows_every_change(gb):
     n = BITS_CTA + 1
     rng = np.random.RandomState(9)
     S = mx.square(rng, n)
-    M = mx.device_matrix(gb, S)
+    M = device_matrix(gb, S)
     desc = gb.Descriptor()
 
     def fresh():
@@ -738,7 +727,7 @@ def test_row_reduce_into_a_shorter_w_is_refused(gb):
     import test_mxv_gpu as mx
     rng = np.random.RandomState(2)
     S = mx.structure(rng, ROW_LENGTHS*4, 6000)
-    M = mx.device_matrix(gb, S)
+    M = device_matrix(gb, S)
     nw = S.nrows - 17
     w, t = adopted(gb, nw, S.nrows, 9.0)
     code = info_of(gb, lambda: gb.reduce(None, 0, M, gb.Descriptor(), out=w))
@@ -834,7 +823,6 @@ def _child(out, eps):
     import graphblast_b200 as g
     from graphblast_b200 import algorithm
     import oracle_binding as orc
-    from test_parity_gpu import make_matrix, ragged_graph
     g.init(0)
     res = {}
     rp, ci = ragged_graph()

@@ -16,7 +16,7 @@ import numpy as np
 import pytest
 
 import ewise_matrix_reference as ref
-from test_mxm_unmasked_gpu import Csr, csr, random_csr, device_matrix, check
+from support import Csr, check_csr, csr, device_matrix, gb, random_csr
 
 TILE = 2048            # GB_EWM_TILE
 IPT = 16               # GB_EWM_IPT
@@ -25,13 +25,6 @@ VALUES = np.array([-4, -2, -1, -0.5, 0, 0.5, 1, 2, 4, np.inf], np.float32)
 KINDS = ["disjoint", "identical", "nested", "partial"]
 HEADER = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "graphblast_b200",
                       "csrc", "graphblas", "backend", "cuda", "kernels", "ewise_matrix.cuh")
-
-
-@pytest.fixture(scope="module")
-def gb():
-    import graphblast_b200 as g
-    g.init(0)
-    return g
 
 
 def reference(add, semiring, A, B, integer=False):
@@ -45,15 +38,17 @@ def op(gb, add):
 
 
 def run(gb, add, semiring, A, B, desc=None, integer=False):
-    dA = device_matrix(gb, A, integer)
-    dB = dA if B is A else device_matrix(gb, B, integer)
+    dA = device_matrix(gb, A, integer=integer)
+    dB = dA if B is A else device_matrix(gb, B, integer=integer)
     C = gb.Matrix(A.nrows, A.ncols, dtype=gb.api.INT32 if integer else gb.api.FP32)
     op(gb, add)(C, None, None, semiring, dA, dB, gb.Descriptor() if desc is None else desc)
     return C
 
 
 def csr_only(gb, S):
-    """A Matrix holding device copies of S's CSR only (no CSC)."""
+    """A Matrix holding device copies of S's CSR only (no CSC).  Unlike
+    device_matrix(csc=False) it never calls the CSC adoption, which even without
+    arrays marks the CSC side initialised."""
     import torch
     dev = lambda a, dt=np.int32: torch.from_numpy(np.ascontiguousarray(a, dt)).cuda()
     M = gb.Matrix(S.nrows, S.ncols)
@@ -75,12 +70,13 @@ def overlap(seed, kind, semiring, m=120, n=170):
         return A, random_csr(rng, m, n, 0.08, vals)
     if kind == "nested":
         keep = rng.rand(A.nnz) < 0.5
-        return A, csr(m, n, A.rows()[keep], A.ind[keep], rng.choice(vals, keep.sum()))
+        return A, csr(m, n, A.rows()[keep], A.ind[keep], rng.choice(vals, keep.sum()),
+                      np.float32)
     B = random_csr(rng, m, n, 0.08, vals)
     taken = set(zip(A.rows().tolist(), A.ind.tolist()))
     keep = np.array([(r, c) not in taken for r, c in zip(B.rows().tolist(), B.ind.tolist())],
                     bool)
-    return A, csr(m, n, B.rows()[keep], B.ind[keep], B.val[keep])
+    return A, csr(m, n, B.rows()[keep], B.ind[keep], B.val[keep], np.float32)
 
 
 # ---------------------------------------------------------------------------
@@ -104,8 +100,9 @@ def straddling(lead):
     cols = np.sort(rng.choice(n, 5*TILE // 2, replace=False))
     ar = np.concatenate([np.zeros(lead, int), np.ones(len(cols), int)])
     ac = np.concatenate([np.arange(lead), cols])
-    A = csr(3, n, ar, ac, rng.choice(VALUES[:-1], len(ac)))
-    B = csr(3, n, np.ones(len(cols), int), cols, rng.choice(VALUES[:-1], len(cols)))
+    A = csr(3, n, ar, ac, rng.choice(VALUES[:-1], len(ac)), np.float32)
+    B = csr(3, n, np.ones(len(cols), int), cols, rng.choice(VALUES[:-1], len(cols)),
+            np.float32)
     return A, B
 
 
@@ -131,7 +128,7 @@ def test_straddling_pairs_cross_every_boundary(lead):
 def test_every_semiring_and_overlap(gb, semiring, add, kind):
     A, B = overlap(semiring*7 + KINDS.index(kind), kind, semiring)
     assert (np.diff(A.ptr) == 0).any() and (A.val == 0).any()
-    check(run(gb, add, semiring, A, B), reference(add, semiring, A, B))
+    check_csr(run(gb, add, semiring, A, B), reference(add, semiring, A, B))
 
 
 @pytest.mark.gpu
@@ -147,10 +144,10 @@ def test_hub_row_over_many_tiles(gb, add, semiring):
     ac = np.concatenate([[5], hub_a, [n - 1]])
     br = np.concatenate([[1], np.full(len(hub_b), 2), [4], [6]])
     bc = np.concatenate([[7], hub_b, [n - 1], [0]])
-    A = csr(8, n, ar, ac, rng.choice(VALUES[:-1], len(ac)))
-    B = csr(8, n, br, bc, rng.choice(VALUES[:-1], len(bc)))
+    A = csr(8, n, ar, ac, rng.choice(VALUES[:-1], len(ac)), np.float32)
+    B = csr(8, n, br, bc, rng.choice(VALUES[:-1], len(bc)), np.float32)
     assert A.nnz + B.nnz > 1000000
-    check(run(gb, add, semiring, A, B), reference(add, semiring, A, B))
+    check_csr(run(gb, add, semiring, A, B), reference(add, semiring, A, B))
 
 
 @pytest.mark.gpu
@@ -158,8 +155,8 @@ def test_hub_row_over_many_tiles(gb, add, semiring):
 @pytest.mark.parametrize("add", [True, False])
 def test_straddling_pairs(gb, lead, add):
     A, B = straddling(lead)
-    check(run(gb, add, 1, A, B), reference(add, 1, A, B))
-    check(run(gb, add, 1, B, A), reference(add, 1, B, A))
+    check_csr(run(gb, add, 1, A, B), reference(add, 1, A, B))
+    check_csr(run(gb, add, 1, B, A), reference(add, 1, B, A))
 
 
 @pytest.mark.gpu
@@ -170,12 +167,12 @@ def test_edge_shapes(gb, shape, add):
     m, n = {"one_row": (1, 5000), "one_col": (5000, 1)}.get(shape, (40, 60))
     A = random_csr(rng, m, n, 0.3, VALUES)
     B = random_csr(rng, m, n, 0.3, VALUES)
-    empty = csr(m, n, [], [], np.zeros(0, np.float32))
+    empty = csr(m, n, [], [], np.zeros(0, np.float32), np.float32)
     if shape in ("nnzA0", "both0"):
         A = empty
     if shape in ("nnzB0", "both0"):
         B = empty
-    check(run(gb, add, 1, A, B), reference(add, 1, A, B))
+    check_csr(run(gb, add, 1, A, B), reference(add, 1, A, B))
 
 
 @pytest.mark.gpu
@@ -199,17 +196,17 @@ def test_transposed_operands(gb, tran, add):
     want = reference(add, 2, A, B)
     C = gb.Matrix(70, 110)
     op(gb, add)(C, None, None, 2, device_matrix(gb, sA), device_matrix(gb, sB), desc)
-    check(C, want)
+    check_csr(C, want)
     plain_A = csr_only(gb, sA) if tran != "inp1" else device_matrix(gb, sA)
     plain_B = csr_only(gb, sB) if tran != "inp0" else device_matrix(gb, sB)
     with pytest.raises(gb.api.GraphBLASError) as err:
         op(gb, add)(C, None, None, 2, plain_A, plain_B, desc)
     assert err.value.info == gb.api.Info.GrB_UNINITIALIZED_OBJECT
-    check(C, want)
+    check_csr(C, want)
     with pytest.raises(gb.api.GraphBLASError) as err:
         op(gb, add)(C, None, None, 2, device_matrix(gb, A), device_matrix(gb, B), desc)
     assert err.value.info == gb.api.Info.GrB_DIMENSION_MISMATCH
-    check(C, want)
+    check_csr(C, want)
 
 
 def _dense(S):
@@ -223,7 +220,7 @@ def check_csc(gb, C, want):
     pull vxm over C (which reads the CSC)."""
     T = gb.Matrix(want.ncols, want.nrows)
     gb.transpose(T, None, None, C, gb.Descriptor())
-    check(T, want.T)
+    check_csr(T, want.T)
     u = np.array([1, 2, -1, 0.5], np.float32)[np.arange(want.nrows) % 4]
     uv = gb.Vector(want.nrows)
     uv.build(u)
@@ -252,7 +249,7 @@ def test_aliasing(gb, alias, add):
     else:
         op(gb, add)(dA, None, None, 1, dA, dA, gb.Descriptor())
         C, want = dA, reference(add, 1, A, A)
-    check(C, want)
+    check_csr(C, want)
     check_csc(gb, C, want)
 
 
@@ -263,7 +260,7 @@ def test_int_plus_times(gb, add):
     ivals = np.array([-3, -2, -1, 0, 1, 2, 3, 5, 7], np.int32)
     A = random_csr(rng, 110, 90, 0.1, ivals)
     B = random_csr(rng, 110, 90, 0.1, ivals)
-    check(run(gb, add, 1, A, B, integer=True), reference(add, 1, A, B, integer=True))
+    check_csr(run(gb, add, 1, A, B, integer=True), reference(add, 1, A, B, integer=True))
 
 
 @pytest.mark.gpu
@@ -282,7 +279,7 @@ def test_refusals_leave_c_unchanged(gb, add):
         with pytest.raises(Err) as err:
             f(*args)
         assert err.value.info == code
-        check(C, want)
+        check_csr(C, want)
         assert C.getStorage() == gb.Storage.GrB_SPARSE
 
     refused(Info.GrB_NOT_IMPLEMENTED, C, dA, None, 1, dA, dB, gb.Descriptor())  # mask
@@ -296,8 +293,8 @@ def test_refusals_leave_c_unchanged(gb, add):
             gb.Descriptor())
     # INT32 operands: another semiring, then mixed element types
     ivals = np.array([-2, 1, 3], np.int32)
-    iA = device_matrix(gb, random_csr(rng, 50, 40, 0.1, ivals), True)
-    iB = device_matrix(gb, random_csr(rng, 50, 40, 0.1, ivals), True)
+    iA = device_matrix(gb, random_csr(rng, 50, 40, 0.1, ivals), integer=True)
+    iB = device_matrix(gb, random_csr(rng, 50, 40, 0.1, ivals), integer=True)
     iC = gb.Matrix(50, 40, dtype=gb.api.INT32)
     with pytest.raises(Err) as err:
         f(iC, None, None, 2, iA, iB, gb.Descriptor())
@@ -313,7 +310,7 @@ def test_refusals_leave_c_unchanged(gb, add):
     assert np.all(Cd.extract_dense() == 3)
     f(Cd, None, None, 1, dA, dB, gb.Descriptor())
     assert Cd.getStorage() == gb.Storage.GrB_SPARSE
-    check(Cd, want)
+    check_csr(Cd, want)
 
 
 @pytest.mark.gpu
@@ -337,7 +334,7 @@ def test_deterministic_with_fixed_launches(gb, add):
         out.append([x.tobytes() for x in C.extract_csr()])
     assert out[0] == out[1] == out[2]
     assert launches[1] == launches[2]
-    check(C, reference(add, 4, A, B))
+    check_csr(C, reference(add, 4, A, B))
 
 
 @pytest.mark.gpu
@@ -351,15 +348,11 @@ def test_transpose(gb, case):
         D = _dense(A)
         D = np.triu(D) + np.triu(D, 1).T
         r, c = np.nonzero(D != 0)
-        A = csr(m, n, r, c, D[r, c].astype(np.float32))
+        A = csr(m, n, r, c, D[r, c].astype(np.float32), np.float32)
     if case == "rect_csr_only":
         dA = csr_only(gb, A)
     elif case == "symmetric":
-        import torch
-        dev = lambda a, dt=np.int32: torch.from_numpy(np.ascontiguousarray(a, dt)).cuda()
-        dA = gb.Matrix(m, n)
-        dA.build_device_csr(dev(A.ptr), dev(A.ind), dev(A.val, np.float32), A.nnz,
-                            symmetric=True)
+        dA = device_matrix(gb, A, symmetric=True)
     else:
         dA = device_matrix(gb, A)
     desc = gb.Descriptor()
@@ -371,12 +364,12 @@ def test_transpose(gb, case):
     else:
         C, want = gb.Matrix(n, m), A.T
     gb.transpose(C, None, None, dA, desc)
-    check(C, want)
+    check_csr(C, want)
     check_csc(gb, C, want)
     with pytest.raises(gb.api.GraphBLASError) as err:
         gb.transpose(C, C, None, dA, desc)                # C as a mask of its shape
     assert err.value.info == gb.api.Info.GrB_NOT_IMPLEMENTED
-    check(C, want)
+    check_csr(C, want)
     if m != n:
         with pytest.raises(gb.api.GraphBLASError) as err:
             gb.transpose(gb.Matrix(m + 1, n + 1), None, None, dA, desc)
@@ -389,11 +382,11 @@ def test_size_limit(gb):
     has 2^31 > INT32_MAX entries.  GrB_OUT_OF_MEMORY, and C keeps its result."""
     import torch
     m, n = 1 << 15, 1 << 16
-    X = csr(m, n, [0, 5, m - 1], [0, 3, n - 1], np.float32([2, -1, 4]))
-    Y = csr(m, n, [0, 7], [0, 9], np.float32([0.5, 1]))
+    X = csr(m, n, [0, 5, m - 1], [0, 3, n - 1], np.float32([2, -1, 4]), np.float32)
+    Y = csr(m, n, [0, 7], [0, 9], np.float32([0.5, 1]), np.float32)
     want = reference(True, 1, X, Y)
     C = run(gb, True, 1, X, Y)
-    check(C, want)
+    check_csr(C, want)
     rowptr = torch.arange(0, m + 1, dtype=torch.int32, device="cuda")*(n // 2)
     even = torch.arange(0, n, 2, dtype=torch.int32, device="cuda").repeat(m)
     ones = torch.ones(m*(n // 2), dtype=torch.float32, device="cuda")
@@ -411,7 +404,7 @@ def test_size_limit(gb):
     with pytest.raises(gb.api.GraphBLASError) as err:
         gb.eWiseAdd(C, None, None, 1, dA, dB, gb.Descriptor())
     assert err.value.info == gb.api.Info.GrB_OUT_OF_MEMORY
-    check(C, want)
+    check_csr(C, want)
     # the intersection of the two is empty
     E = gb.Matrix(m, n)
     gb.eWiseMult(E, None, None, 1, dA, dB, gb.Descriptor())

@@ -6,6 +6,7 @@ import pytest
 
 import ewise_matrix_reference as ref
 from mxm_reference import OPS, SEMIRINGS
+from support import same
 
 VALUES = np.array([-4, -2, -1, -0.5, 0, 0.5, 1, 2, 4], np.float32)
 
@@ -38,10 +39,6 @@ def dok(add, semiring, A, B):
             else:
                 out[k] = da[k] if k in da else db[k]
     return out
-
-
-def same(x, y):
-    return x == y or (np.isnan(x) and np.isnan(y))
 
 
 @pytest.mark.parametrize("add", [True, False])

@@ -11,6 +11,7 @@ import pytest
 import ewise_reference as ref
 import mxm_reference as mref
 import oracle_binding as orc
+from support import same
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CUDA = os.path.join(ROOT, "graphblast_b200", "csrc", "graphblas", "backend", "cuda")
@@ -35,11 +36,6 @@ def _identity_value(expr):
     return {"0": 0.0, "1": 1.0, "false": 0.0,
             "std::numeric_limits<T_out>::max()": float(mref.FLT_MAX),
             "std::numeric_limits<T_out>::min()": float(mref.FLT_MIN)}[expr]
-
-
-def same(x, y):
-    x, y = np.asarray(x, np.float32), np.asarray(y, np.float32)
-    return x.shape == y.shape and bool(np.all((x == y) | (np.isnan(x) & np.isnan(y))))
 
 
 def test_monoid_identities_are_the_ones_stddef_defines():

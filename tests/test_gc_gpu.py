@@ -7,26 +7,15 @@ the kernel's classes: lists a lane takes alone and lists a warp takes, the sweep
 the tail, several 64-colour windows, empty and isolated rows, self-loops, and a
 directed matrix read through its CSR and its CSC.
 """
-import os
-
 import numpy as np
 import pytest
 
 import greedy_oracle
 import oracle_binding as orc
-from test_parity_gpu import make_matrix, path_graph, ragged_graph, star_graph
+from support import (gb, make_matrix, mtx_graph, path_graph, ragged_graph, star_graph,
+                     symmetric_csr)
 
 pytestmark = pytest.mark.gpu
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-GOLDEN = os.path.join(HERE, "golden")
-
-
-@pytest.fixture(scope="module")
-def gb():
-    import graphblast_b200 as g
-    g.init(0)
-    return g
 
 
 def colour(gb, A, n, seed=0):
@@ -37,24 +26,15 @@ def colour(gb, A, n, seed=0):
     return v.extractTuples(), ncolors
 
 
-def check(gb, rp, ci, seeds=(0,), dtype=None):
+def check(gb, rp, ci, seeds=(0,), integer=False):
     n = len(rp) - 1
-    A = make_matrix(gb, rp, ci, dtype=dtype)
+    A = make_matrix(gb, rp, ci, integer=integer)
     for seed in seeds:
         got, ncolors = colour(gb, A, n, seed)
         want, want_n, _ = greedy_oracle.gc(rp, ci, seed)
         assert np.array_equal(got, want.astype(np.float32)), seed
         assert ncolors == want_n, seed
     return A
-
-
-def mtx_graph(name):
-    n, src, dst, _ = orc.read_mtx_edges(os.path.join(GOLDEN, name + ".mtx"))
-    return orc.build_csr(n, src, dst, True)
-
-
-def symmetric_csr(n, src, dst):
-    return orc.build_csr(n, np.asarray(src, np.int32), np.asarray(dst, np.int32), True)
 
 
 @pytest.mark.parametrize("name", ["chesapeake", "test_cc", "test_bc", "test_sgm"])
@@ -170,7 +150,7 @@ def test_rmat(gb, scale):
 
 def test_int32_matrix(gb):
     rp, ci = orc.rmat_csr(12)
-    check(gb, rp, ci, seeds=(0, 6), dtype=gb.api.INT32)
+    check(gb, rp, ci, seeds=(0, 6), integer=True)
 
 
 def test_same_call_twice_is_identical_and_seeds_differ(gb):

@@ -17,37 +17,23 @@ import pytest
 
 import greedy_oracle
 import oracle_binding as orc
+from greedy_oracle import M32, priority_hash
+from support import graphs
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLDEN = os.path.join(ROOT, "tests", "golden")
-M32 = 0xFFFFFFFF
-
-
-def py_hash(seed, v):
-    """fmix32(v ^ (seed * 0x9E3779B9)), the priority hash of kernels/greedy_schedule.cuh."""
-    x = (v ^ (seed*0x9E3779B9)) & M32
-    x ^= x >> 16
-    x = (x*0x85EBCA6B) & M32
-    x ^= x >> 13
-    x = (x*0xC2B2AE35) & M32
-    return x ^ (x >> 16)
 
 
 def py_gc(n, rowptr, colind, seed):
     """Sequential greedy first-fit in decreasing (hash, v) order."""
     colors = [0]*n
-    for v in sorted(range(n), key=lambda v: (py_hash(seed & M32, v), v), reverse=True):
+    key = lambda v: (priority_hash(seed & M32, v), v)
+    for v in sorted(range(n), key=key, reverse=True):
         used = {colors[u] for u in colind[rowptr[v]:rowptr[v + 1]] if u != v}
         c = 1
         while c in used:
             c += 1
         colors[v] = c
     return colors
-
-
-def mtx_graph(name):
-    n, src, dst, _ = orc.read_mtx_edges(os.path.join(GOLDEN, name + ".mtx"))
-    return orc.build_csr(n, src, dst, True)
 
 
 def check_greedy(rowptr, colind, colors, seed):
@@ -62,7 +48,7 @@ def check_greedy(rowptr, colind, colors, seed):
     rows = np.repeat(np.arange(n), deg)
     off_diag = rows != colind
     assert not np.any(colors[rows[off_diag]] == colors[colind[off_diag]]), "not proper"
-    prio = np.array([py_hash(seed & M32, v) for v in range(n)], dtype=np.uint64)
+    prio = priority_hash(seed & M32, np.arange(n))
     key = (prio << np.uint64(32)) | np.arange(n, dtype=np.uint64)
     for v in range(n):
         nb = colind[rowptr[v]:rowptr[v + 1]]
@@ -71,14 +57,6 @@ def check_greedy(rowptr, colind, colors, seed):
         c = int(colors[v])
         assert c not in held
         assert held >= set(range(1, c)), "vertex %d could take a smaller colour" % v
-
-
-def graphs():
-    out = [("chesapeake",) + mtx_graph("chesapeake"), ("test_cc",) + mtx_graph("test_cc"),
-           ("test_bc",) + mtx_graph("test_bc"), ("test_sgm",) + mtx_graph("test_sgm")]
-    for scale in (10, 11, 12):
-        out.append(("rmat%d" % scale,) + orc.rmat_csr(scale))
-    return out
 
 
 @pytest.mark.parametrize("seed", [0, 1, 12345])
@@ -123,7 +101,7 @@ def test_oracle_depth_is_the_longest_priority_chain():
     src = np.arange(n - 1, dtype=np.int32)
     rp, ci = orc.build_csr(n, src, src + 1, True)
     _, ncolors, depth = greedy_oracle.gc(rp, ci, 7)
-    key = [(py_hash(7, v), v) for v in range(n)]
+    key = [(priority_hash(7, v), v) for v in range(n)]
     rounds = [0]*n
     for v in sorted(range(n), key=lambda v: key[v], reverse=True):
         rounds[v] = 1 + max([rounds[u] for u in ci[rp[v]:rp[v + 1]] if key[u] > key[v]],

@@ -8,37 +8,15 @@ takes, the sweeps (more than 32 undecided vertices per resident warp) and the ta
 long blocking chain, empty and isolated rows, self-loops, a directed matrix read
 through its CSR and its CSC, and dense, sparse and aliased candidate vectors.
 """
-import os
-
 import numpy as np
 import pytest
 
 import greedy_oracle
 import oracle_binding as orc
-from test_parity_gpu import make_matrix, path_graph, ragged_graph, star_graph
+from support import (gb, make_matrix, mtx_graph, path_graph, ragged_graph, star_graph,
+                     symmetric_csr)
 
 pytestmark = pytest.mark.gpu
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-GOLDEN = os.path.join(HERE, "golden")
-M32 = np.uint64(0xFFFFFFFF)
-
-
-@pytest.fixture(scope="module")
-def gb():
-    import graphblast_b200 as g
-    g.init(0)
-    return g
-
-
-def np_hash(seed, v):
-    """The priority hash of kernels/greedy_schedule.cuh over an array of vertices."""
-    x = (np.asarray(v, np.uint64) ^ np.uint64((seed*0x9E3779B9) & 0xFFFFFFFF)) & M32
-    x ^= x >> np.uint64(16)
-    x = (x*np.uint64(0x85EBCA6B)) & M32
-    x ^= x >> np.uint64(13)
-    x = (x*np.uint64(0xC2B2AE35)) & M32
-    return x ^ (x >> np.uint64(16))
 
 
 def run_mis(gb, A, n, seed=0, candidates=None, v=None):
@@ -49,24 +27,15 @@ def run_mis(gb, A, n, seed=0, candidates=None, v=None):
     return v.extractTuples(), nmembers
 
 
-def check(gb, rp, ci, seeds=(0,), dtype=None):
+def check(gb, rp, ci, seeds=(0,), integer=False):
     n = len(rp) - 1
-    A = make_matrix(gb, rp, ci, dtype=dtype)
+    A = make_matrix(gb, rp, ci, integer=integer)
     for seed in seeds:
         got, k = run_mis(gb, A, n, seed)
         want, want_k, _ = greedy_oracle.mis(rp, ci, seed)
         assert np.array_equal(got, want.astype(np.float32)), seed
         assert k == want_k, seed
     return A
-
-
-def mtx_graph(name):
-    n, src, dst, _ = orc.read_mtx_edges(os.path.join(GOLDEN, name + ".mtx"))
-    return orc.build_csr(n, src, dst, True)
-
-
-def symmetric_csr(n, src, dst):
-    return orc.build_csr(n, np.asarray(src, np.int32), np.asarray(dst, np.int32), True)
 
 
 @pytest.mark.parametrize("name", ["chesapeake", "test_cc", "test_bc", "test_sgm"])
@@ -186,14 +155,14 @@ def test_rmat(gb, scale):
 
 def test_int32_matrix(gb):
     rp, ci = orc.rmat_csr(12)
-    check(gb, rp, ci, seeds=(0, 6), dtype=gb.api.INT32)
+    check(gb, rp, ci, seeds=(0, 6), integer=True)
 
 
 def test_path_in_increasing_priority_order(gb):
     """A 20 000-vertex path whose vertices follow increasing priority: every vertex
     waits on the next one, so the tail resolves a chain of about 10 000 rounds."""
     n, seed = 20000, 21
-    order = np.argsort(np.asarray(np_hash(seed, np.arange(n))), kind="stable")
+    order = np.argsort(np.asarray(greedy_oracle.priority_hash(seed, np.arange(n))), kind="stable")
     rp, ci = symmetric_csr(n, order[:-1], order[1:])
     _, _, depth = greedy_oracle.mis(rp, ci, seed)
     assert depth >= 9000

@@ -16,13 +16,15 @@ import pytest
 
 import greedy_oracle
 import oracle_binding as orc
-from test_gc_oracle import M32, graphs, py_hash
+from greedy_oracle import M32, priority_hash
+from support import graphs
 
 
 def py_mis(n, rowptr, colind, seed, cand=None):
     """Sequential greedy MIS in decreasing (hash, v) order over the candidates."""
     member = [0]*n
-    for v in sorted(range(n), key=lambda v: (py_hash(seed & M32, v), v), reverse=True):
+    key = lambda v: (priority_hash(seed & M32, v), v)
+    for v in sorted(range(n), key=key, reverse=True):
         if cand is not None and not cand[v]:
             continue
         if not any(member[u] for u in colind[rowptr[v]:rowptr[v + 1]] if u != v):
@@ -34,7 +36,7 @@ def py_luby_rounds(n, rowptr, colind, seed, cand=None):
     """Synchronous Luby rounds with fixed priorities: each round, every undecided
     vertex above all its undecided neighbours joins, and it and its neighbours leave.
     Returns (member, rounds)."""
-    key = [(py_hash(seed & M32, v), v) for v in range(n)]
+    key = [(priority_hash(seed & M32, v), v) for v in range(n)]
     nbrs = [set(colind[rowptr[v]:rowptr[v + 1]]) - {v} for v in range(n)]
     undecided = {v for v in range(n) if cand is None or cand[v]}
     member = [0]*n

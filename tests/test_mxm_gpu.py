@@ -34,6 +34,7 @@ import numpy as np
 import pytest
 
 import oracle_binding as orc
+from support import Csr, csr, device_matrix, gb
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 KERNELS = os.path.join(ROOT, "graphblast_b200", "csrc", "graphblas", "backend",
@@ -51,52 +52,15 @@ POOL = 5000          # short rows / columns that serve as partners
 VALUES = np.array([-3, -2, -1, 1, 2, 3, 4, 5, 6, 7], np.int32)
 
 
-@pytest.fixture(scope="module")
-def gb():
-    import graphblast_b200 as g
-    g.init(0)
-    return g
-
-
 # ---------------------------------------------------------------------------
 # host-side sparse matrices
 # ---------------------------------------------------------------------------
 
-class Csr(collections.namedtuple("Csr", "nrows ncols ptr ind val")):
-    @property
-    def nnz(self):
-        return len(self.ind)
-
-    def rows(self):
-        return np.repeat(np.arange(self.nrows, dtype=np.int32), np.diff(self.ptr))
-
-    @property
-    def T(self):
-        """CSR of the transpose (= this matrix's CSC)."""
-        return csr(self.ncols, self.nrows, self.ind, self.rows(), self.val)
-
-    def padded(self, nrows, ncols):
-        """The same entries in a larger nrows x ncols matrix."""
-        assert nrows >= self.nrows and ncols >= self.ncols
-        ptr = np.concatenate([self.ptr, np.full(nrows - self.nrows, self.ptr[-1],
-                                                np.int32)])
-        return Csr(nrows, ncols, ptr, self.ind, self.val)
-
-    def with_values(self, val):
-        return Csr(self.nrows, self.ncols, self.ptr, self.ind,
-                   np.asarray(val, np.int32))
-
-
-def csr(nrows, ncols, rows, cols, vals):
-    rows = np.asarray(rows, np.int64)
-    cols = np.asarray(cols, np.int64)
-    order = np.lexsort((cols, rows))
-    rows, cols = rows[order], cols[order]
-    assert not np.any((np.diff(rows) == 0) & (np.diff(cols) == 0)), "duplicate entry"
-    ptr = np.zeros(nrows + 1, np.int64)
-    np.add.at(ptr, rows + 1, 1)
-    return Csr(nrows, ncols, np.cumsum(ptr).astype(np.int32), cols.astype(np.int32),
-               np.asarray(vals, np.int32)[order])
+def padded(S, nrows, ncols):
+    """The same entries in a larger nrows x ncols matrix."""
+    assert nrows >= S.nrows and ncols >= S.ncols
+    ptr = np.concatenate([S.ptr, np.full(nrows - S.nrows, S.ptr[-1], np.int32)])
+    return Csr(nrows, ncols, ptr, S.ind, S.val)
 
 
 def random_keys(rng, length, universe=K):
@@ -127,7 +91,7 @@ class Lists(object):
         rows = np.repeat(np.arange(len(self.keys)), [len(k) for k in self.keys])
         cols = np.concatenate(self.keys) if self.keys else np.zeros(0, np.int32)
         vals = self.rng.choice(VALUES, len(cols))
-        return csr(len(self.keys), universe, rows, cols, vals)
+        return csr(len(self.keys), universe, rows, cols, vals, np.int32)
 
 
 Problem = collections.namedtuple("Problem", "A Bt M")   # A m x k, B^T n x k, M m x n
@@ -178,7 +142,7 @@ def designed_problem(seed=7):
     A = rows.matrix()
     Bt = cols.matrix()
     r, c = zip(*entries)
-    M = csr(A.nrows, Bt.nrows, r, c, mask_values(rng, len(entries)))
+    M = csr(A.nrows, Bt.nrows, r, c, mask_values(rng, len(entries)), np.int32)
     return Problem(A, Bt, M)
 
 
@@ -189,7 +153,7 @@ def random_problem(seed, m, k, n, da, db, dm):
     def rand(nr, nc, d, vals):
         cnt = rng.binomial(nr*nc, d)
         flat = np.unique(rng.randint(0, nr*nc, cnt)) if cnt else np.zeros(0, int)
-        return csr(nr, nc, flat // nc, flat % nc, vals(len(flat)))
+        return csr(nr, nc, flat // nc, flat % nc, vals(len(flat)), np.int32)
 
     A = rand(m, k, da, lambda s: rng.choice(VALUES, s))
     Bt = rand(n, k, db, lambda s: rng.choice(VALUES, s))
@@ -231,24 +195,6 @@ def routes(p):
 # device side
 # ---------------------------------------------------------------------------
 
-def device_matrix(gb, S, with_csc=True):
-    """A Matrix adopting device copies of S's CSR and, with_csc, of its CSC;
-    without it the matrix has no column side (the search route for a mask)."""
-    import torch
-
-    def dev(a):
-        return torch.from_numpy(np.ascontiguousarray(a, np.int32)).cuda()
-
-    M = gb.Matrix(S.nrows, S.ncols, dtype=gb.api.INT32)
-    if with_csc:
-        T = S.T
-        M.build_device_csr(dev(S.ptr), dev(S.ind), dev(S.val), S.nnz,
-                           dev(T.ptr), dev(T.ind), dev(T.val))
-    else:
-        M.build_device_csr(dev(S.ptr), dev(S.ind), dev(S.val), S.nnz)
-    return M
-
-
 def check_entries(C, M, want):
     """C's pattern is M's and its values equal `want` bit for bit."""
     rp, ci, val = C.extract_csr()
@@ -265,9 +211,10 @@ def check_entries(C, M, want):
 
 
 def run_mxm(gb, C, p, route, A=None, B=None, mask=None, desc=None):
-    A = device_matrix(gb, p.A) if A is None else A
-    B = device_matrix(gb, p.Bt.T) if B is None else B
-    mask = device_matrix(gb, p.M, with_csc=(route == "hash")) if mask is None else mask
+    A = device_matrix(gb, p.A, integer=True) if A is None else A
+    B = device_matrix(gb, p.Bt.T, integer=True) if B is None else B
+    if mask is None:
+        mask = device_matrix(gb, p.M, csc=(route == "hash"), integer=True)
     gb.mxm(C, mask, None, gb.Semiring.PlusMultiplies, A, B,
            gb.Descriptor() if desc is None else desc)
     return C
@@ -362,15 +309,15 @@ def test_designed_shapes_transposed_operand(gb, designed, route, tran):
     as A^T).  The oracle is fed the explicit transposes."""
     p, want = designed
     N = K
-    P = Problem(p.A.padded(N, N), p.Bt.padded(N, N), p.M.padded(N, N))
+    P = Problem(padded(p.A, N, N), padded(p.Bt, N, N), padded(p.M, N, N))
     desc = gb.Descriptor()
     if tran == "inp1":
-        A = device_matrix(gb, P.A)
-        B = device_matrix(gb, P.Bt)                 # B^T stored
+        A = device_matrix(gb, P.A, integer=True)
+        B = device_matrix(gb, P.Bt, integer=True)                 # B^T stored
         desc.set(gb.Desc_field.GrB_INP1, gb.Desc_value.GrB_TRAN)
     else:
-        A = device_matrix(gb, P.A.T)                # A^T stored
-        B = device_matrix(gb, P.Bt.T)
+        A = device_matrix(gb, P.A.T, integer=True)                # A^T stored
+        B = device_matrix(gb, P.Bt.T, integer=True)
         desc.set(gb.Desc_field.GrB_INP0, gb.Desc_value.GrB_TRAN)
     C = gb.Matrix(N, N, dtype=gb.api.INT32)
     run_mxm(gb, C, P, route, A=A, B=B, desc=desc)
@@ -402,7 +349,7 @@ def test_output_matrix_reuse(gb, designed, route):
     p, want = designed
     rng = np.random.RandomState(11)
     C = gb.Matrix(p.M.nrows, p.M.ncols, dtype=gb.api.INT32)
-    B = device_matrix(gb, p.Bt.T)
+    B = device_matrix(gb, p.Bt.T, integer=True)
     run_mxm(gb, C, p, route, B=B)
     check_entries(C, p.M, want)
 
@@ -413,7 +360,7 @@ def test_output_matrix_reuse(gb, designed, route):
     check_entries(C, p2.M, want2)
 
     perm = rng.permutation(p.M.ncols)                  # same count, new pattern
-    M3 = csr(p.M.nrows, p.M.ncols, p.M.rows(), perm[p.M.ind], p.M.val)
+    M3 = csr(p.M.nrows, p.M.ncols, p.M.rows(), perm[p.M.ind], p.M.val, np.int32)
     p3 = p2._replace(M=M3)
     assert not np.array_equal(M3.ind, p.M.ind)
     run_mxm(gb, C, p3, route, B=B)
@@ -421,7 +368,7 @@ def test_output_matrix_reuse(gb, designed, route):
 
     keep = rng.rand(p.M.nnz) < 0.5                     # fewer entries
     rows = p.M.rows()
-    M4 = csr(p.M.nrows, p.M.ncols, rows[keep], p.M.ind[keep], p.M.val[keep])
+    M4 = csr(p.M.nrows, p.M.ncols, rows[keep], p.M.ind[keep], p.M.val[keep], np.int32)
     p4 = p2._replace(M=M4)
     run_mxm(gb, C, p4, route, B=B)
     check_entries(C, M4, oracle(p4))
@@ -443,7 +390,7 @@ def test_triangle_count_twice_on_the_same_output(gb):
     want = tc_per_entry(L.ptr, L.ind)
     desc = gb.Descriptor(mxvmode=0)
     for route in ROUTES:
-        dL = device_matrix(gb, L, with_csc=(route == "hash"))
+        dL = device_matrix(gb, L, csc=(route == "hash"), integer=True)
         B = gb.Matrix(L.nrows, L.nrows, dtype=gb.api.INT32)
         for _ in range(2):
             ntris, _ = algorithm.tc(dL, B, desc)

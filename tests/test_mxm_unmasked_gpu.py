@@ -26,6 +26,7 @@ import pytest
 
 import mxm_reference as ref
 import oracle_binding as orc
+from support import Csr, check_csr, csr, device_matrix, gb, random_csr
 
 SYM = (1024, 4096, 16384)
 NUM = (256, 2048, 8192)
@@ -33,64 +34,9 @@ VALUES = np.array([-4, -2, -1, -0.5, 0.5, 1, 2, 4], np.float32)
 ACCEPTED = [s for s in range(17) if s not in ref.ORDER_DEPENDENT]
 
 
-@pytest.fixture(scope="module")
-def gb():
-    import graphblast_b200 as g
-    g.init(0)
-    return g
-
-
 # ---------------------------------------------------------------------------
 # host-side operands
 # ---------------------------------------------------------------------------
-
-class Csr(object):
-    def __init__(self, nrows, ncols, ptr, ind, val):
-        self.nrows, self.ncols = nrows, ncols
-        self.ptr = np.asarray(ptr, np.int32)
-        self.ind = np.asarray(ind, np.int32)
-        self.val = np.asarray(val)
-
-    @property
-    def nnz(self):
-        return len(self.ind)
-
-    def rows(self):
-        return np.repeat(np.arange(self.nrows, dtype=np.int32), np.diff(self.ptr))
-
-    @property
-    def T(self):
-        return csr(self.ncols, self.nrows, self.ind, self.rows(), self.val)
-
-    def astype(self, dt):
-        return Csr(self.nrows, self.ncols, self.ptr, self.ind, self.val.astype(dt))
-
-
-def csr(nrows, ncols, rows, cols, vals):
-    rows, cols = np.asarray(rows, np.int64), np.asarray(cols, np.int64)
-    order = np.lexsort((cols, rows))
-    ptr = np.zeros(nrows + 1, np.int64)
-    np.add.at(ptr, rows + 1, 1)
-    return Csr(nrows, ncols, np.cumsum(ptr), cols[order], np.asarray(vals)[order])
-
-
-def random_csr(rng, nrows, ncols, density, values, zeros=0.1, empty=0.1):
-    """Mixed row lengths (a few rows 10x denser), some empty rows and columns,
-    about `zeros` of the stored values 0."""
-    d = np.full(nrows, density)
-    d[rng.rand(nrows) < 0.05] *= 10
-    d[rng.rand(nrows) < empty] = 0
-    dead_cols = rng.rand(ncols) < empty
-    rows, cols = [], []
-    for i in range(nrows):
-        c = np.nonzero((rng.rand(ncols) < d[i]) & ~dead_cols)[0]
-        rows.append(np.full(len(c), i))
-        cols.append(c)
-    rows, cols = np.concatenate(rows), np.concatenate(cols)
-    vals = rng.choice(values, len(cols)).astype(values.dtype)
-    vals[rng.rand(len(vals)) < zeros] = 0
-    return csr(nrows, ncols, rows, cols, vals)
-
 
 def reference(semiring, A, B, integer=False):
     rp, ci, val = ref.mxm(semiring, A.ptr, A.ind, A.val, B.ptr, B.ind, B.val,
@@ -121,9 +67,9 @@ def designed_rows(bound_count):
             left -= take
             first = False
     A = csr(len(bound_count), nb, a_rows, a_cols,
-            rng.choice(VALUES, len(a_cols)))
+            rng.choice(VALUES, len(a_cols)), np.float32)
     bc = np.concatenate(b_cols)
-    B = csr(nb, ncols, np.concatenate(b_rows), bc, rng.choice(VALUES, len(bc)))
+    B = csr(nb, ncols, np.concatenate(b_rows), bc, rng.choice(VALUES, len(bc)), np.float32)
     return A, B
 
 
@@ -147,42 +93,9 @@ DESIGNED = ([(u, 100) for u in _around(SYM[0])] +
 # device side
 # ---------------------------------------------------------------------------
 
-def device_matrix(gb, S, integer=False):
-    """A Matrix adopting device copies of S's CSR and CSC."""
-    import torch
-    vt = np.int32 if integer else np.float32
-
-    def dev(a, dt=np.int32):
-        return torch.from_numpy(np.ascontiguousarray(a, dt)).cuda()
-
-    M = gb.Matrix(S.nrows, S.ncols, dtype=gb.api.INT32 if integer else gb.api.FP32)
-    if S.nnz == 0:                      # adopting takes stored entries: ingest none
-        gb.api._check(M._lib.gb200_matrix_build_coo_device(M._h, None, None, None,
-                                                           0, 0), "empty matrix")
-        return M
-    T = S.T
-    M.build_device_csr(dev(S.ptr), dev(S.ind), dev(S.val, vt), S.nnz,
-                       dev(T.ptr), dev(T.ind), dev(T.val, vt))
-    return M
-
-
-def check(C, want):
-    rp, ci, val = C.extract_csr()
-    assert np.array_equal(rp, want.ptr), "row offsets differ"
-    assert np.array_equal(ci, want.ind), "column indices differ"
-    if val.dtype == np.float32:
-        ok = np.array_equal(val, want.val.astype(np.float32), equal_nan=True)
-    else:
-        ok = np.array_equal(val.astype(np.int64), want.val.astype(np.int64))
-    if not ok:
-        bad = np.nonzero(~((val == want.val) | (np.isnan(val) & np.isnan(want.val))))[0]
-        pytest.fail("%d of %d values differ, first at %d: got %r want %r" % (
-            len(bad), len(val), bad[0], val[bad[0]], want.val[bad[0]]))
-
-
 def run(gb, semiring, A, B, C=None, desc=None, integer=False):
-    dA = device_matrix(gb, A, integer)
-    dB = device_matrix(gb, B, integer)
+    dA = device_matrix(gb, A, integer=integer)
+    dB = device_matrix(gb, B, integer=integer)
     if C is None:
         C = gb.Matrix(A.nrows, B.ncols, dtype=gb.api.INT32 if integer else gb.api.FP32)
     gb.mxm(C, None, None, semiring, dA, dB, gb.Descriptor() if desc is None else desc)
@@ -223,7 +136,7 @@ def test_designed_operands_reach_every_limit():
 def test_every_float_semiring_rectangular(gb, semiring):
     A, B = operands(semiring, semiring)
     assert (np.diff(A.ptr) == 0).any() and (A.val == 0).any()
-    check(run(gb, semiring, A, B), reference(semiring, A, B))
+    check_csr(run(gb, semiring, A, B), reference(semiring, A, B))
 
 
 @pytest.mark.gpu
@@ -235,7 +148,7 @@ def test_order_dependent_semirings_refused(gb, semiring):
     with pytest.raises(gb.api.GraphBLASError) as err:
         run(gb, semiring, A, B, C=C)
     assert err.value.info == gb.api.Info.GrB_NOT_IMPLEMENTED
-    check(C, want)
+    check_csr(C, want)
 
 
 @pytest.mark.gpu
@@ -244,14 +157,14 @@ def test_int_plus_times(gb):
     ivals = np.array([-3, -2, -1, 1, 2, 3, 5, 7], np.int32)
     A = random_csr(rng, 310, 470, 0.03, ivals)
     B = random_csr(rng, 470, 190, 0.04, ivals)
-    check(run(gb, 1, A, B, integer=True), reference(1, A, B, integer=True))
+    check_csr(run(gb, 1, A, B, integer=True), reference(1, A, B, integer=True))
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("semiring", [1, 2])
 def test_every_bin_limit(gb, semiring):
     A, B = designed_rows(DESIGNED)
-    check(run(gb, semiring, A, B), reference(semiring, A, B))
+    check_csr(run(gb, semiring, A, B), reference(semiring, A, B))
 
 
 @pytest.mark.gpu
@@ -268,7 +181,7 @@ def test_transposed_operands(gb, tran):
     if tran in ("inp1", "both"):
         sB = B.T
         desc.set(gb.Desc_field.GrB_INP1, gb.Desc_value.GrB_TRAN)
-    check(run(gb, 1, sA, sB, desc=desc), reference(1, A, B))
+    check_csr(run(gb, 1, sA, sB, desc=desc), reference(1, A, B))
 
 
 @pytest.mark.gpu
@@ -291,11 +204,11 @@ def test_transposed_rectangular_operands(gb, tran):
     want = reference(1, A, B)
     C = gb.Matrix(40, 30)
     gb.mxm(C, None, None, 1, device_matrix(gb, sA), device_matrix(gb, sB), desc)
-    check(C, want)
+    check_csr(C, want)
     with pytest.raises(gb.api.GraphBLASError) as err:
         gb.mxm(C, None, None, 1, device_matrix(gb, A), device_matrix(gb, B), desc)
     assert err.value.info == gb.api.Info.GrB_DIMENSION_MISMATCH
-    check(C, want)
+    check_csr(C, want)
 
 
 @pytest.mark.gpu
@@ -306,11 +219,11 @@ def test_aliasing(gb):
     dA = device_matrix(gb, A)
     gb.mxm(dA, None, None, 1, dA, dA, gb.Descriptor())           # A = A*A
     AA = reference(1, A, A)
-    check(dA, AA)
+    check_csr(dA, AA)
     dA2 = device_matrix(gb, A)
     dC = device_matrix(gb, X)
     gb.mxm(dC, None, None, 1, dA2, dC, gb.Descriptor())          # C = A*C
-    check(dC, reference(1, A, X))
+    check_csr(dC, reference(1, A, X))
 
 
 def _dense(S):
@@ -331,16 +244,16 @@ def test_result_as_operand_and_mask(gb):
     for density in (0.02, 0.035):
         A = random_csr(rng, n, n, density, ivals, zeros=0)
         B = random_csr(rng, n, n, density, ivals, zeros=0)
-        gb.mxm(C, None, None, 1, device_matrix(gb, A, True), device_matrix(gb, B, True),
-               gb.Descriptor())
+        gb.mxm(C, None, None, 1, device_matrix(gb, A, integer=True),
+               device_matrix(gb, B, integer=True), gb.Descriptor())
         want = reference(1, A, B, integer=True)
-        check(C, want)
+        check_csr(C, want)
         # masked mxm with C as the mask
         X = random_csr(rng, n, n, 0.05, ivals, zeros=0)
         Y = random_csr(rng, n, n, 0.05, ivals, zeros=0)
         M = gb.Matrix(n, n, dtype=gb.api.INT32)
-        gb.mxm(M, C, None, 1, device_matrix(gb, X, True), device_matrix(gb, Y, True),
-               gb.Descriptor())
+        gb.mxm(M, C, None, 1, device_matrix(gb, X, integer=True),
+               device_matrix(gb, Y, integer=True), gb.Descriptor())
         Yt = Y.T
         got = M.extract_csr()
         exp = orc.mxm_masked(X.ptr, X.ind, X.val, Yt.ptr, Yt.ind, Yt.val,
@@ -356,7 +269,7 @@ def test_result_as_operand_and_mask(gb):
         gb.mxm(Cf, None, None, 1, device_matrix(gb, Af), device_matrix(gb, Bf),
                gb.Descriptor())
         want = reference(1, Af, Bf)
-        check(Cf, want)
+        check_csr(Cf, want)
         u = rng.choice(np.array([1, 2, -1], np.float32), n)
         D = _dense(want)
         for mode in (gb.Desc_value.GrB_PUSHONLY, gb.Desc_value.GrB_PULLONLY):
@@ -378,7 +291,7 @@ def test_chain_is_associative_on_integers(gb):
     rng = np.random.RandomState(12)
     ivals = np.array([-2, -1, 1, 2], np.int32)
     A = random_csr(rng, 150, 150, 0.04, ivals, zeros=0)
-    dA = device_matrix(gb, A, True)
+    dA = device_matrix(gb, A, integer=True)
     AA = gb.Matrix(150, 150, dtype=gb.api.INT32)
     gb.mxm(AA, None, None, 1, dA, dA, gb.Descriptor())
     left = gb.Matrix(150, 150, dtype=gb.api.INT32)
@@ -389,7 +302,7 @@ def test_chain_is_associative_on_integers(gb):
     for x, y in zip(l, r):
         assert np.array_equal(x, y)
     AAA = reference(1, reference(1, A, A, integer=True), A, integer=True)
-    check(left, AAA)
+    check_csr(left, AAA)
 
 
 @pytest.mark.gpu
@@ -397,17 +310,17 @@ def test_chain_is_associative_on_integers(gb):
 def test_edge_shapes(gb, shape):
     rng = np.random.RandomState(2)
     if shape == "1x1":
-        A = csr(1, 1, [0], [0], np.float32([2]))
-        B = csr(1, 1, [0], [0], np.float32([-0.5]))
+        A = csr(1, 1, [0], [0], np.float32([2]), np.float32)
+        B = csr(1, 1, [0], [0], np.float32([-0.5]), np.float32)
     else:
         m, k, n = (33, 65, 97) if shape == "odd" else (40, 50, 60)
         A = random_csr(rng, m, k, 0.1, VALUES)
         B = random_csr(rng, k, n, 0.1, VALUES)
         if shape == "nnzA0":
-            A = csr(m, k, [], [], np.zeros(0, np.float32))
+            A = csr(m, k, [], [], np.zeros(0, np.float32), np.float32)
         if shape == "nnzB0":
-            B = csr(k, n, [], [], np.zeros(0, np.float32))
-    check(run(gb, 1, A, B), reference(1, A, B))
+            B = csr(k, n, [], [], np.zeros(0, np.float32), np.float32)
+    check_csr(run(gb, 1, A, B), reference(1, A, B))
 
 
 def too_large(case):
@@ -420,12 +333,12 @@ def too_large(case):
     ones = lambda k: np.ones(k, np.float32)
     if case == "outer":
         m = n = 50000
-        A = csr(m, 1, np.arange(m), np.zeros(m), ones(m))
-        B = csr(1, n, np.zeros(n), np.arange(n), ones(n))
+        A = csr(m, 1, np.arange(m), np.zeros(m), ones(m), np.float32)
+        B = csr(1, n, np.zeros(n), np.arange(n), ones(n), np.float32)
     else:
         m, n = 131073, 16384
-        A = csr(m, 2, np.repeat(np.arange(m), 2), np.tile([0, 1], m), ones(2*m))
-        B = csr(2, n, np.repeat([0, 1], n // 2), np.arange(n), ones(n))
+        A = csr(m, 2, np.repeat(np.arange(m), 2), np.tile([0, 1], m), ones(2*m), np.float32)
+        B = csr(2, n, np.repeat([0, 1], n // 2), np.arange(n), ones(n), np.float32)
     return A, B
 
 
@@ -438,20 +351,20 @@ def test_size_limit(gb, case):
     A, B = too_large(case)
     m, k, n = A.nrows, A.ncols, B.ncols
     assert m * n > 2**31 - 1                 # every row of A*B is full
-    X = csr(m, k, [0, 5, m - 1], [0, 0, k - 1], np.float32([2, -1, 4]))
-    Y = csr(k, n, [0, 0, k - 1], [0, 7, n - 1], np.float32([0.5, 1, -2]))
+    X = csr(m, k, [0, 5, m - 1], [0, 0, k - 1], np.float32([2, -1, 4]), np.float32)
+    Y = csr(k, n, [0, 0, k - 1], [0, 7, n - 1], np.float32([0.5, 1, -2]), np.float32)
     want = reference(1, X, Y)
     C = run(gb, 1, X, Y)
-    check(C, want)
+    check_csr(C, want)
     dA, dB = device_matrix(gb, A), device_matrix(gb, B)
     t0 = time.time()
     with pytest.raises(gb.api.GraphBLASError) as err:
         gb.mxm(C, None, None, 1, dA, dB, gb.Descriptor())
     assert err.value.info == gb.api.Info.GrB_OUT_OF_MEMORY
     assert time.time() - t0 < 10
-    check(C, want)
+    check_csr(C, want)
     run(gb, 1, X, Y, C=C)
-    check(C, want)
+    check_csr(C, want)
 
 
 @pytest.mark.gpu

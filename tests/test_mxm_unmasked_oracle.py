@@ -9,6 +9,7 @@ import pytest
 
 import mxm_reference as ref
 import oracle_binding as orc
+from support import same
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 KERNELS = os.path.join(ROOT, "graphblast_b200", "csrc", "graphblas", "backend",
@@ -51,10 +52,6 @@ def as_dict(rp, ci, val):
         if rp[i + 1] > rp[i]:
             out[i] = {int(ci[e]): float(val[e]) for e in range(rp[i], rp[i + 1])}
     return out
-
-
-def same(x, y):
-    return x == y or (np.isnan(x) and np.isnan(y))
 
 
 @pytest.mark.parametrize("shape", [(1, 1, 1), (7, 13, 5), (40, 30, 60), (120, 90, 70)])

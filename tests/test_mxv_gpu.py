@@ -26,7 +26,6 @@ checks these numbers against the #defines):
                PUSH_SEG = 2050 frontier entries; edge-share hand-back to the pull
                from 4096 frontier entries under mxvmode 0
 """
-import ctypes as C
 import os
 import subprocess
 import sys
@@ -36,7 +35,7 @@ import pytest
 
 import mxm_reference as mref
 import mxv_reference as ref
-from test_spmm_gpu import Csr, csr
+from support import Csr, csr, device_matrix, gb, launch_count
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -68,19 +67,6 @@ def values(rng, regime, n):
     return (sign*rng.uniform(0.5, 2.0, n)).astype(np.float32)
 
 
-@pytest.fixture(scope="module")
-def gb():
-    import graphblast_b200 as g
-    g.init(0)
-    return g
-
-
-def launch_count(gb):
-    out = C.c_ulonglong(0)
-    gb.api._lib.load().gb200_launch_count(C.byref(out))
-    return out.value
-
-
 # ---------------------------------------------------------------------------
 # host-side structures
 # ---------------------------------------------------------------------------
@@ -99,11 +85,7 @@ def structure(rng, lengths, ncols, regime="int"):
     start = rng.randint(0, ncols, nrows)
     step = rng.choice(stride, nrows)
     cols = (start[rows] + pos*step[rows]) % ncols
-    return csr(nrows, ncols, rows, cols, values(rng, regime, len(rows)))
-
-
-def with_values(S, vals):
-    return Csr(S.nrows, S.ncols, S.ptr, S.ind, vals)
+    return csr(nrows, ncols, rows, cols, values(rng, regime, len(rows)), np.float32)
 
 
 def lengths_hitting(targets):
@@ -152,35 +134,6 @@ MERGE_CASES = merge_cases()
 # ---------------------------------------------------------------------------
 # device side
 # ---------------------------------------------------------------------------
-
-def _dev(a, dt, offset=0):
-    """Device copy of a, `offset` elements past an aligned allocation."""
-    import torch
-    a = np.ascontiguousarray(a, dt)
-    t = torch.zeros(len(a) + offset + 1, dtype=torch.float32 if dt == np.float32
-                    else torch.int32, device="cuda")
-    view = t[offset:offset + len(a)]
-    if len(a):
-        view.copy_(torch.from_numpy(a))
-    return view
-
-
-def device_matrix(gb, S, offset=0, M=None):
-    """Matrix adopting S's CSR and its CSC; colind / val `offset` elements past a
-    32-byte aligned address (offset 1: the lane-major merge kernel)."""
-    if M is None:
-        M = gb.Matrix(S.nrows, S.ncols)
-    if S.nnz == 0:
-        gb.api._check(M._lib.gb200_matrix_build_coo_device(M._h, None, None, None,
-                                                           0, 0), "empty matrix")
-        return M
-    T = S.T
-    M.build_device_csr(_dev(S.ptr, np.int32), _dev(S.ind, np.int32, offset),
-                       _dev(S.val, np.float32, offset), S.nnz,
-                       _dev(T.ptr, np.int32), _dev(T.ind, np.int32, offset),
-                       _dev(T.val, np.float32, offset))
-    return M
-
 
 def dense_vector(gb, x):
     v = gb.Vector(len(x))
@@ -262,8 +215,8 @@ def run_pull_case(gb, S, regime, seed, semirings=PULL_SEMIRINGS, offsets=(0, 1))
     u = values(rng, regime, S.ncols)
     mats = {}
     for off in offsets:
-        mats[("mxv", off)] = device_matrix(gb, S, off)       # pulls over its CSR
-        mats[("vxm", off)] = device_matrix(gb, S.T, off)     # pulls over its CSC
+        mats[("mxv", off)] = device_matrix(gb, S, offset=off)       # pulls over its CSR
+        mats[("vxm", off)] = device_matrix(gb, S.T, offset=off)     # pulls over its CSC
     for sem in semirings:
         want, bound = reference_pull(sem, S, u, regime)
         for orient in ("mxv", "vxm"):
@@ -342,7 +295,7 @@ def test_hub_designed(gb, case, regime):
         # row i holds columns i and i + 1 (mod ncols): every column exactly twice
         rows = np.repeat(np.arange(ncols), 2)
         cols = (rows + np.tile([0, 1], ncols)) % ncols
-        S = csr(ncols, ncols, rows, cols, values(rng, regime, len(rows)))
+        S = csr(ncols, ncols, rows, cols, values(rng, regime, len(rows)), np.float32)
         assert np.all(np.bincount(S.ind, minlength=ncols) == 2)
     else:
         S = structure(rng, lens, ncols, regime)
@@ -490,7 +443,7 @@ def test_pull_and_push_disagree_on_identity_valued_u(gb):
     short-circuit (FLT_MAX + -2^127 is finite), the push has one (the product is
     the identity).  Each route follows its own reference."""
     big = np.float32(-2.0**127)
-    S = csr(2, 3, [0, 0, 1], [0, 1, 2], np.float32([big, 1, 2]))
+    S = csr(2, 3, [0, 0, 1], [0, 1, 2], np.float32([big, 1, 2]), np.float32)
     At = device_matrix(gb, S)                 # vxm over A: pull over CSC, push over CSR
     u = np.float32([FLT_MAX, 1])
     want, _ = ref.pull(MINPLUS, S.T.ptr, S.T.ind, S.T.val, u)
@@ -696,7 +649,7 @@ def test_push_frontier_sizes(gb, nf):
     S_int = structure(rng, rng.randint(0, 7, n), n, "int")
     f = np.sort(rng.choice(n, nf, replace=False))
     for regime in ("int", "float"):
-        S = S_int if regime == "int" else with_values(S_int, values(rng, regime, S_int.nnz))
+        S = S_int if regime == "int" else S_int.with_values(values(rng, regime, S_int.nnz))
         M = device_matrix(gb, S)
         fv = values(rng, regime, nf)
         for sem in (PLUS, MINPLUS, MAXMUL):
@@ -717,7 +670,7 @@ def _gather_rows(S, f, fv, n):
     sub_rows = np.repeat(np.arange(len(f)), S.ptr[f + 1] - S.ptr[f])
     edge = np.concatenate([np.arange(S.ptr[r], S.ptr[r + 1]) for r in f]) \
         if len(f) else np.zeros(0, np.int64)
-    T = csr(n, len(f), S.ind[edge], sub_rows, S.val[edge])
+    T = csr(n, len(f), S.ind[edge], sub_rows, S.val[edge], np.float32)
     return T.ptr, T.ind, T.val, fv
 
 
@@ -774,7 +727,7 @@ def test_push_negative_and_identity_values(gb):
     for sem, ident in ((MINPLUS, FLT_MAX), (PLUS, 0.0), (MAXMUL, 0.0), (MINMUL, FLT_MAX)):
         vals = S.val.copy()
         vals[rng.rand(len(vals)) < 0.2] = ident
-        T = with_values(S, vals)
+        T = S.with_values(vals)
         M = device_matrix(gb, T)
         f = np.sort(rng.choice(n, 300, replace=False))
         fv = values(rng, "int", len(f))
@@ -803,7 +756,7 @@ def test_push_min_of_negative_and_negative_zero(gb, case):
         sem = MINSECOND
         weights = np.ones(len(rows), np.float32)
         u = np.where(first, -4, -0.0).astype(np.float32)
-    S = csr(len(rows), ncols, rows, cols, weights)
+    S = csr(len(rows), ncols, rows, cols, weights, np.float32)
     M = device_matrix(gb, S)
     got = run_push(gb, M, "vxm", sem, rows, u)
     want = ref.push(sem, S.ptr, S.ind, S.val, rows, u, ncols)
@@ -835,7 +788,7 @@ def test_caches_follow_a_rebuilt_structure(gb):
     mk = mask_values(rng, "any", n)
     ub = rng.choice(np.float32([0, 1]), n)
     for S in (S1, S2, S1):
-        device_matrix(gb, S, M=M)
+        device_matrix(gb, S, into=M)
         for sem in (PLUS, MINPLUS):
             want, bound = reference_pull(sem, S, u, "int")
             got, launches = pull(gb, M, "mxv", sem, u, count=True)

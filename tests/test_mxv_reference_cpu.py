@@ -11,6 +11,7 @@ import pytest
 import mxm_reference as mref
 import mxv_reference as ref
 import oracle_binding as orc
+from support import same
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CUDA = os.path.join(ROOT, "graphblast_b200", "csrc", "graphblas", "backend", "cuda")
@@ -35,12 +36,6 @@ def values_for(semiring, rng, n):
     if semiring != 11:
         pool = np.concatenate([pool, np.float32([-1, 1])])
     return rng.choice(pool, n).astype(np.float32)
-
-
-def same(x, y):
-    """Equal entry by entry, NaN equal to NaN."""
-    x, y = np.asarray(x, np.float32), np.asarray(y, np.float32)
-    return x.shape == y.shape and bool(np.all((x == y) | (np.isnan(x) & np.isnan(y))))
 
 
 SHAPES = [(1, 1), (7, 13), (40, 30), (90, 120)]

@@ -14,57 +14,13 @@ import numpy as np
 import pytest
 
 import oracle_binding as orc
+from support import gb, make_matrix, path_graph, ragged_graph, star_graph, transpose
 
 pytestmark = pytest.mark.gpu
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 GOLDEN = json.load(open(os.path.join(HERE, "golden", "golden.json")))
 FLT_MAX = np.finfo(np.float32).max
-
-
-@pytest.fixture(scope="module")
-def gb():
-    import graphblast_b200 as g
-    g.init(0)
-    return g
-
-
-def coo_of(rp, ci):
-    rows = np.repeat(np.arange(len(rp) - 1, dtype=np.int32), np.diff(rp))
-    return rows, ci.astype(np.int32)
-
-
-def make_matrix(gb, rp, ci, val=None, symmetric=True, dtype=None):
-    """Device-resident CSR (+CSC) adopted through Matrix::build(device pointers)."""
-    import torch
-    dtype = gb.api.FP32 if dtype is None else dtype
-    n = len(rp) - 1
-    tdt = torch.float32 if dtype == gb.api.FP32 else torch.int32
-    d_rp = torch.from_numpy(rp.astype(np.int32)).cuda()
-    d_ci = torch.from_numpy(ci.astype(np.int32)).cuda()
-    if val is None:
-        d_val = torch.ones(len(ci), dtype=tdt, device="cuda")
-    else:
-        d_val = torch.from_numpy(np.asarray(val)).to(tdt).cuda()
-    A = gb.Matrix(n, n, dtype=dtype)
-    if symmetric and val is None:
-        A.build_device_csr(d_rp, d_ci, d_val, len(ci), symmetric=True)
-    else:
-        # explicit transpose for the CSC side
-        rows, cols = coo_of(rp, ci)
-        order = np.lexsort((rows, cols))
-        t_rp = np.zeros(n + 1, dtype=np.int32)
-        np.add.at(t_rp, cols + 1, 1)
-        t_rp = np.cumsum(t_rp).astype(np.int32)
-        t_ci = rows[order].astype(np.int32)
-        v_np = np.ones(len(ci), dtype=np.float32) if val is None else np.asarray(val)
-        t_val = v_np[order]
-        d_trp = torch.from_numpy(t_rp).cuda()
-        d_tci = torch.from_numpy(t_ci).cuda()
-        d_tval = torch.from_numpy(t_val).to(tdt).cuda()
-        A.build_device_csr(d_rp, d_ci, d_val, len(ci), d_trp, d_tci, d_tval,
-                           symmetric=False)
-    return A
 
 
 def chesapeake():
@@ -77,28 +33,6 @@ def cc_graph():
     g = GOLDEN["test_cc"]
     return (np.array(g["rowptr"], dtype=np.int32),
             np.array(g["colind"], dtype=np.int32))
-
-
-def star_graph(nleaves):
-    """Vertex 0 adjacent to all others: one row of nleaves entries (spans many
-    merge-path tiles) plus nleaves rows of one entry."""
-    src = np.zeros(nleaves, dtype=np.int32)
-    dst = np.arange(1, nleaves + 1, dtype=np.int32)
-    return orc.build_csr(nleaves + 1, src, dst, True)
-
-
-def path_graph(n):
-    src = np.arange(n - 1, dtype=np.int32)
-    return orc.build_csr(n, src, src + 1, True)
-
-
-def ragged_graph():
-    """Empty rows at the start, middle and end; isolated vertices; n % 32 != 0."""
-    n = 1003
-    rng = np.random.RandomState(5)
-    src = rng.randint(100, 600, 4000).astype(np.int32)
-    dst = rng.randint(300, 900, 4000).astype(np.int32)
-    return orc.build_csr(n, src, dst, True)
 
 
 # ---------------------------------------------------------------------------
@@ -246,12 +180,8 @@ def test_mxv_matches_vxm_on_transpose(gb):
     rp, ci = orc.build_csr(n, src, dst, undirected=False)
     val = rng.randint(1, 5, len(ci)).astype(np.float32)
     A = make_matrix(gb, rp, ci, val, symmetric=False)
-    rows, cols = coo_of(rp, ci)
-    order = np.lexsort((rows, cols))
-    t_rp = np.zeros(n + 1, dtype=np.int32)
-    np.add.at(t_rp, cols + 1, 1)
-    t_rp = np.cumsum(t_rp).astype(np.int32)
-    t_ci, t_val = rows[order].astype(np.int32), val[order]
+    t_rp, t_ci, order = transpose(rp, ci)
+    t_val = val[order]
     u = rng.randint(1, 4, n).astype(np.float32)
     for mode in (1, 2):
         _, got, _, _ = run_vxm(gb, A, n, gb.PlusMultipliesSemiring, u_dense=u,
@@ -556,7 +486,7 @@ def test_triangle_count_exact(gb, graph):
     n = len(rp) - 1
     lr, lc = orc.tril(rp, ci)
     L = make_matrix(gb, lr, lc, np.ones(len(lc), np.int32), symmetric=False,
-                    dtype=gb.api.INT32)
+                    integer=True)
     B = gb.Matrix(n, n, dtype=gb.api.INT32)
     desc = gb.Descriptor(mxvmode=0)
     ntris, _ = algorithm.tc(L, B, desc)

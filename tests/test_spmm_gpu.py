@@ -24,6 +24,7 @@ import numpy as np
 import pytest
 
 import mxm_reference as ref
+from support import Csr, csr, device_matrix, gb, launch_count
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 KERNELS = os.path.join(ROOT, "graphblast_b200", "csrc", "graphblas", "backend",
@@ -54,49 +55,9 @@ def lanes_for(n):
     return lanes
 
 
-@pytest.fixture(scope="module")
-def gb():
-    import graphblast_b200 as g
-    g.init(0)
-    return g
-
-
 # ---------------------------------------------------------------------------
 # host-side operands
 # ---------------------------------------------------------------------------
-
-class Csr(object):
-    def __init__(self, nrows, ncols, ptr, ind, val):
-        self.nrows, self.ncols = nrows, ncols
-        self.ptr = np.asarray(ptr, np.int64)
-        self.ind = np.asarray(ind, np.int64)
-        self.val = np.asarray(val, np.float32)
-
-    @property
-    def nnz(self):
-        return len(self.ind)
-
-    def rows(self):
-        return np.repeat(np.arange(self.nrows), np.diff(self.ptr))
-
-    @property
-    def T(self):
-        return csr(self.ncols, self.nrows, self.ind, self.rows(), self.val)
-
-    def scipy(self, dtype=np.float64):
-        import scipy.sparse as sp
-        return sp.csr_matrix((self.val.astype(dtype), self.ind, self.ptr),
-                             shape=(self.nrows, self.ncols))
-
-
-def csr(nrows, ncols, rows, cols, vals):
-    rows, cols = np.asarray(rows, np.int64), np.asarray(cols, np.int64)
-    order = np.lexsort((cols, rows))
-    ptr = np.zeros(nrows + 1, np.int64)
-    np.add.at(ptr, rows + 1, 1)
-    return Csr(nrows, ncols, np.cumsum(ptr), cols[order],
-               np.asarray(vals, np.float32)[order])
-
 
 def values_for(semiring):
     return np.array([-1, 1], np.float32) if semiring == 11 else VALUES
@@ -110,7 +71,7 @@ def random_csr(rng, nrows, ncols, density, values, zeros=0.1, empty=0.1):
     rows, cols = np.nonzero(mask)
     vals = rng.choice(values, len(cols)).astype(np.float32)
     vals[rng.rand(len(vals)) < zeros] = 0
-    return csr(nrows, ncols, rows, cols, vals)
+    return csr(nrows, ncols, rows, cols, vals, np.float32)
 
 
 def dense_values(rng, shape, values, zeros=0.1):
@@ -132,7 +93,7 @@ def designed_rows(rng, ncols, values):
     rows, cols = np.concatenate(rows), np.concatenate(cols)
     vals = rng.choice(values, len(cols)).astype(np.float32)
     vals[rng.rand(len(vals)) < 0.05] = 0
-    return csr(len(lengths), ncols, rows, cols, vals), lengths
+    return csr(len(lengths), ncols, rows, cols, vals, np.float32), lengths
 
 
 def reference(semiring, A, B):
@@ -161,24 +122,6 @@ def check(got, want):
 # device side
 # ---------------------------------------------------------------------------
 
-def device_matrix(gb, S):
-    """A Matrix adopting device copies of S's CSR and CSC."""
-    import torch
-
-    def dev(a, dt=np.int32):
-        return torch.from_numpy(np.ascontiguousarray(a, dt)).cuda()
-
-    M = gb.Matrix(S.nrows, S.ncols)
-    if S.nnz == 0:
-        gb.api._check(M._lib.gb200_matrix_build_coo_device(M._h, None, None, None,
-                                                           0, 0), "empty matrix")
-        return M
-    T = S.T
-    M.build_device_csr(dev(S.ptr), dev(S.ind), dev(S.val, np.float32), S.nnz,
-                       dev(T.ptr), dev(T.ind), dev(T.val, np.float32))
-    return M
-
-
 def dense_matrix(gb, B):
     M = gb.Matrix(B.shape[0], B.shape[1])
     M.build_dense(B)
@@ -198,12 +141,6 @@ def refused(gb, code, fn):
     with pytest.raises(gb.api.GraphBLASError) as err:
         fn()
     assert err.value.info == code
-
-
-def launch_count(gb):
-    out = C.c_ulonglong(0)
-    gb.api._lib.load().gb200_launch_count(C.byref(out))
-    return out.value
 
 
 # ---------------------------------------------------------------------------
@@ -318,13 +255,9 @@ def test_refusals_leave_c_unchanged(gb):
 
 @pytest.mark.gpu
 def test_csr_only_a_under_transpose(gb):
-    import torch
     A, B = _operands(n=8)
     AT_rows = A.ncols
-    dA = gb.Matrix(A.nrows, A.ncols)
-    dA.build_device_csr(torch.from_numpy(A.ptr.astype(np.int32)).cuda(),
-                        torch.from_numpy(A.ind.astype(np.int32)).cuda(),
-                        torch.from_numpy(A.val).cuda(), A.nnz)
+    dA = device_matrix(gb, A, csc=False)
     dB = dense_matrix(gb, np.ones((A.nrows, 8), np.float32))
     Cm = gb.Matrix(AT_rows, 8)
     desc = gb.Descriptor()
@@ -349,7 +282,7 @@ def hub_operand(rng, values, hub=300000):
     else:
         vals = rng.choice(values, len(cols)).astype(np.float32)
         vals[rng.rand(len(vals)) < 0.05] = 0
-    return csr(m, k, rows, cols, vals)
+    return csr(m, k, rows, cols, vals, np.float32)
 
 
 @pytest.mark.gpu
@@ -521,7 +454,7 @@ def test_storage_switches(gb):
 @pytest.mark.gpu
 @pytest.mark.parametrize("semiring", [1, 2])
 def test_no_entries_gives_identity(gb, semiring):
-    A = Csr(50, 40, np.zeros(51), [], [])
+    A = Csr(50, 40, np.zeros(51), [], np.float32([]))
     B = dense_values(np.random.RandomState(1), (40, 9), VALUES)
     got = spmm(gb, semiring, A, B)
     assert (got == ref.SEMIRINGS[semiring][2]).all()
@@ -530,7 +463,7 @@ def test_no_entries_gives_identity(gb, semiring):
 
 @pytest.mark.gpu
 def test_one_by_one(gb):
-    A = Csr(1, 1, [0, 1], [0], [-2])
+    A = Csr(1, 1, [0, 1], [0], np.float32([-2]))
     check(spmm(gb, 1, A, np.array([[4]], np.float32)), np.array([[-8]], np.float32))
 
 
@@ -539,8 +472,9 @@ def test_dense_size_limits(gb):
     """m*N > INT32_MAX is refused before anything is allocated, C unchanged."""
     import torch
     m, n = 65536, 32769
-    A = Csr(m, 1, np.r_[0, np.arange(1, m + 1) <= 3].cumsum(), [0, 0, 0], [1, 2, 4])
-    S = Csr(1, n, [0, 2], [0, n - 1], [1, -1])
+    A = Csr(m, 1, np.r_[0, np.arange(1, m + 1) <= 3].cumsum(), [0, 0, 0],
+            np.float32([1, 2, 4]))
+    S = Csr(1, n, [0, 2], [0, n - 1], np.float32([1, -1]))
     dA, dS = device_matrix(gb, A), device_matrix(gb, S)
     Cm = gb.Matrix(m, n)
     gb.mxm(Cm, None, None, 1, dA, dS, gb.Descriptor())

@@ -9,19 +9,13 @@ import numpy as np
 import pytest
 
 import oracle_binding as orc
+from support import gb
 
 pytestmark = [pytest.mark.gpu]
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 REF = np.load(os.path.join(GOLDEN, "reference_cpu.npz"))
-
-
-@pytest.fixture(scope="module")
-def gb():
-    import graphblast_b200 as g
-    g.init(0)
-    return g
 
 
 @pytest.mark.parametrize("n,bits", [(1, 8), (2, 16), (100, 24), (2048, 8), (2049, 40),

@@ -9,18 +9,11 @@ import numpy as np
 import pytest
 
 import oracle_binding as orc
-from test_parity_gpu import make_matrix, ragged_graph
+from support import gb, make_matrix, ragged_graph
 
 pytestmark = [pytest.mark.gpu]
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-@pytest.fixture(scope="module")
-def gb():
-    import graphblast_b200 as g
-    g.init(0)
-    return g
 
 
 @pytest.mark.parametrize("name", ["PlusMultiplies", "MinimumPlus", "MaximumMultiplies"])

@@ -23,7 +23,7 @@ Workloads:
 
 Each line is one JSON record.  "ms" is the median of the CUDA-event times that cc
 returns for warm calls.  A time is quoted only after the labels equal the checker's
-(tests/test_cc_gpu.py components: scipy's weak components, each label mapped to its
+(tests/support.py components: scipy's weak components, each label mapped to its
 component's minimum id) entry for entry and the counts agree ("equals_checker");
 "cpu_ms" is that checker's time on one host thread.  "bfs_ms" is the median tight time
 of algorithm.bfs from the highest-degree vertex on the same matrix (direction-optimised,
@@ -48,7 +48,7 @@ sys.path.insert(0, os.path.join(os.path.dirname(HERE), "tests"))
 from bench_mxm import card, grid27                # noqa: E402
 import graphblast_b200 as gb                      # noqa: E402
 from graphblast_b200 import algorithm, graphs     # noqa: E402
-from test_cc_gpu import components                # noqa: E402
+from support import components                    # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12
 
