@@ -57,31 +57,49 @@ struct BfsDistArgs {
   size_t off_data[2], off_flags2, off_visited[2];
   size_t word_lo, nw, total_words;
   unsigned long long epoch0;         // publishes completed before this traversal
-  unsigned long long* cells;         // [0..2] found (rotating) [3..5] heavy (rotating)
-                                     // [6] unused [7] levels out [8] error
-                                     // [9..11] CTA check-in of the publish (rotating)
+  unsigned long long* cells;         // [GBX_CELLS_BYTES / 8], indexed by BfsDistCell
   Index* heavy;
   long long timeout_cycles;
 };
 
-__device__ __forceinline__ bool distClaim(unsigned int* visited, long long vtx) {
-  const unsigned int bit = 1u << (vtx & 31);
-  unsigned int* word = visited + (vtx >> 5);
-  if (*reinterpret_cast<volatile unsigned int*>(word) & bit) return false;
-  return (atomicOr(word, bit) & bit) == 0;
-}
+// Bytes the host reserves for BfsDistArgs::cells.
+#define GBX_CELLS_BYTES 1024
+// Levels with trace cells: levels 0..11.
+#define GBX_TRACE_LEVELS 12
 
-__device__ __forceinline__ unsigned long long distNow() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return t;
-}
+// The cells of BfsDistArgs::cells.  The rotating triples are used as in the
+// single-GPU kernel (bfsLevelCell).
+enum BfsDistCell {
+  GBX_CELL_FOUND = 0,                    // rotating: vertices this rank found
+  GBX_CELL_HEAVY = GBX_CELL_FOUND + 3,   // rotating: heavy-list length
+  GBX_CELL_LEVELS = 7,                   // levels executed (out)
+  GBX_CELL_ERROR,                        // 1: the cross-GPU barrier timed out (out)
+  GBX_CELL_CHECKIN,                      // rotating: CTAs that checked in to the publish
+  // time stamps of level L, slot k, thread 0 of the grid, nanoseconds, GB200_BFS_TRACE
+  // only: cell GBX_CELL_TRACE + GBX_TRACE_STRIDE*L + k
+  GBX_CELL_TRACE = 16,
+  GBX_TRACE_STRIDE = 8
+};
+// The slots of a traced level.  A level reaches them in the order start, local,
+// stores, fence, check-in, barrier, end.
+enum BfsDistTraceSlot {
+  GBX_T_START = 0,                       // level start
+  GBX_T_LOCAL,                           // local phase done
+  GBX_T_BARRIER,                         // cross-GPU barrier passed
+  GBX_T_END,                             // level end
+  GBX_T_STORES,                          // slice stored to every rank
+  GBX_T_FENCE,                           // system-scope fence done
+  GBX_T_CHECKIN,                         // checked in (the last CTA: flags posted)
+  GBX_T_NSLOTS
+};
+static_assert(GBX_T_NSLOTS <= GBX_TRACE_STRIDE, "a level's trace slots overlap the next's");
+static_assert((GBX_CELL_TRACE + GBX_TRACE_STRIDE*(GBX_TRACE_LEVELS - 1) + GBX_T_NSLOTS)*
+                  sizeof(unsigned long long) <= GBX_CELLS_BYTES,
+              "the trace cells of the last traced level are past the cells");
 
-// Phase time stamps of the first 12 levels (thread 0 of the grid, nanoseconds):
-// cells[16 + 4*level + {0: level start, 1: local phase done, 2: barrier passed,
-// 3: level end}]; read by the host when GB200_BFS_TRACE=1.
-#define GBX_TRACE(slot) do {                                                  \
-  if (gtid == 0 && level < 12) a.cells[16 + 8*level + (slot)] = distNow();    \
+#define GBX_TRACE(slot) do {                                                         \
+  if (gtid == 0 && level < GBX_TRACE_LEVELS)                                         \
+    a.cells[GBX_CELL_TRACE + GBX_TRACE_STRIDE*level + (slot)] = bfsClockNs();        \
 } while (0)
 
 __global__ void __launch_bounds__(GBX_BFS_NT, 2)
@@ -121,7 +139,7 @@ bfsFusedDistKernel(BfsDistArgs a) {
     a.seed[w] = seed;
   }
   for (Index w = gtid; w < nw + 8; w += gthreads) a.next_own[w] = 0u;
-  if (gtid < 12) a.cells[gtid] = 0ull;
+  if (gtid < GBX_CELL_CHECKIN + 3) a.cells[gtid] = 0ull;
   grid.sync();
 
   const unsigned int* F = a.seed;
@@ -140,16 +158,16 @@ bfsFusedDistKernel(BfsDistArgs a) {
         if (ratio <= a.switchpoint && ratio < prev_ratio) dense = false; else prev_ratio = ratio;
       }
     }
-    unsigned long long* const found_cell = a.cells + (level % 3);
-    unsigned long long* const heavy_cell = a.cells + 3 + (level % 3);
+    unsigned long long* const found_cell = bfsLevelCell(a.cells, GBX_CELL_FOUND, level);
+    unsigned long long* const heavy_cell = bfsLevelCell(a.cells, GBX_CELL_HEAVY, level);
     if (gtid == 0) {
-      a.cells[(level + 1) % 3] = 0ull;
-      a.cells[3 + (level + 1) % 3] = 0ull;
+      bfsZeroNextCell(a.cells, GBX_CELL_FOUND, level);
+      bfsZeroNextCell(a.cells, GBX_CELL_HEAVY, level);
     }
     const float next_level = static_cast<float>(level + 1);
     int found_here = 0;
     unsigned int* const vis = vis_copy[level & 1];     // as of the level's start
-    GBX_TRACE(0);
+    GBX_TRACE(GBX_T_START);
 
     if (!dense) {
       // ---------------- push over the local CSC --------------------------------------
@@ -179,7 +197,7 @@ bfsFusedDistKernel(BfsDistArgs a) {
             }
             for (Index k = lane; k < deg; k += 32) {
               const Index r = __ldg(a.push_ind + beg + k);      // owned, local id
-              if (distClaim(vis, a.lo + r)) {
+              if (bfsClaim(vis, a.lo + r)) {
                 a.levels[r] = next_level;
                 atomicOr(a.next_own + (r >> 5), 1u << (r & 31));
                 ++found_here;
@@ -197,7 +215,7 @@ bfsFusedDistKernel(BfsDistArgs a) {
         const Index deg = __ldg(a.push_ptr + u + 1) - beg;
         for (Index k = gtid; k < deg; k += gthreads) {
           const Index r = __ldg(a.push_ind + beg + k);
-          if (distClaim(vis, a.lo + r)) {
+          if (bfsClaim(vis, a.lo + r)) {
             a.levels[r] = next_level;
             atomicOr(a.next_own + (r >> 5), 1u << (r & 31));
             ++found_here;
@@ -257,7 +275,7 @@ bfsFusedDistKernel(BfsDistArgs a) {
     if (threadIdx.x == 0 && block_found)
       atomicAdd(found_cell, static_cast<unsigned long long>(block_found));
     grid.sync();
-    GBX_TRACE(1);
+    GBX_TRACE(GBX_T_LOCAL);
 
     // ---------------- publish the owned slice, cross-GPU level barrier -----------------
     // Every CTA stores its share of the slice into every rank's buffer and checks
@@ -296,13 +314,13 @@ bfsFusedDistKernel(BfsDistArgs a) {
     // one system-scope fence per CTA, after the CTA barrier: cumulativity carries
     // the other threads' peer stores
     __syncthreads();
-    GBX_TRACE(4);
+    GBX_TRACE(GBX_T_STORES);
     if (threadIdx.x == 0) {
       __threadfence_system();
-      GBX_TRACE(5);
-      unsigned long long* const done_cell = a.cells + 9 + (level % 3);
+      GBX_TRACE(GBX_T_FENCE);
+      unsigned long long* const done_cell = bfsLevelCell(a.cells, GBX_CELL_CHECKIN, level);
       if (atomicAdd(done_cell, 1ull) == gridDim.x - 1) {
-        a.cells[9 + (level + 1) % 3] = 0ull;           // next level's check-in counter
+        bfsZeroNextCell(a.cells, GBX_CELL_CHECKIN, level);
         __threadfence();
         const unsigned long long mine =
             *reinterpret_cast<volatile unsigned long long*>(found_cell);
@@ -312,7 +330,7 @@ bfsFusedDistKernel(BfsDistArgs a) {
           reinterpret_cast<volatile unsigned long long*>(
               a.peers[p] + a.off_flags2)[a.rank] = word;
       }
-      GBX_TRACE(6);
+      GBX_TRACE(GBX_T_CHECKIN);
       const volatile unsigned long long* flags =
           reinterpret_cast<const volatile unsigned long long*>(local + a.off_flags2);
       const long long t0 = clock64();
@@ -328,19 +346,19 @@ bfsFusedDistKernel(BfsDistArgs a) {
         total += seen & 0xffffffffull;
       }
       __threadfence_system();
-      if (!ok) { total = 0ull; a.cells[8] = 1ull; }
+      if (!ok) { total = 0ull; a.cells[GBX_CELL_ERROR] = 1ull; }
       s_total = total;
       s_failed = !ok;
     }
     __syncthreads();
     fcount = s_total;
     failed = s_failed;
-    GBX_TRACE(2);
+    GBX_TRACE(GBX_T_BARRIER);
 
     F = reinterpret_cast<const unsigned int*>(local + a.off_data[par]);
-    GBX_TRACE(3);
+    GBX_TRACE(GBX_T_END);
   }
-  if (gtid == 0) a.cells[7] = static_cast<unsigned long long>(level - 1);
+  if (gtid == 0) a.cells[GBX_CELL_LEVELS] = static_cast<unsigned long long>(level - 1);
 }
 
 }  // namespace gbx
@@ -383,7 +401,7 @@ int gb200_dist_bfs_fused(gb200_xchg_t x, gb200_vector_t v, gb200_matrix_t M,
   const size_t nw = x->word_off[x->rank + 1] - w_lo;
   const size_t own_bytes = ((nw + 8)*4 + 255)/256*256;
   unsigned char* base = reinterpret_cast<unsigned char*>(d.scratch(GB_SCRATCH_BFS,
-      own_bytes + 1024 + GB_BFS_HEAVY_CAP*sizeof(Index)));
+      own_bytes + GBX_CELLS_BYTES + GB_BFS_HEAVY_CAP*sizeof(Index)));
   gbx::BfsDistArgs a;
   a.pull_ptr = S.d_csrRowPtr_;  a.pull_ind = S.d_csrColInd_;
   a.pull_first = first;
@@ -400,7 +418,7 @@ int gb200_dist_bfs_fused(gb200_xchg_t x, gb200_vector_t v, gb200_matrix_t M,
   a.seed = x->d_seed;
   a.next_own = reinterpret_cast<unsigned int*>(base);
   a.cells = reinterpret_cast<unsigned long long*>(base + own_bytes);
-  a.heavy = reinterpret_cast<Index*>(base + own_bytes + 1024);
+  a.heavy = reinterpret_cast<Index*>(base + own_bytes + GBX_CELLS_BYTES);
   a.peers = x->d_peer;
   a.world = x->world;  a.rank = x->rank;
   a.off_data[0] = x->off_data[0];  a.off_data[1] = x->off_data[1];
@@ -410,36 +428,36 @@ int gb200_dist_bfs_fused(gb200_xchg_t x, gb200_vector_t v, gb200_matrix_t M,
   a.epoch0 = x->epoch;
   a.timeout_cycles = 20000000000ll;
 
-  void (*kernel)(gbx::BfsDistArgs) = gbx::bfsFusedDistKernel;
-  static int resident = 0;
-  if (resident == 0) {
-    int per_sm = 0;
-    CUDA_CALL(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, GBX_BFS_NT, 0));
-    resident = per_sm*runtime().sm_count;
-    if (resident < 1) return rc(GrB_PANIC);
-  }
+  const int grid = cooperativeGrid<gbx::bfsFusedDistKernel, GBX_BFS_NT>();
+  if (grid < 1) return rc(GrB_PANIC);
   void* params[] = { &a };
   profiler().begin(GB_PROF_PULL_BOOL, s);
-  CUDA_CALL(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kernel), dim3(resident),
+  CUDA_CALL(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(gbx::bfsFusedDistKernel),
+      dim3(grid),
       dim3(GBX_BFS_NT), params, 0, s));
   GB_KERNEL_CHECK();
   profiler().end(GB_PROF_PULL_BOOL, s, 0.0);
   v->f->vector_.dense_.touched();
   // every rank ran the same number of levels = publishes
-  unsigned long long out[2];
-  CUDA_CALL(cudaMemcpyAsync(out, a.cells + 7, 2*sizeof(unsigned long long),
+  static_assert(gbx::GBX_CELL_ERROR == gbx::GBX_CELL_LEVELS + 1,
+                "levels and error are read together");
+  unsigned long long out[2];              // levels, error
+  CUDA_CALL(cudaMemcpyAsync(out, a.cells + gbx::GBX_CELL_LEVELS, sizeof(out),
       cudaMemcpyDeviceToHost, s));
   runtime().sync();
   x->epoch += out[0];
-  static const int trace = getEnv("GB200_BFS_TRACE", 0);
-  if (trace) {
-    unsigned long long t[112];
-    CUDA_CALL(cudaMemcpy(t, a.cells + 16, sizeof(t), cudaMemcpyDeviceToHost));
-    for (unsigned long long l = 1; l <= out[0] && l < 12; ++l)
+  if (bfsTrace()) {
+    unsigned long long t[gbx::GBX_TRACE_STRIDE*GBX_TRACE_LEVELS];
+    CUDA_CALL(cudaMemcpy(t, a.cells + gbx::GBX_CELL_TRACE, sizeof(t), cudaMemcpyDeviceToHost));
+    for (unsigned long long l = 1; l <= out[0] && l < GBX_TRACE_LEVELS; ++l) {
+      const unsigned long long* const at = t + gbx::GBX_TRACE_STRIDE*l;
       fprintf(stderr, "rank %d level %llu: local %.1f | stores %.1f fence %.1f check-in %.1f "
-              "wait %.1f us\n", x->rank, l, (t[8*l + 1] - t[8*l])*1e-3,
-              (t[8*l + 4] - t[8*l + 1])*1e-3, (t[8*l + 5] - t[8*l + 4])*1e-3,
-              (t[8*l + 6] - t[8*l + 5])*1e-3, (t[8*l + 2] - t[8*l + 6])*1e-3);
+              "wait %.1f us\n", x->rank, l, (at[gbx::GBX_T_LOCAL] - at[gbx::GBX_T_START])*1e-3,
+              (at[gbx::GBX_T_STORES] - at[gbx::GBX_T_LOCAL])*1e-3,
+              (at[gbx::GBX_T_FENCE] - at[gbx::GBX_T_STORES])*1e-3,
+              (at[gbx::GBX_T_CHECKIN] - at[gbx::GBX_T_FENCE])*1e-3,
+              (at[gbx::GBX_T_BARRIER] - at[gbx::GBX_T_CHECKIN])*1e-3);
+    }
   }
   if (levels_out != NULL) *levels_out = static_cast<int>(out[0]);
   return out[1] != 0ull ? rc(GrB_PANIC) : 0;

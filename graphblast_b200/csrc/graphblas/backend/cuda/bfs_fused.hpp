@@ -13,8 +13,6 @@ namespace backend {
 
 // True when the traversal described by desc is the one the fused kernel computes.
 inline bool bfsFusedApplies(Descriptor* desc) {
-  static const int enabled = getEnv("GB200_BFS_FUSED", 1);
-  if (!enabled) return false;
   Desc_value mask_mode, outp, inp0, inp1;
   if (desc->get(GrB_MASK, &mask_mode) != GrB_SUCCESS) return false;
   desc->get(GrB_OUTP, &outp); desc->get(GrB_INP0, &inp0); desc->get(GrB_INP1, &inp1);
@@ -23,17 +21,57 @@ inline bool bfsFusedApplies(Descriptor* desc) {
          inp1 == GrB_DEFAULT && !desc->debug() && desc->timing_ != 1;
 }
 
+// GB200_BFS_TRACE=1: every fused traversal, single- or multi-GPU, prints its
+// per-level times on stderr.  Read once per process.
+inline bool bfsTrace() {
+  static const bool on = getEnv("GB200_BFS_TRACE", 0) != 0;
+  return on;
+}
+
+// Layout of GB_SCRATCH_BFS for a traversal of n vertices: the byte offset of each
+// array of BfsFusedArgs, each on a 256-byte boundary, and the bytes of the slot.
+struct BfsScratchLayout {
+  size_t visited[2], frontier, next, counters, heavy, walk, walk_count, walk_chunks,
+         level8, bytes;
+};
+
+inline BfsScratchLayout bfsScratchLayout(Index n) {
+  const size_t nwords = (static_cast<size_t>(n) + 31)/32;
+  const size_t nchunks = (nwords + 31)/32;
+  BfsScratchLayout l;
+  size_t at = 0;
+  auto place = [&at](size_t bytes) {
+    const size_t off = at;
+    at += (bytes + 255)/256*256;
+    return off;
+  };
+  l.visited[0]  = place(nwords*sizeof(unsigned int));
+  l.visited[1]  = place(nwords*sizeof(unsigned int));
+  l.frontier    = place(nwords*sizeof(unsigned int));
+  l.next        = place(nwords*sizeof(unsigned int));
+  l.counters    = place(GB_BFS_NCOUNTERS*sizeof(unsigned long long));
+  l.heavy       = place(GB_BFS_HEAVY_CAP*sizeof(Index));
+  l.walk        = place(nchunks*GB_BFS_CHUNK*sizeof(Index));
+  l.walk_count  = place(nchunks*sizeof(int));
+  l.walk_chunks = place(nchunks*sizeof(Index));
+  l.level8      = place(static_cast<size_t>(n));
+  l.bytes = at;
+  return l;
+}
+
 // Work counters of the last fused traversal run with this descriptor: levels,
 // entries inspected pulling, pull levels, vertices pushed, edges pushed, vertices
 // discovered pushing.  Zeros when none has run.
 inline void bfsFusedStats(Descriptor* desc, Index n, unsigned long long out[6]) {
+  static_assert(GB_BFS_CELL_FOUND_PUSHING == GB_BFS_CELL_LEVELS + 5,
+                "the six result cells are not consecutive");
   for (int i = 0; i < 6; ++i) out[i] = 0ull;
-  const size_t nwords = (static_cast<size_t>(n) + 31)/32;
-  const size_t words_bytes = ((nwords*sizeof(unsigned int) + 255)/256)*256;
-  if (desc->scratchSize(GB_SCRATCH_BFS) < 4*words_bytes + 256) return;
+  const BfsScratchLayout l = bfsScratchLayout(n);
+  const size_t cells = l.counters + GB_BFS_CELL_LEVELS*sizeof(unsigned long long);
+  if (desc->scratchSize(GB_SCRATCH_BFS) < cells + 6*sizeof(unsigned long long)) return;
   unsigned char* base = reinterpret_cast<unsigned char*>(desc->scratch(GB_SCRATCH_BFS, 0));
-  CUDA_CALL(cudaMemcpyAsync(out, base + 4*words_bytes + 6*sizeof(unsigned long long),
-      6*sizeof(unsigned long long), cudaMemcpyDeviceToHost, gbStream()));
+  CUDA_CALL(cudaMemcpyAsync(out, base + cells, 6*sizeof(unsigned long long),
+      cudaMemcpyDeviceToHost, gbStream()));
   runtime().sync();
 }
 
@@ -54,17 +92,9 @@ Info bfsFused(Vector<float>* v, const Matrix<a>* A, Index s, Descriptor* desc, i
   const int fw = 1;                                   // vxm pulls over the CSC
   const Index* probe = pullMaxDegreeNeighbours(S, fw, S->d_cscColPtr_, S->d_cscRowInd_, n);
 
-  const size_t nwords = (static_cast<size_t>(n) + 31)/32;
-  const size_t words_bytes = ((nwords*sizeof(unsigned int) + 255)/256)*256;
-  const size_t nchunks = (nwords + 31)/32;
-  const size_t counters_bytes = GB_BFS_NCOUNTERS*sizeof(unsigned long long);
-  const size_t heavy_bytes = GB_BFS_HEAVY_CAP*sizeof(Index);
-  const size_t walk_bytes = nchunks*GB_BFS_CHUNK*sizeof(Index);
-  const size_t lists_bytes = ((nchunks*(sizeof(int) + sizeof(Index)) + 255)/256)*256;
-  const size_t level8_bytes = ((static_cast<size_t>(n) + 255)/256)*256;
-  unsigned char* base = reinterpret_cast<unsigned char*>(desc->scratch(GB_SCRATCH_BFS,
-      4*words_bytes + counters_bytes + heavy_bytes + walk_bytes + lists_bytes +
-      level8_bytes));
+  const BfsScratchLayout l = bfsScratchLayout(n);
+  unsigned char* base =
+      reinterpret_cast<unsigned char*>(desc->scratch(GB_SCRATCH_BFS, l.bytes));
   BfsFusedArgs args;
   args.push_ptr = S->d_csrRowPtr_;  args.push_ind = S->d_csrColInd_;
   args.pull_ptr = S->d_cscColPtr_;  args.pull_ind = S->d_cscRowInd_;
@@ -85,23 +115,19 @@ Info bfsFused(Vector<float>* v, const Matrix<a>* A, Index s, Descriptor* desc, i
   CHECK(desc->get(GrB_MXVMODE, &mode));
   args.mode = (mode == GrB_PUSHONLY) ? 1 : (mode == GrB_PULLONLY ? 2 : 0);
   args.levels = v->dense_.d_val_;
-  args.visited[0] = reinterpret_cast<unsigned int*>(base);
-  args.visited[1] = reinterpret_cast<unsigned int*>(base + words_bytes);
-  args.frontier   = reinterpret_cast<unsigned int*>(base + 2*words_bytes);
-  args.next       = reinterpret_cast<unsigned int*>(base + 3*words_bytes);
-  args.counters   = reinterpret_cast<unsigned long long*>(base + 4*words_bytes);
-  args.heavy      = reinterpret_cast<Index*>(base + 4*words_bytes + counters_bytes);
-  args.walk       = reinterpret_cast<Index*>(base + 4*words_bytes + counters_bytes +
-                                             heavy_bytes);
-  args.walk_count = reinterpret_cast<int*>(base + 4*words_bytes + counters_bytes +
-                                           heavy_bytes + walk_bytes);
-  args.walk_chunks = reinterpret_cast<Index*>(args.walk_count + nchunks);
+  args.visited[0]  = reinterpret_cast<unsigned int*>(base + l.visited[0]);
+  args.visited[1]  = reinterpret_cast<unsigned int*>(base + l.visited[1]);
+  args.frontier    = reinterpret_cast<unsigned int*>(base + l.frontier);
+  args.next        = reinterpret_cast<unsigned int*>(base + l.next);
+  args.counters    = reinterpret_cast<unsigned long long*>(base + l.counters);
+  args.heavy       = reinterpret_cast<Index*>(base + l.heavy);
+  args.walk        = reinterpret_cast<Index*>(base + l.walk);
+  args.walk_count  = reinterpret_cast<int*>(base + l.walk_count);
+  args.walk_chunks = reinterpret_cast<Index*>(base + l.walk_chunks);
   // no fill: the kernel reads the byte of a row only when it wrote it in this traversal
-  args.level8     = base + 4*words_bytes + counters_bytes + heavy_bytes + walk_bytes +
-                    lists_bytes;
+  args.level8      = base + l.level8;
 
-  static const int trace = getEnv("GB200_BFS_TRACE", 0);
-  args.trace = trace;
+  args.trace = bfsTrace();
   args.prof_bytes = NULL;               // the kernel adds its bytes when profiling
   if (profiler().enabled) {
     profiler().ensureCells();
@@ -115,44 +141,47 @@ Info bfsFused(Vector<float>* v, const Matrix<a>* A, Index s, Descriptor* desc, i
       push_only ? bfsFusedKernel<GB_BFS_PUSH_NT, GB_BFS_PUSH_MINB, false>
                 : bfsFusedKernel<GB_BFS_NT, GB_BFS_MINB, true>;
   const int nt = push_only ? GB_BFS_PUSH_NT : GB_BFS_NT;
-  static int resident_of[2] = {0, 0};    // CTAs that fit at once (cooperative launch)
-  int& resident = resident_of[push_only ? 1 : 0];
-  if (resident == 0) {
-    int per_sm = 0;
-    CUDA_CALL(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, nt, 0));
-    resident = per_sm*runtime().sm_count;
-    if (resident < 1) return GrB_PANIC;
-  }
+  const int grid = push_only
+      ? cooperativeGrid<bfsFusedKernel<GB_BFS_PUSH_NT, GB_BFS_PUSH_MINB, false>,
+                        GB_BFS_PUSH_NT>()
+      : cooperativeGrid<bfsFusedKernel<GB_BFS_NT, GB_BFS_MINB, true>, GB_BFS_NT>();
+  if (grid < 1) return GrB_PANIC;
   void* params[] = { &args };
   profiler().begin(GB_PROF_PULL_BOOL, stream);
   CUDA_CALL(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kernel),
-      dim3(resident), dim3(nt), params, 0, stream));
+      dim3(grid), dim3(nt), params, 0, stream));
   GB_KERNEL_CHECK();
   profiler().end(GB_PROF_PULL_BOOL, stream, 0.0);
   v->dense_.touched();
-  if (trace) {                           // per-level times of this traversal
+  if (args.trace) {                      // per-level times of this traversal
     unsigned long long cells[GB_BFS_NCOUNTERS];
     CUDA_CALL(cudaMemcpyAsync(cells, args.counters, sizeof(cells), cudaMemcpyDeviceToHost,
         stream));
     runtime().sync();
-    const int levels = static_cast<int>(cells[6] < 15 ? cells[6] : 15);
+    const unsigned long long* const clock = cells + GB_BFS_CELL_LEVEL_CLOCK;
+    const int levels = static_cast<int>(
+        cells[GB_BFS_CELL_LEVELS] < GB_BFS_TIMED_LEVELS - 1 ? cells[GB_BFS_CELL_LEVELS]
+                                                            : GB_BFS_TIMED_LEVELS - 1);
     fprintf(stderr, "bfs trace: set-up %.1fus",
-            1e-3*static_cast<double>((cells[12] >> 1) - cells[28]));
+            1e-3*static_cast<double>((clock[0] >> 1) - cells[GB_BFS_CELL_START_CLOCK]));
     for (int l = 1; l <= levels; ++l) {
-      const unsigned long long start = cells[12 + l - 1] >> 1, end = cells[12 + l] >> 1;
-      if (cells[12 + l] & 1ull)          // pull: scan, walk, rows walked, chunks listed
+      const unsigned long long start = clock[l - 1] >> 1, end = clock[l] >> 1;
+      const unsigned long long scan = cells[GB_BFS_CELL_SCAN_CLOCK + l];
+      if (clock[l] & 1ull)               // pull: scan, walk, rows walked, chunks listed
         fprintf(stderr, " L%d pull %.1fus (scan %.1f walk %.1f, %llu walked, %llu listed)",
                 l, 1e-3*static_cast<double>(end - start),
-                1e-3*static_cast<double>(cells[44 + l] - start),
-                1e-3*static_cast<double>(end - cells[44 + l]), cells[60 + l],
-                cells[76 + l]);
+                1e-3*static_cast<double>(scan - start),
+                1e-3*static_cast<double>(end - scan), cells[GB_BFS_CELL_WALKED + l],
+                cells[GB_BFS_CELL_LISTED_CHUNKS + l]);
       else
         fprintf(stderr, " L%d push %.1fus", l, 1e-3*static_cast<double>(end - start));
     }
-    fprintf(stderr, " end-pass %.1fus\n", 1e-3*static_cast<double>(cells[29] - cells[30]));
+    fprintf(stderr, " end-pass %.1fus\n",
+            1e-3*static_cast<double>(cells[GB_BFS_CELL_END_PASS_CLOCK] -
+                                     cells[GB_BFS_CELL_LAST_LEVEL_CLOCK]));
   }
   if (depth != NULL) {
-    const unsigned long long levels = runtime().fetch(args.counters + 6);
+    const unsigned long long levels = runtime().fetch(args.counters + GB_BFS_CELL_LEVELS);
     *depth = static_cast<int>(levels);
     desc->lastmxv_ = GrB_PULLONLY;
   }

@@ -117,30 +117,63 @@ struct BfsFusedArgs {
   unsigned int* visited[2];
   unsigned int* frontier;    // F
   unsigned int* next;        // N
-  // small cells
-  unsigned long long* counters;   // [0..2] next-frontier size, [3..5] heavy-list length
-                                  // (both rotate with level % 3: the cell of level L
-                                  // is zeroed during level L-1, filled during L and
-                                  // read after L's barrier, when slow threads may still
-                                  // be reading the cell of L-1),
-                                  // [6] levels executed, [7..11] work counters (out),
-                                  // [12..27] time at the end of the set-up and of every
-                                  // level (ns << 1 | pulled), [28] time at the start,
-                                  // [29] at the end of the pass that writes v, [30]
-                                  // at the end of the last level,
-                                  // [35..37] walk-chunk claim counters of the pull
-                                  // levels, [38..40] chunks listed in walk_chunks
-                                  // (both rotating like [0..2]),
-                                  // [44..59] time at the scan barrier of every pull
-                                  // level, [60..75] rows it left to walk (inline and
-                                  // listed), [76..91] chunks it listed; [12..] and
-                                  // [44..] for GB200_BFS_TRACE (GB_BFS_NCOUNTERS cells)
+  // small cells, indexed by BfsCell
+  unsigned long long* counters;   // [GB_BFS_NCOUNTERS]
   Index*        heavy;            // [GB_BFS_HEAVY_CAP]
   Index*        walk;             // [nchunks * GB_BFS_CHUNK] rows to walk, by chunk
   int*          walk_count;       // [nchunks] rows to walk per chunk
   Index*        walk_chunks;      // [nchunks] the chunks with rows to walk, listed
 };
-#define GB_BFS_NCOUNTERS 128
+
+// Levels whose clocks and trace counts have a cell: levels 0..15.
+#define GB_BFS_TIMED_LEVELS 16
+
+// The cells of BfsFusedArgs::counters.  A rotating cell is a triple used by level L
+// as cell L % 3 (bfsLevelCell): it is zeroed during level L-1, filled during L and
+// read after L's barrier, when slow threads may still be reading the cell of L-1.
+// Clocks are %globaltimer nanoseconds.
+enum BfsCell {
+  // zeroed at the start of a traversal
+  GB_BFS_CELL_FOUND = 0,                              // rotating: next-frontier size
+  GB_BFS_CELL_HEAVY = GB_BFS_CELL_FOUND + 3,          // rotating: heavy-list length
+  // results, read by bfsFusedStats in this order
+  GB_BFS_CELL_LEVELS = GB_BFS_CELL_HEAVY + 3,         // levels executed
+  GB_BFS_CELL_INSPECTED,                              // entries inspected pulling
+  GB_BFS_CELL_PULL_LEVELS,                            // pull levels
+  GB_BFS_CELL_PUSHED_VERTICES,                        // vertices pushed
+  GB_BFS_CELL_PUSHED_EDGES,                           // edges pushed
+  GB_BFS_CELL_FOUND_PUSHING,                          // vertices discovered pushing
+  // clocks
+  GB_BFS_CELL_LEVEL_CLOCK,                            // per level: end of the set-up
+                                                      // (0) and of every level, ns << 1
+                                                      // | pulled
+  GB_BFS_CELL_START_CLOCK = GB_BFS_CELL_LEVEL_CLOCK + GB_BFS_TIMED_LEVELS,
+  GB_BFS_CELL_END_PASS_CLOCK,                         // end of the pass that writes v
+                                                      // (GB200_BFS_TRACE only)
+  GB_BFS_CELL_LAST_LEVEL_CLOCK,                       // end of the last level
+  // pull levels, zeroed at the start of a traversal
+  GB_BFS_CELL_WALK_CLAIM = 35,                        // rotating: walk-chunk claims
+  GB_BFS_CELL_LISTED = GB_BFS_CELL_WALK_CLAIM + 3,    // rotating: chunks in walk_chunks
+  GB_BFS_CELL_SCAN_CLOCK = 44,                        // per level: the scan barrier
+  // per level, GB200_BFS_TRACE only: rows the scan left to walk (inline and listed,
+  // zeroed at the start of a traversal) and chunks it listed
+  GB_BFS_CELL_WALKED = GB_BFS_CELL_SCAN_CLOCK + GB_BFS_TIMED_LEVELS,
+  GB_BFS_CELL_LISTED_CHUNKS = GB_BFS_CELL_WALKED + GB_BFS_TIMED_LEVELS,
+  GB_BFS_NCOUNTERS = 128
+};
+static_assert(GB_BFS_CELL_LISTED_CHUNKS + GB_BFS_TIMED_LEVELS <= GB_BFS_NCOUNTERS,
+              "the per-level cells of the last timed level are past the counters");
+
+// Level's cell of the rotating triple that starts at cell `first`, and the next
+// level's, zeroed.
+__device__ __forceinline__ unsigned long long* bfsLevelCell(unsigned long long* cells,
+                                                            int first, int level) {
+  return cells + first + level % 3;
+}
+__device__ __forceinline__ void bfsZeroNextCell(unsigned long long* cells, int first,
+                                                int level) {
+  cells[first + (level + 1) % 3] = 0ull;
+}
 
 __device__ __forceinline__ unsigned long long bfsClockNs() {
   unsigned long long t;
@@ -148,7 +181,10 @@ __device__ __forceinline__ unsigned long long bfsClockNs() {
   return t;
 }
 
-__device__ __forceinline__ bool bfsClaim(unsigned int* visited, Index vtx) {
+// Sets vertex vtx's bit in visited; true for the one thread that set it.  V: the
+// vertex-id type (Index, or long long for the global ids of the multi-GPU kernel).
+template <typename V>
+__device__ __forceinline__ bool bfsClaim(unsigned int* visited, V vtx) {
   const unsigned int bit = 1u << (vtx & 31);
   unsigned int* word = visited + (vtx >> 5);
   if (*reinterpret_cast<volatile unsigned int*>(word) & bit) return false;
@@ -284,7 +320,7 @@ bfsFusedKernel(BfsFusedArgs a) {
   const Index gwarps = gthreads >> 5;
   const Index nchunks = (nwords + 31) >> 5;               // pull chunks of 32 words
 
-  if (gtid == 0) a.counters[28] = bfsClockNs();
+  if (gtid == 0) a.counters[GB_BFS_CELL_START_CLOCK] = bfsClockNs();
   // ---- level 0: clear the bitmaps, seed the source (v is written once per row, after
   // the last level) ---------------------------------------------------------------------
   if (gtid == 0) a.level8[a.source] = 1;
@@ -295,11 +331,12 @@ bfsFusedKernel(BfsFusedArgs a) {
     a.visited[0][w] = seed | bfsIsolated(a, w);
     a.visited[1][w] = 0u; a.frontier[w] = seed; a.next[w] = 0u;
   }
-  if (gtid < 12) a.counters[gtid] = 0ull;
-  if (gtid >= 35 && gtid < 41) a.counters[gtid] = 0ull;
-  if (gtid >= 60 && gtid < 76) a.counters[gtid] = 0ull;
+  if (gtid <= GB_BFS_CELL_FOUND_PUSHING) a.counters[gtid] = 0ull;
+  if (gtid >= GB_BFS_CELL_WALK_CLAIM && gtid < GB_BFS_CELL_LISTED + 3) a.counters[gtid] = 0ull;
+  if (gtid >= GB_BFS_CELL_WALKED && gtid < GB_BFS_CELL_WALKED + GB_BFS_TIMED_LEVELS)
+    a.counters[gtid] = 0ull;
   grid.sync();
-  if (gtid == 0) a.counters[12] = bfsClockNs() << 1;          // [12..27]: level clock
+  if (gtid == 0) a.counters[GB_BFS_CELL_LEVEL_CLOCK] = bfsClockNs() << 1;
 
   int vsel = 0;                           // bfsVis / bfsVisOther
   int fsel = 0;                           // bfsF / bfsN
@@ -323,13 +360,13 @@ bfsFusedKernel(BfsFusedArgs a) {
         if (ratio <= a.switchpoint && ratio < prev_ratio) dense = false; else prev_ratio = ratio;
       }
     }
-    unsigned long long* const count_cell = a.counters + (level % 3);
-    unsigned long long* const heavy_cell = a.counters + 3 + (level % 3);
-    if (gtid == 0) {                        // next level's cells
-      a.counters[(level + 1) % 3] = 0ull;
-      a.counters[3 + (level + 1) % 3] = 0ull;
-      a.counters[35 + (level + 1) % 3] = 0ull;
-      a.counters[38 + (level + 1) % 3] = 0ull;
+    unsigned long long* const count_cell = bfsLevelCell(a.counters, GB_BFS_CELL_FOUND, level);
+    unsigned long long* const heavy_cell = bfsLevelCell(a.counters, GB_BFS_CELL_HEAVY, level);
+    if (gtid == 0) {
+      bfsZeroNextCell(a.counters, GB_BFS_CELL_FOUND, level);
+      bfsZeroNextCell(a.counters, GB_BFS_CELL_HEAVY, level);
+      bfsZeroNextCell(a.counters, GB_BFS_CELL_WALK_CLAIM, level);
+      bfsZeroNextCell(a.counters, GB_BFS_CELL_LISTED, level);
     }
     int found_here = 0;
 
@@ -400,8 +437,9 @@ bfsFusedKernel(BfsFusedArgs a) {
     } else if (PULL) {
       ++pull_levels;
       // ---------------- pull: every unvisited row looks for a visited neighbour ----
-      unsigned long long* const walk_cell = a.counters + 35 + (level % 3);
-      unsigned long long* const list_cell = a.counters + 38 + (level % 3);
+      unsigned long long* const walk_cell =
+          bfsLevelCell(a.counters, GB_BFS_CELL_WALK_CLAIM, level);
+      unsigned long long* const list_cell = bfsLevelCell(a.counters, GB_BFS_CELL_LISTED, level);
       // scan: a lane per bitmap word of the chunk, chunks dealt round-robin (the
       // grid has ~4 chunks per warp at RMAT-24 and they cost about the same); the
       // next chunk's words are requested before this one is worked on
@@ -583,17 +621,19 @@ bfsFusedKernel(BfsFusedArgs a) {
             a.walk_count[c] = nwalk;
             a.walk_chunks[atomicAdd(list_cell, 1ull)] = c;
           }
-          if (a.trace && level < 16)
-            atomicAdd(a.counters + 60 + level, static_cast<unsigned long long>(nwalk));
+          if (a.trace && level < GB_BFS_TIMED_LEVELS)
+            atomicAdd(a.counters + GB_BFS_CELL_WALKED + level,
+                      static_cast<unsigned long long>(nwalk));
         }
         c = c_next;
       }
       grid.sync();
       const Index nlisted = static_cast<Index>(
           *reinterpret_cast<volatile unsigned long long*>(list_cell));
-      if (gtid == 0 && level < 16) {
-        a.counters[44 + level] = bfsClockNs();
-        if (a.trace) a.counters[76 + level] = static_cast<unsigned long long>(nlisted);
+      if (gtid == 0 && level < GB_BFS_TIMED_LEVELS) {
+        a.counters[GB_BFS_CELL_SCAN_CLOCK + level] = bfsClockNs();
+        if (a.trace)
+          a.counters[GB_BFS_CELL_LISTED_CHUNKS + level] = static_cast<unsigned long long>(nlisted);
       }
       // walk: the heavy chunks' rows, chunks claimed from a counter, a lane per row
       for (Index i = gwarp; i < nlisted; ) {
@@ -618,18 +658,19 @@ bfsFusedKernel(BfsFusedArgs a) {
     const int block_found = blockSum<NT>(found_here, s_red);
     if (threadIdx.x == 0 && block_found) {
       atomicAdd(count_cell, static_cast<unsigned long long>(block_found));
-      if (!dense)                           // [11] vertices discovered pushing
-        atomicAdd(a.counters + 11, static_cast<unsigned long long>(block_found));
+      if (!dense)
+        atomicAdd(a.counters + GB_BFS_CELL_FOUND_PUSHING,
+                  static_cast<unsigned long long>(block_found));
     }
     grid.sync();
-    if (gtid == 0 && level < 16)
-      a.counters[12 + level] = (bfsClockNs() << 1) | (dense ? 1ull : 0ull);
+    if (gtid == 0 && level < GB_BFS_TIMED_LEVELS)
+      a.counters[GB_BFS_CELL_LEVEL_CLOCK + level] = (bfsClockNs() << 1) | (dense ? 1ull : 0ull);
     fcount = static_cast<unsigned int>(
         *reinterpret_cast<volatile unsigned long long*>(count_cell));
     if (dense) vsel ^= 1;
     fsel ^= 1;
   }
-  if (gtid == 0) a.counters[30] = bfsClockNs();   // [30]: the end of the last level
+  if (gtid == 0) a.counters[GB_BFS_CELL_LAST_LEVEL_CLOCK] = bfsClockNs();
   // ---- v, every row once, in full lines ----------------------------------------
   // A row is reached when it is visited now and not only because nothing points at
   // it (the source is reached).  A traversal cut off after max_levels (the frontier
@@ -689,31 +730,35 @@ bfsFusedKernel(BfsFusedArgs a) {
       }
     }
   }
-  if (a.trace) {                          // [29]: the end of the pass above
+  if (a.trace) {
     grid.sync();
-    if (gtid == 0) a.counters[29] = bfsClockNs();
+    if (gtid == 0) a.counters[GB_BFS_CELL_END_PASS_CLOCK] = bfsClockNs();
   }
-  // ---- results -----------------------------------------------------------------
-  // [7] entries inspected pulling, [8] pull levels, [9] vertices pushed, [10] edges
-  // pushed, [11] vertices discovered pushing — the algorithmic bytes of SURVEY.md §8d
+  // ---- results: the work counters, the algorithmic bytes of SURVEY.md §8d --------
   const int block_insp = blockSum<NT>(inspected, s_red);
   const int block_pv = blockSum<NT>(pushed_vertices, s_red);
   if (threadIdx.x == 0) {
-    if (block_insp) atomicAdd(a.counters + 7, static_cast<unsigned long long>(block_insp));
-    if (block_pv)   atomicAdd(a.counters + 9, static_cast<unsigned long long>(block_pv));
+    if (block_insp)
+      atomicAdd(a.counters + GB_BFS_CELL_INSPECTED, static_cast<unsigned long long>(block_insp));
+    if (block_pv)
+      atomicAdd(a.counters + GB_BFS_CELL_PUSHED_VERTICES,
+                static_cast<unsigned long long>(block_pv));
   }
-  if (pushed_edges) atomicAdd(a.counters + 10, static_cast<unsigned long long>(pushed_edges));
+  if (pushed_edges)
+    atomicAdd(a.counters + GB_BFS_CELL_PUSHED_EDGES,
+              static_cast<unsigned long long>(pushed_edges));
   if (gtid == 0) {
-    a.counters[6] = static_cast<unsigned long long>(level - 1);
-    a.counters[8] = static_cast<unsigned long long>(pull_levels);
+    a.counters[GB_BFS_CELL_LEVELS] = static_cast<unsigned long long>(level - 1);
+    a.counters[GB_BFS_CELL_PULL_LEVELS] = static_cast<unsigned long long>(pull_levels);
   }
   if (a.prof_bytes != NULL) {
     // The traversal's algorithmic bytes (SURVEY.md §8d): per pull level 4(n+1) + 4n
     // + 4n, 4 per inspected entry; per push 12 per frontier entry, 8 per expanded
     // edge (colind + visited lookup), 8 per discovered vertex.  The sum is linear in
     // the work counters, so every CTA adds its own share and CTA 0 the per-level
-    // terms ([11] is complete: the last level ended with a grid barrier).  A last-CTA
-    // ticket would need a device-scope fence, and with one in the kernel ptxas turns
+    // terms (the count of vertices discovered pushing is complete: the last level
+    // ended with a grid barrier).  A last-CTA ticket would need a device-scope
+    // fence, and with one in the kernel ptxas turns
     // every fire-and-forget reduction (REDG) into an atomic that waits (ATOMG),
     // the push levels' visited and next-frontier ORs included: push-only BFS
     // 156.7-157.5 ms per launch against 149.7-150.7 (DESIGN.md §9).
@@ -724,7 +769,8 @@ bfsFusedKernel(BfsFusedArgs a) {
       if (blockIdx.x == 0)
         bytes += static_cast<unsigned long long>(pull_levels)*
                      (12ull*static_cast<unsigned long long>(n) + 4ull) +
-                 8ull*(*reinterpret_cast<volatile unsigned long long*>(a.counters + 11));
+                 8ull*(*reinterpret_cast<volatile unsigned long long*>(
+                           a.counters + GB_BFS_CELL_FOUND_PUSHING));
       if (bytes) atomicAdd(a.prof_bytes, bytes);
     }
   }

@@ -5,8 +5,8 @@
 //   succ = reduce(+, f1) ; stop when succ == 0.
 // With the flags of the reference's benchmark script (run_bfs.sh:8-27) that whole
 // loop runs as ONE cooperative kernel (backend/cuda/bfs_fused.hpp): same levels,
-// no launch or host round trip per level.  GB200_BFS_FUSED=0, --timing 1 or any
-// other flag combination takes the operation-by-operation loop below.
+// no launch or host round trip per level.  --timing 1 or any other flag
+// combination takes the operation-by-operation loop below.
 // Output convention: level of the source is 1, unreached vertices stay 0.
 // Returns the device time of the loop in milliseconds ("tight" in the reference
 // drivers), excluding the initial fill of v.  With timed = false the fused
