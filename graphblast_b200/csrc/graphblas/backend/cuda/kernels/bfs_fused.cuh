@@ -485,7 +485,9 @@ bfsFusedKernel(BfsFusedArgs a) {
           __syncwarp();
           for (int r0 = 0; r0 < total; r0 += 32*GB_BFS_BATCH) {
             // GB_BFS_BATCH rounds of 32 open rows: all summary loads, then all
-            // probes, then the decisions
+            // probes, then the decisions.  The summary is read once per level, so
+            // its loads bypass L1 (ldStream32) and leave it to the probes' bitmap
+            // lines (DESIGN.md §4.5)
             int local[GB_BFS_BATCH];          // offset of the row in the chunk
             Index f[GB_BFS_BATCH];
 #pragma unroll
@@ -505,7 +507,7 @@ bfsFusedKernel(BfsFusedArgs a) {
                 if (k >= lo) { k -= lo; b += width; m >>= width; }
               }
               local[j] = wl*32 + b;
-              f[j] = (r < total) ? __ldg(a.pull_probe + c*GB_BFS_CHUNK + local[j])
+              f[j] = (r < total) ? ldStream32(a.pull_probe + c*GB_BFS_CHUNK + local[j])
                                  : static_cast<Index>(-1);
             }
             unsigned int pword[GB_BFS_BATCH];
@@ -538,8 +540,8 @@ bfsFusedKernel(BfsFusedArgs a) {
           my_out = found_bits[lane];
         }
         while (open != 0u) {
-          // up to GB_BFS_BATCH open words: all summary loads, then all probes, then
-          // the decisions
+          // up to GB_BFS_BATCH open words: all summary loads (bypassing L1, as on
+          // the row path), then all probes, then the decisions
           const unsigned int batch = open;
           Index f[GB_BFS_BATCH];
 #pragma unroll
@@ -550,7 +552,7 @@ bfsFusedKernel(BfsFusedArgs a) {
             if (wl >= 0) {
               const unsigned int m = __shfl_sync(GB_FULL_MASK, my_vis, wl);
               const Index row = c*GB_BFS_CHUNK + wl*32 + lane;
-              if (row < n && !((m >> lane) & 1u)) f[j] = __ldg(a.pull_probe + row);
+              if (row < n && !((m >> lane) & 1u)) f[j] = ldStream32(a.pull_probe + row);
             }
           }
           unsigned int pword[GB_BFS_BATCH];
@@ -687,45 +689,118 @@ bfsFusedKernel(BfsFusedArgs a) {
   // are written row by row.  The loop counts blocks of 16 words, not rows, so that
   // stepping past the last block cannot overflow (rows stay below n + 512, as the
   // pull scan's stay below n + 1024).  The 4-byte load also takes the bytes of rows
-  // not reached, which this traversal never wrote; their values are not used.
+  // not reached, which this traversal never wrote; their values are not used.  The
+  // 16-byte stores are streaming (st.global.cs, evict-first): nothing reads the 4n
+  // bytes of v again in the kernel, and marked so they do not push the level bytes
+  // and bitmaps the pass still reads out of L2.
   const Index nblocks = (nwords + 15) >> 4;
-  for (Index blk = gwarp; blk < nblocks; blk += gwarps) {
-    const Index r0 = blk*512;
-    const Index w = blk*16 + (lane & 15);
-    unsigned int reached = 0u;
-    if (lane < 16 && w < nwords) {
-      reached = bfsVis(a, vsel)[w] & ~bfsIsolated(a, w);
-      if (cut_rows != NULL) reached &= ~cut_rows[w];
-      if (w == (a.source >> 5)) reached |= 1u << (a.source & 31);
-    }
+  if (PULL) {
+    // The loads of a block go out before the stores of the block before it: the warp
+    // requests block blk + gwarps's reach masks and level bytes, then stores block
+    // blk's floats, so the loads' latency sits under the stores instead of between
+    // one block's stores and the next (RMAT-24: end pass 36-38 -> 30-32 us, DESIGN.md
+    // §6).  A block past the last loads nothing, and a group of 4 rows gets its
+    // 4-byte load only when it can be stored as a line.  Not in the push-only
+    // instantiation: the 5 more live registers spill there at 768 x 2.  The two
+    // loops share no lambda: one gave the pull instantiation another register
+    // allocation throughout and a slower scan (DESIGN.md §4.5).
+    auto load_block = [&](Index blk, unsigned int& reached, unsigned int (&b)[4]) {
+      reached = 0u;
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const unsigned int bits =
-          (__shfl_sync(GB_FULL_MASK, reached, 4*j + (lane >> 3)) >> (4*(lane & 7))) & 0xfu;
-      const Index row = r0 + 128*j + 4*lane;
-      if (row >= n) continue;
-      if (lines && row + 4 <= n) {
-        const unsigned int b = *reinterpret_cast<const unsigned int*>(a.level8 + row);
-        float f[4];
-        bool escape = false;
+      for (int j = 0; j < 4; ++j) b[j] = 0u;
+      if (blk >= nblocks) return;
+      const Index w = blk*16 + (lane & 15);
+      if (lane < 16 && w < nwords) {
+        reached = bfsVis(a, vsel)[w] & ~bfsIsolated(a, w);
+        if (cut_rows != NULL) reached &= ~cut_rows[w];
+        if (w == (a.source >> 5)) reached |= 1u << (a.source & 31);
+      }
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const unsigned int byte = (b >> (8*k)) & 0xffu;
-          const bool r = (bits >> k) & 1u;
-          escape |= r && byte == 255u;
-          f[k] = r ? static_cast<float>(byte) : 0.f;
+      for (int j = 0; j < 4; ++j) {
+        const Index row = blk*512 + 128*j + 4*lane;
+        if (lines && row + 4 <= n) b[j] = *reinterpret_cast<const unsigned int*>(a.level8 + row);
+      }
+    };
+    unsigned int next_reached, next_b[4];
+    load_block(gwarp, next_reached, next_b);
+    for (Index blk = gwarp; blk < nblocks; blk += gwarps) {
+      const Index r0 = blk*512;
+      const unsigned int reached = next_reached;
+      unsigned int lb[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) lb[j] = next_b[j];
+      load_block(blk + gwarps, next_reached, next_b);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const unsigned int bits =
+            (__shfl_sync(GB_FULL_MASK, reached, 4*j + (lane >> 3)) >> (4*(lane & 7))) & 0xfu;
+        const Index row = r0 + 128*j + 4*lane;
+        if (row >= n) continue;
+        if (lines && row + 4 <= n) {
+          const unsigned int b = lb[j];
+          float f[4];
+          bool escape = false;
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const unsigned int byte = (b >> (8*k)) & 0xffu;
+            const bool r = (bits >> k) & 1u;
+            escape |= r && byte == 255u;
+            f[k] = r ? static_cast<float>(byte) : 0.f;
+          }
+          if (!escape) {
+            __stcs(reinterpret_cast<float4*>(a.levels + row), make_float4(f[0], f[1], f[2], f[3]));
+            continue;
+          }
         }
-        if (!escape) {
-          *reinterpret_cast<float4*>(a.levels + row) = make_float4(f[0], f[1], f[2], f[3]);
-          continue;
+        for (int k = 0; k < 4 && row + k < n; ++k) {
+          if (!((bits >> k) & 1u)) {
+            a.levels[row + k] = 0.f;
+          } else {
+            const unsigned int byte = a.level8[row + k];
+            if (byte != 255u) a.levels[row + k] = static_cast<float>(byte);
+          }
         }
       }
-      for (int k = 0; k < 4 && row + k < n; ++k) {
-        if (!((bits >> k) & 1u)) {
-          a.levels[row + k] = 0.f;
-        } else {
-          const unsigned int byte = a.level8[row + k];
-          if (byte != 255u) a.levels[row + k] = static_cast<float>(byte);
+    }
+  } else {
+    for (Index blk = gwarp; blk < nblocks; blk += gwarps) {
+      const Index r0 = blk*512;
+      const Index w = blk*16 + (lane & 15);
+      unsigned int reached = 0u;
+      if (lane < 16 && w < nwords) {
+        reached = bfsVis(a, vsel)[w] & ~bfsIsolated(a, w);
+        if (cut_rows != NULL) reached &= ~cut_rows[w];
+        if (w == (a.source >> 5)) reached |= 1u << (a.source & 31);
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const unsigned int bits =
+            (__shfl_sync(GB_FULL_MASK, reached, 4*j + (lane >> 3)) >> (4*(lane & 7))) & 0xfu;
+        const Index row = r0 + 128*j + 4*lane;
+        if (row >= n) continue;
+        if (lines && row + 4 <= n) {
+          const unsigned int b = *reinterpret_cast<const unsigned int*>(a.level8 + row);
+          float f[4];
+          bool escape = false;
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const unsigned int byte = (b >> (8*k)) & 0xffu;
+            const bool r = (bits >> k) & 1u;
+            escape |= r && byte == 255u;
+            f[k] = r ? static_cast<float>(byte) : 0.f;
+          }
+          if (!escape) {
+            __stcs(reinterpret_cast<float4*>(a.levels + row), make_float4(f[0], f[1], f[2], f[3]));
+            continue;
+          }
+        }
+        for (int k = 0; k < 4 && row + k < n; ++k) {
+          if (!((bits >> k) & 1u)) {
+            a.levels[row + k] = 0.f;
+          } else {
+            const unsigned int byte = a.level8[row + k];
+            if (byte != 255u) a.levels[row + k] = static_cast<float>(byte);
+          }
         }
       }
     }

@@ -13,7 +13,11 @@ its entries from entry 0 up to and including the first visited one (all of them
 when none is).  Per pull level it gives the walk's shape: rows to walk per chunk of
 1024 rows (p50, p99, max), the entries those walks inspect, and the chunks and rows
 above GB_BFS_WALK_INLINE, which the kernel lists and walks grid-wide after the scan
-instead of in the warp that scanned them.
+instead of in the warp that scanned them.  And per pull level the floor of the
+scan's summary stream: every open word needs its 32 `pull_probe` entries, one
+128-byte line, so the scan reads at least 128 bytes per open word; those bytes
+over the H100 SXM data sheet's 3.35 TB/s of HBM3 bandwidth are a floor computed
+from the data sheet, not a measurement.
 
     python tools/bfs_pull_model.py [--scale 24] [--seed 1] [--mxvmode 0]
                                    [--walk-inline 64]
@@ -29,6 +33,8 @@ import numpy as np
 
 BLOCK = 1 << 21          # rows per block of the entry-wise passes (bounds memory)
 WALK_INLINE = 64         # GB_BFS_WALK_INLINE: a chunk with more rows to walk is listed
+LINE = 128               # bytes of the summary line of one bitmap word (32 entries)
+HBM_BYTES_PER_S = 3.35e12  # H100 SXM data sheet, HBM3
 
 
 def probe_summary(rp, ci, rule, lengths=None):
@@ -208,6 +214,11 @@ def main():
                   it["level"], it["walked_maxdeg"], it["walk_chunks"], p50, p99, top,
                   it["walk_entries"], it["walk_entries_row_max"], args.walk_inline,
                   it["listed_chunks"], it["listed_rows"]))
+    for it in iters:
+        nbytes = LINE*it["open_words"]
+        print("L%d summary floor: %d open words, %d bytes of pull_probe lines, "
+              "%.1f us at the data sheet's 3.35 TB/s (not a measurement)" % (
+                  it["level"], it["open_words"], nbytes, 1e6*nbytes/HBM_BYTES_PER_S))
     print("entries inspected pulling (maxdeg probe, walk from entry 0): %d"
           % inspected["maxdeg"])
 
