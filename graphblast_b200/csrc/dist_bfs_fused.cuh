@@ -3,8 +3,9 @@
 // over NVLink peer memory and the cross-GPU level barrier all run on the device.
 // Included by capi.cu after dist_exchange.cuh, whose exchange block it uses:
 //   data[2][total_words]  the replicated frontier bitmap, double buffered by epoch
-//   flags2[world]         flags2[r] = (last epoch rank r has published << 32) | size of
-//                         the slice it published
+//   flags2[2][32]         flags2[e & 1][r] = (epoch e << 32) | size of the slice rank r
+//                         published in epoch e; by parity, like the data, since a rank
+//                         can post epoch e + 1 while another one's CTAs still read e
 //
 // A level loop on the host paid about 40 us of launches and host round trips per
 // level against 10..100 us of work, so two GPUs were slower than one.  Here a level is:
@@ -164,7 +165,10 @@ bfsFusedDistKernel(BfsDistArgs a) {
       bfsZeroNextCell(a.cells, GBX_CELL_FOUND, level);
       bfsZeroNextCell(a.cells, GBX_CELL_HEAVY, level);
     }
-    const float next_level = static_cast<float>(level + 1);
+    // A traversal cut off after max_levels assigns levels 1..max_levels only, as
+    // the operation-by-operation loop and the single-GPU kernel do: the rows found
+    // at the last level keep 0.
+    const float next_level = (level < a.max_levels) ? static_cast<float>(level + 1) : 0.f;
     int found_here = 0;
     unsigned int* const vis = vis_copy[level & 1];     // as of the level's start
     GBX_TRACE(GBX_T_START);
@@ -285,7 +289,9 @@ bfsFusedDistKernel(BfsDistArgs a) {
     const unsigned long long epoch = a.epoch0 + static_cast<unsigned long long>(level);
     const int par = static_cast<int>(epoch & 1ull);
     const int vnext = (level + 1) & 1;
-    // 16-byte peer stores (slices start and end on multiples of 1024 vertices)
+    // 16-byte peer stores of the slice's whole groups of 4 words: word_lo is a
+    // multiple of 4 (slices start on multiples of 128 vertices, checked by the host
+    // entry), the last slice's < 4 remaining words are stored one by one below
     {
       uint4* const mine4 = reinterpret_cast<uint4*>(a.next_own);
       const uint4* const vis4 = reinterpret_cast<const uint4*>(vis + word_lo);
@@ -328,11 +334,11 @@ bfsFusedDistKernel(BfsDistArgs a) {
         const unsigned long long word = (epoch << 32) | (mine & 0xffffffffull);
         for (int p = 0; p < a.world; ++p)
           reinterpret_cast<volatile unsigned long long*>(
-              a.peers[p] + a.off_flags2)[a.rank] = word;
+              a.peers[p] + a.off_flags2)[par*32 + a.rank] = word;
       }
       GBX_TRACE(GBX_T_CHECKIN);
       const volatile unsigned long long* flags =
-          reinterpret_cast<const volatile unsigned long long*>(local + a.off_flags2);
+          reinterpret_cast<const volatile unsigned long long*>(local + a.off_flags2) + par*32;
       const long long t0 = clock64();
       bool ok = true;
       unsigned long long total = 0ull;
@@ -379,6 +385,8 @@ int gb200_dist_bfs_fused(gb200_xchg_t x, gb200_vector_t v, gb200_matrix_t M,
                          int* levels_out) {
   if (x == NULL || v == NULL || M == NULL || desc == NULL)
     return rc(graphblas::GrB_NULL_POINTER);
+  // the publish stores the owned slice as uint4 at word offset word_lo
+  if (x->word_off[x->rank] % 4 != 0) return rc(graphblas::GrB_INVALID_VALUE);
   if (!x->connected || M->f == NULL) return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
   GB200_REQUIRE_DEVICE();
   using namespace graphblas;              // NOLINT(build/namespaces)
@@ -388,6 +396,13 @@ int gb200_dist_bfs_fused(gb200_xchg_t x, gb200_vector_t v, gb200_matrix_t M,
   backend::Descriptor& d = desc->desc.descriptor_;
   Index nl;
   CHECK(v->f->size(&nl));
+  // v holds the owned vertices [32*word_lo, min(32*word_hi, n)), and the exchange's
+  // bitmap covers n vertices
+  const long long v_lo = 32ll*static_cast<long long>(x->word_off[x->rank]);
+  const long long v_hi = std::min(32ll*static_cast<long long>(x->word_off[x->rank + 1]), n);
+  if (x->total_words != static_cast<size_t>((n + 31)/32) ||
+      static_cast<long long>(nl) != v_hi - v_lo)
+    return rc(GrB_DIMENSION_MISMATCH);
   if (S.d_csrRowPtr_ == NULL || S.d_cscColPtr_ == NULL) return rc(GrB_UNINITIALIZED_OBJECT);
   CHECK(v->f->vector_.setStorage(GrB_DENSE));
   CHECK(v->f->vector_.dense_.allocateGpu());

@@ -178,6 +178,16 @@ int gb200_xchg_create(gb200_xchg_t* out, int world, int rank,
   if (out == NULL || word_offsets == NULL || world < 1 || world > 32 ||
       rank < 0 || rank >= world)
     return rc(graphblas::GrB_INVALID_VALUE);
+  // The ranks' slices cover the words from 0 and every rank owns at least one:
+  // words before the first slice would never be published, and a rank with an
+  // empty slice could not run the loops over it while the others waited for its
+  // publishes until the timeout.  Every rank sees the same offsets, so all of
+  // them refuse.
+  if (word_offsets[0] != 0)
+    return rc(graphblas::GrB_INVALID_VALUE);
+  for (int p = 0; p < world; ++p)
+    if (word_offsets[p + 1] <= word_offsets[p])
+      return rc(graphblas::GrB_INVALID_VALUE);
   GB200_REQUIRE_DEVICE();
   gb200_xchg_s* x = new gb200_xchg_s();
   x->world = world; x->rank = rank;
@@ -194,8 +204,10 @@ int gb200_xchg_create(gb200_xchg_t* out, int world, int rank,
   // owners store their slice of the NEXT level's copy into every rank
   for (int b = 0; b < 2; ++b) { x->off_visited[b] = off; off += data_bytes; }
   // flags of the fused kernel: one word per rank = (epoch << 32) | slice count, so
-  // the count needs no store + fence of its own
-  x->off_flags2 = off; off += 256;
+  // the count needs no store + fence of its own; two sets by epoch parity, so that
+  // a rank that has posted the next epoch cannot overwrite a count another rank's
+  // CTAs have still to read
+  x->off_flags2 = off; off += 2*256;
   x->bytes = off;
   CUDA_CALL(cudaMalloc(&x->local, x->bytes));
   CUDA_CALL(cudaMemset(x->local, 0, x->bytes));

@@ -166,22 +166,32 @@ def partition_bounds(rowptr, world, align=1024, row_weight=0.0):
     passes a row weight (GB200_DIST_ROW_WEIGHT; default 1e9 = equal vertex counts,
     measured best on R-MAT scale 24 at 2 GPUs: 0.464 ms entries-balanced, 0.428 at
     weight 32, 0.390 at 128, 0.385 with equal vertex counts).  rowptr: 1-D integer tensor/array of length n+1.  Returns a
-    list of world+1 ints."""
+    list of world+1 ints.
+
+    No slice is empty: a bound that would not pass the one before it (a row
+    heavier than 1/world of the cost) moves forward by `align`, and one that would
+    leave a later rank empty moves back, as far as needed to leave one block to
+    each later rank but the last and one vertex to the last.  A graph with fewer
+    than world * align vertices raises ValueError."""
     rp = rowptr if isinstance(rowptr, np.ndarray) else rowptr.cpu().numpy()
     n = len(rp) - 1
     assert align % 32 == 0
+    if n < world * align:
+        raise ValueError("partition_bounds: %d vertices cannot give each of %d ranks "
+                         "a slice of at least %d" % (n, world, align))
     cost = rp.astype(np.float64) + row_weight * np.arange(n + 1, dtype=np.float64)
     total = float(cost[-1])
     bounds = [0]
     for p in range(1, world):
         target = total * p / world
         v = int(np.searchsorted(cost, target, side="left"))
-        v = min(n, max(bounds[-1], (v + align // 2) // align * align))
-        bounds.append(v)
+        v = (v + align // 2) // align * align
+        # one block past the previous bound at least, one block left for each rank
+        # after this one but the last, one vertex for the last (n >= world * align
+        # keeps both possible)
+        last = (n - 1 - (world - p - 1) * align) // align * align
+        bounds.append(min(max(v, bounds[-1] + align), last))
     bounds.append(n)
-    for p in range(world):
-        if bounds[p + 1] < bounds[p]:
-            bounds[p + 1] = bounds[p]
     return bounds
 
 
@@ -208,6 +218,25 @@ def local_slice(rowptr, colind, lo, hi, n, return_order=False):
         return (rp_local, ci_local, colptr.to(torch.int32).contiguous(), rowind,
                 order)
     return rp_local, ci_local, colptr.to(torch.int32).contiguous(), rowind
+
+
+def pagerank_local_matrix(gb, n, rowptr, colind, lo, hi, alpha):
+    """(owned x n) CSR of the owned rows [lo, hi) of (alpha * A ./ outdeg)^T for a
+    structurally symmetric A: entry (i, j) = alpha / deg(j), what gb200_dist_pr
+    multiplies.  The matrix keeps its arrays alive."""
+    e0, e1 = int(rowptr[lo]), int(rowptr[hi])
+    rp_l = (rowptr[lo:hi + 1] - rowptr[lo]).to(torch.int32).contiguous()
+    ci_l = colind[e0:e1].contiguous()
+    deg = (rowptr[1:] - rowptr[:-1]).to(torch.float32)
+    val_l = (alpha / deg[ci_l.to(torch.int64)]).contiguous()
+    M = gb.Matrix(hi - lo, n)
+    M._keep = [rp_l, ci_l, val_l]
+    rc = gb._lib.load().gb200_matrix_adopt_csr(
+        M._h, C.c_void_p(rp_l.data_ptr()), C.c_void_p(ci_l.data_ptr()),
+        C.c_void_p(val_l.data_ptr()), int(ci_l.numel()))
+    if rc != 0:
+        raise RuntimeError("gb200_matrix_adopt_csr failed: %d" % rc)
+    return M
 
 
 def weighted_local_matrix(gb, n, rowptr, colind, cscval, lo, hi):
@@ -243,17 +272,25 @@ class PeerExchange(object):
     to agree that every rank connected."""
 
     def __init__(self, gb, bounds, device, bits):
-        """bounds: the vertex partition (world + 1 ints, multiples of 32 but the
-        last).  bits: the replicated array holds one bit per vertex (BFS) instead
-        of one 32-bit word (float payloads)."""
+        """bounds: the vertex partition (world + 1 increasing ints, multiples of 32
+        but the last; of 128 with bits, since the BFS kernel stores the owned
+        bitmap slice 16 bytes at a time).  bits: the replicated array holds one bit
+        per vertex (BFS) instead of one 32-bit word (float payloads)."""
         import torch.distributed as dist
-        self.lib = gb._lib.load()
+        self._h = C.c_void_p()
         self.world = len(bounds) - 1
+        unit = 128 if bits else 32
+        if any(b % unit for b in bounds[:-1]):
+            raise ValueError("PeerExchange: every bound but the last must be a multiple "
+                             "of %d vertices%s: %s" % (
+                                 unit, " for a bitmap exchange" if bits else "", bounds))
+        if any(bounds[p + 1] <= bounds[p] for p in range(self.world)):
+            raise ValueError("PeerExchange: every rank must own at least one vertex: %s"
+                             % bounds)
+        self.lib = gb._lib.load()
         self.rank = dist.get_rank() if self.world > 1 else 0
-        assert all(b % 32 == 0 for b in bounds[:-1])
         offsets = [(b + 31) // 32 for b in bounds] if bits else bounds
         offs = (C.c_longlong * (self.world + 1))(*[int(o) for o in offsets])
-        self._h = C.c_void_p()
         mine = (C.c_ubyte * 64)()
         why = None
         rc = self.lib.gb200_xchg_create(C.byref(self._h), self.world, self.rank,
@@ -375,19 +412,8 @@ def _setup_pr(gb, args, n, rowptr, colind, world, rank, dev):
     alpha, niter = 0.85, 10
     bounds = partition_bounds(rowptr, world)
     lo, hi = bounds[rank], bounds[rank + 1]
-    e0, e1 = int(rowptr[lo]), int(rowptr[hi])
-    rp_l = (rowptr[lo:hi + 1] - rowptr[lo]).to(torch.int32).contiguous()
-    ci_l = colind[e0:e1].contiguous()
-    # (alpha * A ./ outdeg)^T restricted to the owned rows: entry (i, j) = alpha/deg(j)
-    deg = (rowptr[1:] - rowptr[:-1]).to(torch.float32)
-    val_l = (alpha / deg[ci_l.to(torch.int64)]).contiguous()
-    M = gb.Matrix(max(hi - lo, 1), n)
-    M._keep = [rp_l, ci_l, val_l]
-    rc = gb._lib.load().gb200_matrix_adopt_csr(
-        M._h, C.c_void_p(rp_l.data_ptr()), C.c_void_p(ci_l.data_ptr()),
-        C.c_void_p(val_l.data_ptr()), int(ci_l.numel()))
-    assert rc == 0, rc
-    p_own = gb.Vector(max(hi - lo, 1))
+    M = pagerank_local_matrix(gb, n, rowptr, colind, lo, hi, alpha)
+    p_own = gb.Vector(hi - lo)
     desc = gb.Descriptor(mxvmode=0, max_niter=niter)
     xchg = PeerExchange(gb, bounds, dev, bits=False)
     return dict(

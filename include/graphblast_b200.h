@@ -357,6 +357,8 @@ int gb200_rmat_edges(int scale, long long nedges, unsigned long long seed,
  * the replicated bitmap (word_offsets[world+1], in 32-bit words; rank r owns words
  * [word_offsets[r], word_offsets[r+1])), passes its 64-byte IPC handle to every
  * other rank by any host channel (torch.distributed, MPI, a file), and connects.
+ * The offsets must start at 0 and every rank must own at least one word: other
+ * offsets are GrB_INVALID_VALUE on every rank, before anything is allocated.
  * After that the exchange needs no host library: the owner's kernel stores its
  * slice, count and epoch flag directly into every peer's copy over NVLink.
  * The reference has no multi-GPU code; this is the frontier all-gather that
@@ -374,7 +376,11 @@ int gb200_xchg_free(gb200_xchg_t x);
  * (word_offsets = vertex bounds / 32, rounded up).  v_own = levels of the owned
  * vertices (length = owned rows of M_local), M_local = the owned rows of A^T as an
  * (owned x n) matrix with CSR and CSC.  Collective: every rank calls it with the
- * same n and source. */
+ * same n and source.  The slices are stored 16 bytes at a time, so every owned
+ * word offset must be a multiple of 4 (vertex bounds multiples of 128), else
+ * GrB_INVALID_VALUE before anything is launched; a v_own whose size is not the
+ * owned vertex count, or an n that does not fill the exchange, is
+ * GrB_DIMENSION_MISMATCH. */
 int gb200_dist_bfs_fused(gb200_xchg_t x, gb200_vector_t v_own, gb200_matrix_t M_local,
                          long long n, long long source, gb200_desc_t desc,
                          int* levels_out);

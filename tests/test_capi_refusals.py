@@ -30,6 +30,7 @@ NULL_POINTER = int(gb.Info.GrB_NULL_POINTER)
 INVALID_VALUE = int(gb.Info.GrB_INVALID_VALUE)
 INVALID_INDEX = int(gb.Info.GrB_INVALID_INDEX)
 DOMAIN = int(gb.Info.GrB_DOMAIN_MISMATCH)
+DIMENSION = int(gb.Info.GrB_DIMENSION_MISMATCH)
 NO_VALUE = int(gb.Info.GrB_NO_VALUE)
 NOT_IMPLEMENTED = int(gb.Info.GrB_NOT_IMPLEMENTED)
 PANIC = int(gb.Info.GrB_PANIC)
@@ -197,6 +198,17 @@ def before_device_cases(desc):
         ("gb200_xchg_create", [_out(C.c_void_p), 0, 0, (C.c_longlong*2)(0, 1)], INVALID_VALUE),
         ("gb200_xchg_create", [_out(C.c_void_p), 33, 0, (C.c_longlong*34)()], INVALID_VALUE),
         ("gb200_xchg_create", [_out(C.c_void_p), 2, 2, (C.c_longlong*3)(0, 1, 2)], INVALID_VALUE),
+        # a rank that owns nothing: every rank refuses, none waits on its publishes
+        ("gb200_xchg_create", [_out(C.c_void_p), 2, 0, (C.c_longlong*3)(0, 0, 4)], INVALID_VALUE),
+        ("gb200_xchg_create", [_out(C.c_void_p), 2, 1, (C.c_longlong*3)(0, 0, 4)], INVALID_VALUE),
+        ("gb200_xchg_create", [_out(C.c_void_p), 2, 0, (C.c_longlong*3)(0, 4, 4)], INVALID_VALUE),
+        ("gb200_xchg_create", [_out(C.c_void_p), 3, 2, (C.c_longlong*4)(0, 8, 4, 12)],
+         INVALID_VALUE),
+        ("gb200_xchg_create", [_out(C.c_void_p), 1, 0, (C.c_longlong*2)(0, 0)], INVALID_VALUE),
+        # the slices start at word 0: words before the first would belong to no rank
+        ("gb200_xchg_create", [_out(C.c_void_p), 1, 0, (C.c_longlong*2)(-4, 4)], INVALID_VALUE),
+        ("gb200_xchg_create", [_out(C.c_void_p), 1, 0, (C.c_longlong*2)(4, 8)], INVALID_VALUE),
+        ("gb200_xchg_create", [_out(C.c_void_p), 2, 1, (C.c_longlong*3)(4, 8, 12)], INVALID_VALUE),
         ("gb200_xchg_handle", [None, P], NULL_POINTER),
         ("gb200_xchg_connect", [None, P], NULL_POINTER),
         ("gb200_xchg_free", [None], SUCCESS),
@@ -388,6 +400,41 @@ def test_source_out_of_range(g):
     for s in (-1, g.n):
         expect(g, INVALID_INDEX, "gb200_bfs", g.w, g.F, s, g.desc, None)
         expect(g, INVALID_INDEX, "gb200_sssp", g.w, g.F, s, g.desc, None)
+
+
+@pytest.mark.gpu
+def test_dist_entries_refuse_slices_the_kernels_cannot_run(g):
+    """Nothing is launched: the bitmap BFS refuses an owned slice that does not
+    start on a multiple of 4 words (128 vertices) before it looks at the peers,
+    and every traversal refuses a vector that is not the owned slice."""
+    lib, n, d = g.lib, g.n, g.desc
+
+    def xchg(world, rank, offsets):
+        h = C.c_void_p()
+        assert lib.gb200_xchg_create(C.byref(h), world, rank,
+                                     (C.c_longlong*len(offsets))(*offsets)) == SUCCESS
+        return h
+
+    # rank 1 of 2 owns words [1, 4): not connected, refused for the offset first
+    x = xchg(2, 1, [0, 1, 4])
+    try:
+        expect(g, INVALID_VALUE, "gb200_dist_bfs_fused", x, gb.Vector(96), g.F, 128, 0, d,
+               None)
+        expect(g, UNINITIALIZED, "gb200_dist_pr", x, gb.Vector(96), g.F, 128, 0.85, 0.0, d,
+               None)
+    finally:
+        lib.gb200_xchg_free(x)
+    # one rank over the chesapeake graph: 39 vertices, 2 bitmap words / 39 floats
+    for words, entry, args in (
+            (2, "gb200_dist_bfs_fused", (0, d, None)),
+            (n, "gb200_dist_sssp", (0, d, None)),
+            (n, "gb200_dist_pr", (0.85, 0.0, d, None))):
+        x = xchg(1, 0, [0, words])
+        try:
+            for size, nn in ((n - 1, n), (n + 1, n), (n, n + 33)):
+                expect(g, DIMENSION, entry, x, gb.Vector(size), g.F, nn, *args)
+        finally:
+            lib.gb200_xchg_free(x)
 
 
 @pytest.mark.gpu
