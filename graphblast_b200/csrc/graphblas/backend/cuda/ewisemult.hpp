@@ -158,6 +158,8 @@ Info eWiseMultColInner(SparseMatrix<c>* C, const Matrix<m>* mask, BinaryOpT accu
   A->nrows(&A_nrows);
   A->nvals(&A_nvals);
   if (A != C) CHECK(C->dup(A));
+  // a CSC sharing the CSR's value array would be scaled twice, once per side
+  C->separateCscValues();
   cudaStream_t s = gbStream();
   if (A_nvals > 0) {
     ewiseMultRowBroadcastKernel<<<gridFor(static_cast<size_t>(A_nrows)*32, 256),
@@ -192,6 +194,7 @@ Info eWiseMultRowInner(SparseMatrix<c>* C, const Matrix<m>* mask, BinaryOpT accu
   A->ncols(&A_ncols);
   A->nvals(&A_nvals);
   if (A != C) CHECK(C->dup(A));
+  C->separateCscValues();
   cudaStream_t s = gbStream();
   if (A_nvals > 0) {
     ewiseMultIndexBroadcastKernel<<<gridFor(A_nvals, 256), 256, 0, s>>>(

@@ -168,6 +168,15 @@ class SparseMatrix {
   // The entry set stopped being symmetric (tril): from the next upload on the
   // column-major side owns its index arrays instead of borrowing the CSR's.
   void dropSymmetry() { if (symmetric_) { releaseDevice(); symmetric_ = false; } }
+  // The CSC values become an array of this object's own when they are the CSR
+  // value array (an adopted CSC may name it), so that an operation can scale the
+  // two sides apart; a stream-ordered copy of the current values.
+  void separateCscValues() {
+    if (d_cscVal_ == NULL || d_cscVal_ != d_csrVal_) return;
+    d_cscVal_ = devArray<T>(atLeastOne(nvals_));
+    copyAsync(d_cscVal_, d_csrVal_, static_cast<size_t>(nvals_), cudaMemcpyDeviceToDevice);
+    cscval_ownership_ = true;
+  }
 
   Side hostCsr() { return Side{h_csrRowPtr_, h_csrColInd_, h_csrVal_, nrows_}; }
   Side hostCsc() { return Side{h_cscColPtr_, h_cscRowInd_, h_cscVal_, ncols_}; }
@@ -549,7 +558,10 @@ Info SparseMatrix<T>::build(Index* row_ptr, Index* col_ind, T* values, Index nva
 // may be NULL).  values == NULL: an owned copy of the CSR values is made, which
 // is only right when the values are symmetric too (pattern matrices) — a copy,
 // not an alias, because per-row rescaling (PageRank) must be able to make the
-// two sides differ.
+// two sides differ.  values == the CSR value array is taken as given; the
+// matrix x broadcast-vector eWiseMult (PageRank's normalisation) first gives the
+// CSC its own copy (separateCscValues), and the matrix x scalar one scales the
+// shared array once.
 template <typename T>
 Info SparseMatrix<T>::adoptCsc(Index* col_ptr, Index* row_ind, T* values,
     bool symmetric) {

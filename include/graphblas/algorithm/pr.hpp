@@ -60,6 +60,10 @@ inline float pr(Vector<float>* p, const Matrix<float>* A, float alpha, float eps
     GB_ALGO_STEP(p->swap(&p_prev));
     vxm<float, float, float, float>(&p_swap, GrB_NULL, GrB_NULL,
         PlusMultipliesSemiring<float>(), &p_prev, A, desc);
+    // A push (mxvmode 1) leaves p_prev and p_swap sparse; the update below and the
+    // next iteration's swap take them dense (no work when they already are).
+    GB_ALGO_STEP(p_prev.sparse2dense(0.f));
+    GB_ALGO_STEP(p_swap.sparse2dense(0.f));
     if (backend::prUpdateStep(&p->vector_, &p_swap.vector_, &p_prev.vector_,
                               (1.f - alpha)/n, &error, &desc->descriptor_) != GrB_SUCCESS) {
       eWiseAdd<float, float, float, float>(p, GrB_NULL, GrB_NULL,

@@ -259,30 +259,6 @@ def pr_params(r, g):
     return PR_ALPHA, 0.0, 10, 10
 
 
-def sssp_rounds(rp, ci, w, s, max_rounds):
-    """The frontier Bellman-Ford of the library's SSSP in float32: per round,
-    relaxed[j] = min over frontier entries u of fl(f[u] + A(u, j)), v = min(v,
-    relaxed), the next frontier = the entries that improved v.  Returns (distances,
-    rounds run): the last round is the one that leaves the frontier empty, or
-    max_rounds."""
-    n = len(rp) - 1
-    rows = np.repeat(np.arange(n), np.diff(rp))
-    inf = np.float32(FLT_MAX)
-    d = np.full(n, inf, np.float32)
-    f = np.full(n, inf, np.float32)
-    d[s] = f[s] = 0
-    rounds = 0
-    while rounds < max_rounds and np.any(f < inf):
-        rounds += 1
-        act = f[rows] < inf
-        relaxed = np.full(n, inf, np.float32)
-        np.minimum.at(relaxed, ci[act], f[rows[act]] + w[act])
-        improved = relaxed < d
-        d = np.minimum(d, relaxed)
-        f = np.where(improved, relaxed, inf).astype(np.float32)
-    return d, rounds
-
-
 # ---------------------------------------------------------------------------
 # the launch (pytest side)
 # ---------------------------------------------------------------------------
@@ -454,13 +430,14 @@ def test_sssp(ranks, world, i, j):
     integer weights, the single-GPU algorithm.sssp's with real weights, and within
     1e-6 of float64 Dijkstra; every rank returns the host's round count."""
     import oracle_binding as orc
+    from sssp_pr_reference import sssp_rounds
     c, r = CASES[world][i], CASES[world][i]["runs"][j]
     res = ranks(world, i)
     rp, ci = graph(c["graph"])
     src = int(res["%d_source" % j])
     _check_source(r, world, i, src, res["bounds"].tolist())
     w = weights(r["w"], len(ci))
-    want, rounds = sssp_rounds(rp, ci, w, src, r["cut"] or 10**6)
+    want, rounds = sssp_rounds(rp, ci, w, src, r["cut"])
     if r["cut"] is None and r["w"] == "int":
         assert np.array_equal(want, orc.sssp(rp, ci, w, src))
     if r["cut"] is None and r["w"] == "real":
