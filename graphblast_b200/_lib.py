@@ -121,6 +121,13 @@ SIGNATURES = [
     ("gb200_dist_sssp", _I, [_P, _P, _P, _LL, _LL, _P, C.POINTER(_I)]),
 ]
 
+# (name, restype, argtypes) for every symbol declared in include/graphblast_b200_lgc.h,
+# the companion header of local graph clustering; load() binds these too.
+LGC_SIGNATURES = [
+    ("gb200_lgc", _I, [_P, _P, _P, _I, _D, _D, _P, _IP, C.POINTER(_F)]),
+    ("gb200_lgc_sweep", _I, [_P, _P, _P, _P, _IP, C.POINTER(_D), C.POINTER(_F)]),
+]
+
 
 class ExtensionMissing(RuntimeError):
     pass
@@ -137,7 +144,7 @@ def load():
             "`python -c 'import __graft_entry__ as g; g.build()'`; "
             "there is no CPU fallback." % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
-    for name, restype, argtypes in SIGNATURES:
+    for name, restype, argtypes in SIGNATURES + LGC_SIGNATURES:
         fn = getattr(lib, name)   # AttributeError if a declared symbol is missing
         fn.restype = restype
         fn.argtypes = argtypes

@@ -1,10 +1,11 @@
 """graphblas::algorithm — the GraphBLAS algorithm drivers of the reference
 (graphblas/algorithm/{bfs,sssp,pr,tc}.hpp), executed inside the native library as
 loops of backend operations (include/graphblas/algorithm/*.hpp), and the graph
-colouring gc, the maximal independent set mis and the connected components cc, one
-kernel each on the device.
+colouring gc, the maximal independent set mis, the connected components cc and the
+local graph clustering lgc, one kernel each on the device, with lgc_sweep, the
+conductance sweep cut of lgc's result.
 
-sssp, pr, tc, gc, mis and cc return the device time of the operation loop in milliseconds
+sssp, pr, tc, gc, mis, cc, lgc and lgc_sweep return the device time of the operation loop in milliseconds
 ("tight" in the reference drivers, example/gbfs.cu:110-115).  bfs returns it only
 when called with timed=True; otherwise it returns None and, when the traversal runs
 as the fused kernel, only enqueues it, so that back-to-back traversals keep the GPU
@@ -96,3 +97,39 @@ def cc(v, A, desc):
     _check(_lib.load().gb200_cc(v._h, A._h, desc._h, C.byref(k), C.byref(ms)),
            "algorithm::cc")
     return k.value, ms.value
+
+
+def lgc(p, A, s, alpha, eps, desc, residual=None):
+    """p = the approximate personalised PageRank of source s on the lazy walk of A's
+    pattern (Andersen-Chung-Lang push, synchronous rounds), bit for bit the floats of
+    the reference's CPU checker SimpleReferenceLgc<float> (algorithm/test_lgc.hpp) for
+    sorted column lists; one cooperative kernel (include/graphblas/algorithm/lgc.hpp).
+    residual: None or a Vector that receives the final residual r.  At most desc's
+    max_niter rounds; desc's mxvmode picks each round's route (1 sparse, 2 dense, 0 by
+    the frontier's volume against switchpoint * nnz) and never changes the result.  A
+    is FP32 or INT32 (same result); a non-symmetric A needs its CSC.  alpha in (0, 1],
+    eps > 0.  p and residual become dense.  Returns (rounds, tight_ms)."""
+    ms = C.c_float(0)
+    k = C.c_int(0)
+    _check(_lib.load().gb200_lgc(p._h, residual._h if residual is not None else None, A._h,
+                                 int(s), float(alpha), float(eps), desc._h, C.byref(k),
+                                 C.byref(ms)),
+           "algorithm::lgc")
+    return k.value, ms.value
+
+
+def lgc_sweep(cluster, p, A, desc):
+    """cluster[i] = 1 for the members of the sweep cut of p, else 0: of the prefixes of
+    {v : p[v] > 0, row v not empty} ordered by p[v]/d[v] descending (fp32, ties by
+    ascending id), the smallest one of least conductance cut/min(vol, nnz - vol), with
+    exact integer cut and volume (include/graphblas/algorithm/lgc.hpp).  A is FP32 or
+    INT32; a non-symmetric A needs its CSC.  A p held sparse is converted to dense
+    storage (its values unchanged).  Returns (size, conductance, tight_ms);
+    (0, nan, ...) and an empty cluster when no prefix qualifies."""
+    ms = C.c_float(0)
+    k = C.c_int(0)
+    phi = C.c_double(0)
+    _check(_lib.load().gb200_lgc_sweep(cluster._h, p._h, A._h, desc._h, C.byref(k),
+                                       C.byref(phi), C.byref(ms)),
+           "algorithm::lgc_sweep")
+    return k.value, phi.value, ms.value

@@ -27,8 +27,10 @@
 #include "graphblas/algorithm/gc.hpp"
 #include "graphblas/algorithm/mis.hpp"
 #include "graphblas/algorithm/cc.hpp"
+#include "graphblas/algorithm/lgc.hpp"
 
 #include "graphblast_b200.h"
+#include "graphblast_b200_lgc.h"
 
 bool debug_;
 bool memory_;
@@ -1108,6 +1110,46 @@ int gb200_cc(gb200_vector_t v, gb200_matrix_t A, gb200_desc_t desc, int* ncompon
     });
   });
   if (info == 0 && ncomponents) *ncomponents = count;
+  return info;
+}
+
+int gb200_lgc(gb200_vector_t p, gb200_vector_t r, gb200_matrix_t A, int source,
+              double alpha, double eps, gb200_desc_t desc, int* rounds, float* tight_ms) {
+  if (p == NULL || A == NULL || desc == NULL)
+    return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
+  if (A->f == NULL && A->i == NULL) return rc(graphblas::GrB_DOMAIN_MISMATCH);
+  int n = 0;
+  onMatrix(A, [&](auto M) { return M->nrows(&n); });
+  if (source < 0 || source >= n) return rc(graphblas::GrB_INVALID_INDEX);
+  if (!(alpha > 0.0 && alpha <= 1.0) || !(eps > 0.0)) return rc(graphblas::GrB_INVALID_VALUE);
+  GB200_REQUIRE_DEVICE();
+  int count = 0;
+  const int info = runAlgorithm(tight_ms, [&] {
+    return onMatrix(A, [&](auto M) {
+      return graphblas::algorithm::lgc(p->f, vec(r), M, source, alpha, eps, &desc->desc,
+                                       &count);
+    });
+  });
+  if (info == 0 && rounds) *rounds = count;
+  return info;
+}
+
+int gb200_lgc_sweep(gb200_vector_t cluster, gb200_vector_t p, gb200_matrix_t A,
+                    gb200_desc_t desc, int* size, double* conductance, float* tight_ms) {
+  if (cluster == NULL || p == NULL || A == NULL || desc == NULL)
+    return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
+  if (A->f == NULL && A->i == NULL) return rc(graphblas::GrB_DOMAIN_MISMATCH);
+  GB200_REQUIRE_DEVICE();
+  int members = 0;
+  double phi = 0.0;
+  const int info = runAlgorithm(tight_ms, [&] {
+    return onMatrix(A, [&](auto M) {
+      return graphblas::algorithm::lgcSweep(cluster->f, p->f, M, &desc->desc, &members,
+                                            &phi);
+    });
+  });
+  if (info == 0 && size) *size = members;
+  if (info == 0 && conductance) *conductance = phi;
   return info;
 }
 

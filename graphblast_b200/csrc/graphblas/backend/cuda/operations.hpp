@@ -41,6 +41,7 @@
 #include "graphblas/backend/cuda/color.hpp"
 #include "graphblas/backend/cuda/mis.hpp"
 #include "graphblas/backend/cuda/cc.hpp"
+#include "graphblas/backend/cuda/lgc.hpp"
 
 namespace graphblas {
 namespace backend {
