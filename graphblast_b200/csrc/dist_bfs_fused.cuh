@@ -426,9 +426,7 @@ int gb200_dist_bfs_fused(gb200_xchg_t x, gb200_vector_t v, gb200_matrix_t M,
   a.lo = static_cast<long long>(w_lo)*32;
   a.max_levels = d.max_niter_;
   a.switchpoint = d.switchpoint();
-  Desc_value mode;
-  CHECK(desc->desc.get(GrB_MXVMODE, &mode));
-  a.mode = (mode == GrB_PUSHONLY) ? 1 : (mode == GrB_PULLONLY ? 2 : 0);
+  a.mode = d.mxvRoute();
   a.levels = v->f->vector_.dense_.d_val_;
   a.seed = x->d_seed;
   a.next_own = reinterpret_cast<unsigned int*>(base);
@@ -443,14 +441,8 @@ int gb200_dist_bfs_fused(gb200_xchg_t x, gb200_vector_t v, gb200_matrix_t M,
   a.epoch0 = x->epoch;
   a.timeout_cycles = 20000000000ll;
 
-  const int grid = cooperativeGrid<gbx::bfsFusedDistKernel, GBX_BFS_NT>();
-  if (grid < 1) return rc(GrB_PANIC);
-  void* params[] = { &a };
   profiler().begin(GB_PROF_PULL_BOOL, s);
-  CUDA_CALL(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(gbx::bfsFusedDistKernel),
-      dim3(grid),
-      dim3(GBX_BFS_NT), params, 0, s));
-  GB_KERNEL_CHECK();
+  CHECK((launchCooperative<gbx::bfsFusedDistKernel, GBX_BFS_NT>(s, a)));
   profiler().end(GB_PROF_PULL_BOOL, s, 0.0);
   v->f->vector_.dense_.touched();
   // every rank ran the same number of levels = publishes

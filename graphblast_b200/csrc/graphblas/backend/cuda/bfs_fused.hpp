@@ -1,8 +1,9 @@
 // graphblast_b200 backend — host side of the fused BFS (kernels/bfs_fused.cuh):
-// one cooperative launch per traversal.  Entered from algorithm::bfs of this
-// project's frontend when the descriptor carries the BFS flags of the reference's
-// benchmark script (run_bfs.sh:8-27: --struconly 1 --opreuse 1 --earlyexit 1,
-// --fusedmask 1); every other combination runs the operation-by-operation loop.
+// one cooperative launch (launchCooperative, util.hpp) per traversal.  Entered from
+// algorithm::bfs of this project's frontend when the descriptor carries the BFS flags
+// of the reference's benchmark script (run_bfs.sh:8-27: --struconly 1 --opreuse 1
+// --earlyexit 1, --fusedmask 1); every other combination runs the operation-by-operation
+// loop.
 #ifndef GRAPHBLAS_BACKEND_CUDA_BFS_FUSED_HPP_
 #define GRAPHBLAS_BACKEND_CUDA_BFS_FUSED_HPP_
 
@@ -28,8 +29,10 @@ inline bool bfsTrace() {
   return on;
 }
 
-// Layout of GB_SCRATCH_BFS for a traversal of n vertices: the byte offset of each
-// array of BfsFusedArgs, each on a 256-byte boundary, and the bytes of the slot.
+// Layout of GB_SCRATCH_BFS for a traversal of n vertices (ScratchLayout, util.hpp): the
+// byte offset of each array of BfsFusedArgs, and the bytes of the slot.  The slot stays
+// with the descriptor, not with the call: a traversal that was only enqueued still uses
+// it after bfsFused returns.
 struct BfsScratchLayout {
   size_t visited[2], frontier, next, counters, heavy, walk, walk_count, walk_chunks,
          level8, bytes;
@@ -39,23 +42,18 @@ inline BfsScratchLayout bfsScratchLayout(Index n) {
   const size_t nwords = (static_cast<size_t>(n) + 31)/32;
   const size_t nchunks = (nwords + 31)/32;
   BfsScratchLayout l;
-  size_t at = 0;
-  auto place = [&at](size_t bytes) {
-    const size_t off = at;
-    at += (bytes + 255)/256*256;
-    return off;
-  };
-  l.visited[0]  = place(nwords*sizeof(unsigned int));
-  l.visited[1]  = place(nwords*sizeof(unsigned int));
-  l.frontier    = place(nwords*sizeof(unsigned int));
-  l.next        = place(nwords*sizeof(unsigned int));
-  l.counters    = place(GB_BFS_NCOUNTERS*sizeof(unsigned long long));
-  l.heavy       = place(GB_BFS_HEAVY_CAP*sizeof(Index));
-  l.walk        = place(nchunks*GB_BFS_CHUNK*sizeof(Index));
-  l.walk_count  = place(nchunks*sizeof(int));
-  l.walk_chunks = place(nchunks*sizeof(Index));
-  l.level8      = place(static_cast<size_t>(n));
-  l.bytes = at;
+  ScratchLayout at;
+  l.visited[0]  = at.place(nwords*sizeof(unsigned int));
+  l.visited[1]  = at.place(nwords*sizeof(unsigned int));
+  l.frontier    = at.place(nwords*sizeof(unsigned int));
+  l.next        = at.place(nwords*sizeof(unsigned int));
+  l.counters    = at.place(GB_BFS_NCOUNTERS*sizeof(unsigned long long));
+  l.heavy       = at.place(GB_BFS_HEAVY_CAP*sizeof(Index));
+  l.walk        = at.place(nchunks*GB_BFS_CHUNK*sizeof(Index));
+  l.walk_count  = at.place(nchunks*sizeof(int));
+  l.walk_chunks = at.place(nchunks*sizeof(Index));
+  l.level8      = at.place(static_cast<size_t>(n));
+  l.bytes = at.bytes;
   return l;
 }
 
@@ -111,9 +109,7 @@ Info bfsFused(Vector<float>* v, const Matrix<a>* A, Index s, Descriptor* desc, i
   args.source = s;
   args.max_levels = desc->max_niter_;
   args.switchpoint = desc->switchpoint();
-  Desc_value mode;
-  CHECK(desc->get(GrB_MXVMODE, &mode));
-  args.mode = (mode == GrB_PUSHONLY) ? 1 : (mode == GrB_PULLONLY ? 2 : 0);
+  args.mode = desc->mxvRoute();
   args.levels = v->dense_.d_val_;
   args.visited[0]  = reinterpret_cast<unsigned int*>(base + l.visited[0]);
   args.visited[1]  = reinterpret_cast<unsigned int*>(base + l.visited[1]);
@@ -136,21 +132,12 @@ Info bfsFused(Vector<float>* v, const Matrix<a>* A, Index s, Descriptor* desc, i
 
   // push-only traversals run the instantiation without the pull level, with more
   // warps per SM
-  const bool push_only = (args.mode == 1);
-  void (*kernel)(BfsFusedArgs) =
-      push_only ? bfsFusedKernel<GB_BFS_PUSH_NT, GB_BFS_PUSH_MINB, false>
-                : bfsFusedKernel<GB_BFS_NT, GB_BFS_MINB, true>;
-  const int nt = push_only ? GB_BFS_PUSH_NT : GB_BFS_NT;
-  const int grid = push_only
-      ? cooperativeGrid<bfsFusedKernel<GB_BFS_PUSH_NT, GB_BFS_PUSH_MINB, false>,
-                        GB_BFS_PUSH_NT>()
-      : cooperativeGrid<bfsFusedKernel<GB_BFS_NT, GB_BFS_MINB, true>, GB_BFS_NT>();
-  if (grid < 1) return GrB_PANIC;
-  void* params[] = { &args };
   profiler().begin(GB_PROF_PULL_BOOL, stream);
-  CUDA_CALL(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(kernel),
-      dim3(grid), dim3(nt), params, 0, stream));
-  GB_KERNEL_CHECK();
+  const Info launched = args.mode == 1
+      ? launchCooperative<bfsFusedKernel<GB_BFS_PUSH_NT, GB_BFS_PUSH_MINB, false>,
+                          GB_BFS_PUSH_NT>(stream, args)
+      : launchCooperative<bfsFusedKernel<GB_BFS_NT, GB_BFS_MINB, true>, GB_BFS_NT>(stream, args);
+  if (launched != GrB_SUCCESS) return launched;
   profiler().end(GB_PROF_PULL_BOOL, stream, 0.0);
   v->dense_.touched();
   if (args.trace) {                      // per-level times of this traversal

@@ -152,6 +152,12 @@ class Descriptor {
   bool  atomic()      { return atomic_; }
   float switchpoint() { return switchpoint_; }
   float memusage()    { return memusage_; }
+  // The route of a cooperative kernel that picks push or pull itself, by mxvmode: 1 push
+  // only, 2 pull only, 0 its own choice at every level or round.
+  int mxvRoute() const {
+    const Desc_value mode = desc_[GrB_MXVMODE];
+    return mode == GrB_PUSHONLY ? 1 : (mode == GrB_PULLONLY ? 2 : 0);
+  }
 
   // ---- legacy two-buffer scratch (reference :156-192), for callers that name
   // "buffer" / "temp" -------------------------------------------------------------------

@@ -4,9 +4,9 @@
 //
 // Semantics.  i and j are joined when A(i,j) or A(j,i) is stored (stored zeros count,
 // self-loops are ignored, values are never read).  out[i] = the smallest vertex id in
-// the weakly connected component of i; counters[1] = the number of components, the
-// number of i with out[i] == i.  Only the CSR is read: union-find joins both ends of
-// each stored entry, so a non-symmetric A needs no CSC.
+// the weakly connected component of i; counters[CC_COMPONENTS] = the number of
+// components, the number of i with out[i] == i.  Only the CSR is read: union-find
+// joins both ends of each stored entry, so a non-symmetric A needs no CSC.
 //
 // Forest.  parent[x] <= x for every x, and x is a root iff parent[x] == x.  A word only
 // ever changes to a smaller vertex of x's tree:
@@ -27,7 +27,7 @@
 //   rounds    r = 0, 1: every v with more than r entries links (v, colind[rowptr[v]+r]);
 //             each round is followed by a compress.
 //   sample    symmetric A only: CTA 0 counts the roots of GB_CC_SAMPLES hashed vertices
-//             in shared memory and publishes the most frequent one, L, in counters[0].
+//             in shared memory and publishes the most frequent one, L, in CC_LARGEST.
 //   finish    every v links its entries from position 2 on, except, for a symmetric A,
 //             a v whose parent reads L (already in L's tree; each of its edges to a
 //             vertex outside L's tree is the other end's entry, linked from there).
@@ -63,14 +63,20 @@ namespace backend {
 #define GB_CC_SAMPLES   1024           // vertices whose roots the sample counts
 #define GB_CC_SLOTS     2048           // shared hash slots for the sampled roots
 
+enum CcCell {
+  CC_LARGEST    = 0,                   // L, the most frequent sampled root
+  CC_COMPONENTS = 1,                   // the number of components
+  CC_QUEUED     = 2,                   // the number of rows queued for the grid pass
+  CC_NCELLS     = 3
+};
+
 struct CcArgs {
   const Index* row_ptr;  const Index* row_ind;   // CSR; row_ptr NULL: no stored entries
   Index n;
   int skip;                      // A is symmetric: the finish skips L's tree
   Index* parent;                 // [n] the union-find forest
   Index* queued;                 // [nnz / GB_CC_GRID_MIN + 1] rows for the grid pass
-  unsigned long long* counters;  // [0] L, the most frequent sampled root; [1] the count;
-                                 // [2] the number of queued rows
+  unsigned long long* counters;  // [CC_NCELLS] CcCell
 };
 
 __device__ __forceinline__ Index ccLoad(const Index* p) {
@@ -81,14 +87,6 @@ __device__ __forceinline__ Index ccLoad(const Index* p) {
 
 __device__ __forceinline__ void ccStore(Index* p, Index x) {
   asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" :: "l"(p), "r"(x) : "memory");
-}
-
-// The sample's vertex hash (fmix32, the murmur3 finaliser).
-__device__ __forceinline__ unsigned int ccHash(unsigned int x) {
-  x ^= x >> 16; x *= 0x85EBCA6Bu;
-  x ^= x >> 13; x *= 0xC2B2AE35u;
-  x ^= x >> 16;
-  return x;
 }
 
 // The root of x, halving the path on the way by CAS.
@@ -138,10 +136,10 @@ __device__ __forceinline__ Index ccSample(const CcArgs& a) {
   if (threadIdx.x == 0) best = 0ull;
   __syncthreads();
   for (int i = threadIdx.x; i < GB_CC_SAMPLES; i += GB_CC_NT) {
-    const Index v = static_cast<Index>(ccHash(static_cast<unsigned int>(i)) %
+    const Index v = static_cast<Index>(fmix32(static_cast<unsigned int>(i)) %
                                        static_cast<unsigned int>(a.n));
     const Index r = ccLoad(a.parent + v);
-    unsigned int slot = ccHash(static_cast<unsigned int>(r)) & (GB_CC_SLOTS - 1);
+    unsigned int slot = fmix32(static_cast<unsigned int>(r)) & (GB_CC_SLOTS - 1);
     while (true) {
       const Index k = atomicCAS(keys + slot, -1, r);
       if (k == -1 || k == r) { atomicAdd(counts + slot, 1u); break; }
@@ -187,12 +185,11 @@ ccKernel(CcArgs a, W* out) {
     // ---- sample ----------------------------------------------------------------------
     if (a.skip && blockIdx.x == 0) {
       const Index L = ccSample(a);
-      if (threadIdx.x == 0) a.counters[0] = static_cast<unsigned long long>(L);
+      if (threadIdx.x == 0) a.counters[CC_LARGEST] = static_cast<unsigned long long>(L);
     }
     if (a.skip) grid.sync();
-    const Index L = a.skip
-        ? static_cast<Index>(*reinterpret_cast<volatile unsigned long long*>(a.counters))
-        : -1;
+    const Index L = a.skip ? static_cast<Index>(
+        *reinterpret_cast<volatile unsigned long long*>(a.counters + CC_LARGEST)) : -1;
 
     // ---- finish: entries from position 2 on, a lane or a warp per list ---------------
     for (Index i0 = gwarp*32; i0 < a.n; i0 += gwarps*32) {
@@ -204,7 +201,7 @@ ccKernel(CcArgs a, W* out) {
         if (e < b) e = b;
       }
       const bool grid_v = e - b >= GB_CC_GRID_MIN;
-      if (grid_v) a.queued[atomicAdd(a.counters + 2, 1ull)] = v;
+      if (grid_v) a.queued[atomicAdd(a.counters + CC_QUEUED, 1ull)] = v;
       const bool heavy_v = !grid_v && e - b >= GB_CC_LANE_MAX;
       if (!heavy_v && !grid_v)
         for (Index k = b; k < e; ++k) ccLink(a.parent, v, __ldg(a.row_ind + k));
@@ -221,7 +218,7 @@ ccKernel(CcArgs a, W* out) {
     grid.sync();
 
     // ---- grid pass: the queued lists in 32-entry chunks, chunk c to warp c % warps ----
-    const Index nq = static_cast<Index>(__ldcg(a.counters + 2));
+    const Index nq = static_cast<Index>(__ldcg(a.counters + CC_QUEUED));
     Index before = 0;                  // chunks of the lists before q, modulo warps
     for (Index q = 0; q < nq; ++q) {
       const Index h = __ldcg(a.queued + q);
@@ -249,7 +246,7 @@ ccKernel(CcArgs a, W* out) {
   }
   roots = __reduce_add_sync(GB_FULL_MASK, roots);
   if (lane == 0 && roots != 0u)
-    atomicAdd(a.counters + 1, static_cast<unsigned long long>(roots));
+    atomicAdd(a.counters + CC_COMPONENTS, static_cast<unsigned long long>(roots));
 }
 
 }  // namespace backend

@@ -122,7 +122,8 @@ struct ColorStep {
       top = c > top ? c : top;
     }
     top = __reduce_max_sync(GB_FULL_MASK, top);
-    if (lane == 0 && top != 0u) atomicMax(a.counters + 3, static_cast<unsigned long long>(top));
+    if (lane == 0 && top != 0u) atomicMax(a.counters + GREEDY_COUNT,
+                                          static_cast<unsigned long long>(top));
   }
 };
 

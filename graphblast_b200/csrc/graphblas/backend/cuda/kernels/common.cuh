@@ -252,6 +252,15 @@ __device__ __forceinline__ bool bitSetAtomic(unsigned int* bits, int i) {
   return (atomicOr(w, m) & m) == 0;
 }
 
+// fmix32, the murmur3 finaliser: the vertex hash of the components sample and of the
+// greedy priority (host and device; the colouring oracle restates it).
+__host__ __device__ __forceinline__ unsigned int fmix32(unsigned int x) {
+  x ^= x >> 16; x *= 0x85EBCA6Bu;
+  x ^= x >> 13; x *= 0xC2B2AE35u;
+  x ^= x >> 16;
+  return x;
+}
+
 // upper_bound over a sorted int array: first index with a[idx] > key.
 __device__ __forceinline__ int upperBound(const int* a, int n, int key) {
   int lo = 0, hi = n;

@@ -9,8 +9,7 @@
 // pattern.  Every vertex has the priority
 //     p(v) = (gcHash(seed, v), v), compared lexicographically,
 //     gcHash(seed, v) = fmix32(v ^ (seed * 0x9E3779B9)),
-//     fmix32(x): x ^= x >> 16; x *= 0x85EBCA6B; x ^= x >> 13; x *= 0xC2B2AE35; x ^= x >> 16
-// (32-bit unsigned arithmetic; fmix32 is the murmur3 finaliser).
+// in 32-bit unsigned arithmetic, with fmix32 the murmur3 finaliser (common.cuh).
 //
 // Step.  What deciding a vertex means is the step type's; the schedule never branches
 // on which algorithm it serves.  A step supplies
@@ -21,7 +20,7 @@
 //     is decided, otherwise waiting / resume hold where to look next time (the same in
 //     every lane);
 //   out(a, out, first, stride, lane) — the out pass over all n vertices, and its count
-//     into counters[3].
+//     into GREEDY_COUNT.
 // A step keeps progress: the highest-priority undecided vertex is never blocked, and
 // no warp waits on another warp; a blocked vertex is put back.
 //
@@ -51,6 +50,13 @@ namespace backend {
 #define GB_GC_MINB      2              // resident CTAs per SM the register budget allows
 #define GB_GC_LANE_MAX  32             // longest list a single lane takes in a sweep
 
+enum GreedyCell {
+  GREEDY_LEFT   = 0,                   // [3] list length of sweep s in cell s % 3 (the
+                                       // cell of sweep s + 1 is zeroed during s)
+  GREEDY_COUNT  = 3,                   // the step's count: colours or members
+  GREEDY_NCELLS = 4
+};
+
 struct GreedyArgs {
   const Index* row_ptr;  const Index* row_ind;        // CSR
   const Index* col_ptr;  const Index* col_ind;        // CSC; NULL when it is the CSR
@@ -60,19 +66,14 @@ struct GreedyArgs {
   Index* waiting_on;             // [n] undecided higher-priority neighbour last seen
   Index* resume;                 // [n] list position where the blocker scan goes on
   Index* list[2];                // [n] undecided vertices, ping-pong between sweeps
-  unsigned long long* counters;  // [0..2] list length (rotating with the sweep % 3: the
-                                 // cell of sweep s + 1 is zeroed during s), [3] the count
+  unsigned long long* counters;  // [GREEDY_NCELLS] GreedyCell
 };
 
 enum GreedyPoll { GREEDY_DONE, GREEDY_BLOCKED, GREEDY_ATTEMPT };
 
 // The priority hash, host and device (the oracle restates it).
 __host__ __device__ __forceinline__ unsigned int gcHash(unsigned int seed, unsigned int v) {
-  unsigned int x = v ^ (seed*0x9E3779B9u);
-  x ^= x >> 16; x *= 0x85EBCA6Bu;
-  x ^= x >> 13; x *= 0xC2B2AE35u;
-  x ^= x >> 16;
-  return x;
+  return fmix32(v ^ (seed*0x9E3779B9u));
 }
 
 // p(u) > p(v)
@@ -133,8 +134,8 @@ __device__ __forceinline__ void greedySchedule(const GreedyArgs a, W* out) {
   int s = 0;
   while (m > tail_max) {
     Index* next = (s & 1) ? a.list[1] : a.list[0];   // no dynamic index into the params
-    unsigned long long* count = a.counters + (s % 3);
-    if (gtid == 0) a.counters[(s + 1) % 3] = 0ull;
+    unsigned long long* count = a.counters + GREEDY_LEFT + s % 3;
+    if (gtid == 0) a.counters[GREEDY_LEFT + (s + 1) % 3] = 0ull;
     for (Index i0 = gwarp*32; i0 < m; i0 += gwarps*32) {
       const Index i = i0 + lane;
       Index v = -1, waiting = -1, resume = 0;

@@ -137,7 +137,7 @@ struct MisStep {
     }
     members = __reduce_add_sync(GB_FULL_MASK, members);
     if (lane == 0 && members != 0u)
-      atomicAdd(a.counters + 3, static_cast<unsigned long long>(members));
+      atomicAdd(a.counters + GREEDY_COUNT, static_cast<unsigned long long>(members));
   }
 };
 

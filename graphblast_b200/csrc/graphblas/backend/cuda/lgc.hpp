@@ -1,6 +1,6 @@
 // graphblast_b200 backend — host side of local graph clustering (kernels/lgc.cuh): the
-// refusals, the scratch, the one cooperative launch of the push and the launches of the
-// sweep cut.  algorithm::lgc and algorithm::lgcSweep come here.
+// input (graph_input.hpp), the scratch, the one cooperative launch of the push and the
+// launches of the sweep cut.  algorithm::lgc and algorithm::lgcSweep come here.
 #ifndef GRAPHBLAS_BACKEND_CUDA_LGC_HPP_
 #define GRAPHBLAS_BACKEND_CUDA_LGC_HPP_
 
@@ -9,36 +9,12 @@
 
 #include <cub/cub.cuh>
 
+#include "graphblas/backend/cuda/graph_input.hpp"
 #include "graphblas/backend/cuda/ingest.hpp"
 #include "graphblas/backend/cuda/kernels/lgc.cuh"
 
 namespace graphblas {
 namespace backend {
-
-// The refusals lgc and lgcSweep share, in this order and before anything is touched: a
-// dense A (GrB_NOT_IMPLEMENTED, naming `what`); A not square, or x or y (when not
-// NULL) not of size nrows(A) (GrB_DIMENSION_MISMATCH); an A with stored entries but
-// without a device CSR, or non-symmetric without a device CSC (GrB_UNINITIALIZED_OBJECT).
-template <typename a>
-Info lgcCheck(const char* what, Vector<float>* x, Vector<float>* y, const Matrix<a>* A) {
-  if (!A->isSparse()) {
-    std::cout << "Error: " << what << " of a dense matrix is not implemented in this backend\n";
-    return GrB_NOT_IMPLEMENTED;
-  }
-  const SparseMatrix<a>* S = &A->sparse_;
-  const Index n = S->nrows_;
-  if (n != S->ncols_) return GrB_DIMENSION_MISMATCH;
-  for (Vector<float>* v : {x, y}) {
-    if (v == NULL) continue;
-    Index size = 0;
-    CHECK(v->size(&size));
-    if (size != n) return GrB_DIMENSION_MISMATCH;
-  }
-  if (n > 0 && S->nvals_ > 0 &&
-      (S->d_csrRowPtr_ == NULL || (!S->sameStructure() && S->d_cscColPtr_ == NULL)))
-    return GrB_UNINITIALIZED_OBJECT;
-  return GrB_SUCCESS;
-}
 
 // p = the approximate personalised PageRank of source s (kernels/lgc.cuh states the
 // arithmetic); r (when not NULL) = the final residual; *rounds = the rounds run, at most
@@ -46,62 +22,54 @@ Info lgcCheck(const char* what, Vector<float>* x, Vector<float>* y, const Matrix
 // NULL) = the device time, from CUDA events.  p and r become dense with nrows(A)
 // entries.  mode: 0 chooses each round's route by the frontier volume against
 // switchpoint*nnz, 1 takes only sparse rounds, 2 only dense rounds.  s, alpha and eps
-// are checked by the caller.  Refusals as lgcCheck, then r the same vector as p
-// (GrB_INVALID_VALUE).  stats (when not NULL) = {pushed volume, dense rounds}.
-// Scratch: 256 bytes of counters, six n-word arrays (r when not asked for, c, in_f,
-// claim, two frontier lists) and the touched list, freed after the launch.
+// are checked by the caller.  Refusals: those of graphCheck (with the CSC), then r the
+// same vector as p (GrB_INVALID_VALUE).  stats (when not NULL) = {pushed volume, dense
+// rounds}.
+// Scratch: the counter cells, seven n-word arrays (c, in_f, claim, two frontier lists,
+// the touched list, r when not asked for) and the pattern's zero row pointers.
 template <typename a>
 Info lgcRun(Vector<float>* p, Vector<float>* r, const Matrix<a>* A, Index s, double alpha,
             double eps, int max_rounds, int mode, float switchpoint, int* rounds,
             float* ms = NULL, unsigned long long* stats = NULL) {
-  CHECK(lgcCheck("lgc", p, r, A));
+  CHECK(graphCheck("lgc", A, true, p, r));
   if (r == p) return GrB_INVALID_VALUE;
-  const SparseMatrix<a>* S = &A->sparse_;
-  const Index n = S->nrows_;
+  const SparseMatrix<a>& S = A->sparse_;
+  const Index n = S.nrows_;
   GpuTimer clock;
   clock.Start();
   if (rounds != NULL) *rounds = 0;
   if (stats != NULL) stats[0] = stats[1] = 0ull;
-  const int grid = cooperativeGrid<lgcKernel, GB_LGC_NT>();
-  if (grid < 1) return GrB_PANIC;
   cudaStream_t stream = gbStream();
-  const bool stored = S->nvals_ > 0;
 
-  const size_t words = (static_cast<size_t>(n) + 63)/64*64;      // 256-byte aligned arrays
-  const size_t rp_words = stored ? 0 : (static_cast<size_t>(n) + 64)/64*64;
-  unsigned char* block = static_cast<unsigned char*>(gbMalloc(
-      256 + (7*words + rp_words)*sizeof(Index)));
-  Index* arrays = reinterpret_cast<Index*>(block + 256);
+  const size_t array = static_cast<size_t>(n)*sizeof(Index);   // bytes of an n-word array
+  ScratchLayout l;
+  const size_t counters = l.place(LGC_NCELLS*sizeof(unsigned long long));
+  const size_t c = l.place(array), in_f = l.place(array), claim = l.place(array);
+  const size_t front0 = l.place(array), front1 = l.place(array), touched = l.place(array);
+  const size_t r_scratch = l.place(array);
+  const size_t zero_rows = l.place(GraphPattern::zeroRowBytes(S));
+  const DeviceBlock block(gbMalloc(l.bytes));
+  const GraphPattern g(S, block.at<Index>(zero_rows));
   LgcArgs args;
   args.n = n;
   args.source = s;
-  args.nnz = S->nvals_;
+  args.nnz = S.nvals_;
   args.alpha = alpha;
   args.eps = eps;
   args.max_rounds = max_rounds;
   args.mode = mode;
   args.switchpoint = switchpoint;
-  args.counters = reinterpret_cast<unsigned long long*>(block);
-  args.c        = reinterpret_cast<float*>(arrays);
-  args.in_f     = arrays + words;
-  args.claim    = arrays + 2*words;
-  args.front[0] = arrays + 3*words;
-  args.front[1] = arrays + 4*words;
-  args.touched  = arrays + 5*words;
-  float* r_scratch = reinterpret_cast<float*>(arrays + 6*words);
-  if (stored) {
-    const bool same = S->sameStructure();
-    args.row_ptr = S->d_csrRowPtr_;                 args.row_ind = S->d_csrColInd_;
-    args.in_ptr = same ? S->d_csrRowPtr_ : S->d_cscColPtr_;
-    args.in_ind = same ? S->d_csrColInd_ : S->d_cscRowInd_;
-  } else {                             // no entries: every list is empty
-    Index* zero_ptr = arrays + 7*words;
-    CUDA_CALL(cudaMemsetAsync(zero_ptr, 0, (static_cast<size_t>(n) + 1)*sizeof(Index),
-                              stream));
-    args.row_ptr = zero_ptr;  args.row_ind = NULL;
-    args.in_ptr = zero_ptr;   args.in_ind = NULL;
-  }
-  CUDA_CALL(cudaMemsetAsync(block, 0, LGC_NCELLS*sizeof(unsigned long long), stream));
+  args.counters = block.at<unsigned long long>(counters);
+  args.c        = block.at<float>(c);
+  args.in_f     = block.at<int>(in_f);
+  args.claim    = block.at<int>(claim);
+  args.front[0] = block.at<Index>(front0);
+  args.front[1] = block.at<Index>(front1);
+  args.touched  = block.at<Index>(touched);
+  args.row_ptr = g.row_ptr;  args.row_ind = g.row_ind;
+  args.in_ptr = g.col_ptr != NULL ? g.col_ptr : g.row_ptr;
+  args.in_ind = g.col_ptr != NULL ? g.col_ind : g.row_ind;
+  CUDA_CALL(cudaMemsetAsync(args.counters, 0, LGC_NCELLS*sizeof(unsigned long long), stream));
 
   CHECK(p->setStorage(GrB_DENSE));
   CHECK(p->dense_.allocateGpu());
@@ -111,12 +79,9 @@ Info lgcRun(Vector<float>* p, Vector<float>* r, const Matrix<a>* A, Index s, dou
     CHECK(r->dense_.allocateGpu());
     args.r = r->dense_.d_val_;
   } else {
-    args.r = r_scratch;
+    args.r = block.at<float>(r_scratch);
   }
-  void* params[] = { &args };
-  CUDA_CALL(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(lgcKernel),
-      dim3(grid), dim3(GB_LGC_NT), params, 0, stream));
-  GB_KERNEL_CHECK();
+  CHECK((launchCooperative<lgcKernel, GB_LGC_NT>(stream, args)));
   clock.Stop();
   p->dense_.touched();
   if (r != NULL) r->dense_.touched();
@@ -126,7 +91,6 @@ Info lgcRun(Vector<float>* p, Vector<float>* r, const Matrix<a>* A, Index s, dou
   runtime().sync();
   if (rounds != NULL) *rounds = static_cast<int>(cells[LGC_ROUNDS]);
   if (stats != NULL) { stats[0] = cells[LGC_PUSHED]; stats[1] = cells[LGC_DENSE]; }
-  gbFree(block);
   if (ms != NULL) *ms = clock.ElapsedMillis();
   return GrB_SUCCESS;
 }
@@ -137,19 +101,19 @@ Info lgcRun(Vector<float>* p, Vector<float>* r, const Matrix<a>* A, Index s, dou
 // is positive, with vol and cut exact 64-bit counts (d = row lengths; cut counts the
 // stored A(i,j) with i in S_k, j not, self-loops never).  cluster = 1 on S_k* for the
 // smallest k* of least phi, else 0, dense; *size = k*, *conductance = phi_k*; when no k
-// qualifies, an empty cluster, *size = 0 and *conductance = NaN.  Refusals as lgcCheck,
-// then cluster the same vector as p (GrB_INVALID_VALUE).
+// qualifies, an empty cluster, *size = 0 and *conductance = NaN.  Refusals: those of
+// graphCheck (with the CSC), then cluster the same vector as p (GrB_INVALID_VALUE).
 // Device work: the keys of U by an atomic append, the stable radix sort of
 // ingest.hpp on them, rank[v], a warp per position counting its neighbours ranked
 // before it, two inclusive 64-bit scans and a two-pass (phi, k) minimum.
 template <typename a>
 Info lgcSweepRun(Vector<float>* cluster, Vector<float>* p, const Matrix<a>* A, int* size,
                  double* conductance, float* ms = NULL) {
-  CHECK(lgcCheck("lgcSweep", cluster, p, A));
+  CHECK(graphCheck("lgcSweep", A, true, cluster, p));
   if (cluster == p) return GrB_INVALID_VALUE;
-  const SparseMatrix<a>* S = &A->sparse_;
-  const Index n = S->nrows_;
-  const long long nnz = S->nvals_;
+  const SparseMatrix<a>& S = A->sparse_;
+  const Index n = S.nrows_;
+  const long long nnz = S.nvals_;
   GpuTimer clock;
   clock.Start();
   if (size != NULL) *size = 0;
@@ -168,27 +132,22 @@ Info lgcSweepRun(Vector<float>* cluster, Vector<float>* p, const Matrix<a>* A, i
     return GrB_SUCCESS;
   }
   const float* pv = p_type != GrB_UNKNOWN ? p->dense_.d_val_ : NULL;
-  const bool stored = nnz > 0;
-  const bool same = S->sameStructure();
   const size_t nn = static_cast<size_t>(n);
-  Index* zero_ptr = NULL;
-  if (!stored) {
-    zero_ptr = static_cast<Index*>(gbMalloc((nn + 1)*sizeof(Index)));
-    CUDA_CALL(cudaMemsetAsync(zero_ptr, 0, (nn + 1)*sizeof(Index), stream));
-  }
-  const Index* row_ptr = stored ? S->d_csrRowPtr_ : zero_ptr;
-  unsigned long long* cells = static_cast<unsigned long long*>(gbMalloc(
-      4*sizeof(unsigned long long)));
-  unsigned long long* const key_buf[2] = {
-      static_cast<unsigned long long*>(gbMalloc(nn*8)),
-      static_cast<unsigned long long*>(gbMalloc(nn*8))};
-  unsigned long long* keys = key_buf[0];
-  unsigned long long* keys_tmp = key_buf[1];
-  Index* rank = static_cast<Index*>(gbMalloc(nn*sizeof(Index)));
+  ScratchLayout l;
+  const size_t cells_at = l.place(3*sizeof(unsigned long long));   // m, then (phi, k)
+  const size_t keys_at = l.place(nn*8), keys_tmp_at = l.place(nn*8);
+  const size_t rank_at = l.place(nn*sizeof(Index));
+  const size_t zero_rows = l.place(GraphPattern::zeroRowBytes(S));
+  const DeviceBlock block(gbMalloc(l.bytes));
+  const GraphPattern g(S, block.at<Index>(zero_rows));
+  unsigned long long* cells = block.at<unsigned long long>(cells_at);
+  unsigned long long* keys = block.at<unsigned long long>(keys_at);
+  unsigned long long* keys_tmp = block.at<unsigned long long>(keys_tmp_at);
+  Index* rank = block.at<Index>(rank_at);
   CUDA_CALL(cudaMemsetAsync(cells, 0, sizeof(unsigned long long), stream));
   CUDA_CALL(cudaMemsetAsync(cells + 1, 0xff, 2*sizeof(unsigned long long), stream));
-  const int g = gridFor(nn, GB_SWEEP_NT);
-  lgcSweepKeysKernel<<<g, GB_SWEEP_NT, 0, stream>>>(pv, row_ptr, n, keys, cells, rank);
+  const int gn = gridFor(nn, GB_SWEEP_NT);
+  lgcSweepKeysKernel<<<gn, GB_SWEEP_NT, 0, stream>>>(pv, g.row_ptr, n, keys, cells, rank);
   GB_KERNEL_CHECK();
   const Index m = static_cast<Index>(runtime().fetch(cells));
   Index best_k = -1;
@@ -201,16 +160,19 @@ Info lgcSweepRun(Vector<float>* cluster, Vector<float>* p, const Matrix<a>* A, i
     GB_KERNEL_CHECK();
     // dcut and dvol in the other key buffer and a fresh one, the scans in place
     long long* dcut = reinterpret_cast<long long*>(keys_tmp);
-    long long* dvol = static_cast<long long*>(gbMalloc(static_cast<size_t>(m)*8));
+    const DeviceBlock dvol_block(gbMalloc(static_cast<size_t>(m)*8));
+    long long* dvol = dvol_block.at<long long>();
     lgcSweepDeltaKernel<<<gridFor(static_cast<size_t>(m)*32, GB_SWEEP_NT), GB_SWEEP_NT, 0,
-                          stream>>>(sorted, m, row_ptr, S->d_csrColInd_,
-        same ? NULL : S->d_cscColPtr_, same ? NULL : S->d_cscRowInd_, rank, dcut, dvol);
+                          stream>>>(sorted, m, g.row_ptr, g.row_ind, g.col_ptr, g.col_ind,
+                                    rank, dcut, dvol);
     GB_KERNEL_CHECK();
     size_t cub_bytes = 0;
     CUDA_CALL(cub::DeviceScan::InclusiveSum(NULL, cub_bytes, dcut, dcut, m, stream));
-    void* cub_tmp = gbMalloc(cub_bytes);
-    CUDA_CALL(cub::DeviceScan::InclusiveSum(cub_tmp, cub_bytes, dcut, dcut, m, stream));
-    CUDA_CALL(cub::DeviceScan::InclusiveSum(cub_tmp, cub_bytes, dvol, dvol, m, stream));
+    const DeviceBlock cub_tmp(gbMalloc(cub_bytes));
+    CUDA_CALL(cub::DeviceScan::InclusiveSum(cub_tmp.at<void>(), cub_bytes, dcut, dcut, m,
+                                            stream));
+    CUDA_CALL(cub::DeviceScan::InclusiveSum(cub_tmp.at<void>(), cub_bytes, dvol, dvol, m,
+                                            stream));
     lgcSweepBestKernel<false><<<gm, GB_SWEEP_NT, 0, stream>>>(dcut, dvol, m, nnz, cells + 1);
     GB_KERNEL_CHECK();
     lgcSweepBestKernel<true><<<gm, GB_SWEEP_NT, 0, stream>>>(dcut, dvol, m, nnz, cells + 1);
@@ -222,15 +184,12 @@ Info lgcSweepRun(Vector<float>* cluster, Vector<float>* p, const Matrix<a>* A, i
       best_k = static_cast<Index>(best[1]);
       std::memcpy(&best_phi, &best[0], sizeof(best_phi));
     }
-    gbFree(cub_tmp);
-    gbFree(dvol);
   }
   const Index members = best_k + 1;    // 0 when no prefix qualifies
-  lgcSweepOutKernel<<<g, GB_SWEEP_NT, 0, stream>>>(rank, n, members, out);
+  lgcSweepOutKernel<<<gn, GB_SWEEP_NT, 0, stream>>>(rank, n, members, out);
   GB_KERNEL_CHECK();
   clock.Stop();
   cluster->dense_.touched();
-  gbFree(key_buf[0]); gbFree(key_buf[1]); gbFree(rank); gbFree(cells); gbFree(zero_ptr);
   if (size != NULL) *size = static_cast<int>(members);
   if (conductance != NULL) *conductance = best_phi;
   if (ms != NULL) *ms = clock.ElapsedMillis();

@@ -19,17 +19,15 @@ namespace backend {
 // vector holds a non-zero value for it (a dense value, or a stored sparse entry).  The
 // candidate vector is read in the storage it has, never converted, and read completely
 // before v is written, so it may be v itself.
-// Every refusal comes before v is touched: A not square, or v or the candidates not of
-// size nrows(A) (GrB_DIMENSION_MISMATCH), a dense A (GrB_NOT_IMPLEMENTED), an A without
-// a device CSR, or a non-symmetric A without a device CSC (GrB_UNINITIALIZED_OBJECT).
+// Refusals, before v is touched: those of graphCheck (with the CSC) for v and the
+// candidates, then candidates without device arrays (GrB_UNINITIALIZED_OBJECT).
 template <typename W, typename a>
 Info misRun(Vector<W>* v, const Matrix<a>* A, unsigned int seed,
             const Vector<W>* candidates, int* nmembers, float* ms = NULL) {
   static_assert(std::is_same<W, int>::value || std::is_same<W, float>::value,
                 "mis writes int or float vectors");
   Vector<W>* cand = const_cast<Vector<W>*>(candidates);    // read only
-  const Info refused = greedyCheck("mis", v, A, cand);
-  if (refused != GrB_SUCCESS) return refused;
+  CHECK(graphCheck("mis", A, true, v, cand));
   const Index n = A->sparse_.nrows_;
 
   // the candidates as device arrays, in the storage they have

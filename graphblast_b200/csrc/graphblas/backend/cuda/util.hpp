@@ -245,6 +245,32 @@ inline void gbFree(void* p) {
   if (p != NULL) (void)cudaFreeAsync(p, runtime().stream);
 }
 
+// Owner of one gbMalloc block (or of NULL): gbFree'd when the owner goes out of scope,
+// on every return path.
+class DeviceBlock {
+ public:
+  explicit DeviceBlock(void* p) : p_(static_cast<unsigned char*>(p)) {}
+  ~DeviceBlock() { gbFree(p_); }
+  DeviceBlock(const DeviceBlock&) = delete;
+  DeviceBlock& operator=(const DeviceBlock&) = delete;
+  // The array at byte offset `off` of the block.
+  template <typename T> T* at(size_t off = 0) const { return reinterpret_cast<T*>(p_ + off); }
+
+ private:
+  unsigned char* p_;
+};
+
+// Arrays placed one after another in one device block, each on a 256-byte boundary:
+// place() returns an array's byte offset, `bytes` is the size of the block so far.
+struct ScratchLayout {
+  size_t bytes = 0;
+  size_t place(size_t array_bytes) {
+    const size_t off = bytes;
+    bytes += (array_bytes + 255)/256*256;
+    return off;
+  }
+};
+
 // Copy of count elements on the backend stream; none for an empty count, a NULL
 // end or a copy of an array onto itself.
 template <typename X>
@@ -253,18 +279,25 @@ void copyAsync(X* dst, const X* src, size_t count, cudaMemcpyKind kind) {
     CUDA_CALL(cudaMemcpyAsync(dst, src, count*sizeof(X), kind, gbStream()));
 }
 
-// CTAs of NT threads of the cooperative kernel K that fit on the device at once: the
-// grid of its cooperative launch.  The occupancy query runs on the first call and is
-// cached per kernel; 0 when no CTA fits.
-template <auto K, int NT>
-int cooperativeGrid() {
+// One cooperative launch of kernel K, CTAs of NT threads, with K's arguments, on
+// `stream`.  The grid is every CTA of K that fits on the device at once; the occupancy
+// query runs on K's first launch and is cached.  GrB_PANIC when no CTA fits.
+template <auto K, int NT, typename... Args>
+Info launchCooperative(cudaStream_t stream, Args... args) {
+  static_assert(std::is_same<decltype(K), void (*)(Args...)>::value,
+                "the arguments must have the kernel's parameter types");
   static int resident = 0;
   if (resident == 0) {
     int per_sm = 0;
     CUDA_CALL(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, K, NT, 0));
     resident = per_sm*runtime().sm_count;
   }
-  return resident;
+  if (resident < 1) return GrB_PANIC;
+  void* params[] = { &args... };
+  CUDA_CALL(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(K), dim3(resident), dim3(NT),
+                                        params, 0, stream));
+  GB_KERNEL_CHECK();
+  return GrB_SUCCESS;
 }
 
 // Grid sizing helper: a grid-stride launch sized in whole waves of the SM count.

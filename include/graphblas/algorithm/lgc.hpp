@@ -20,8 +20,8 @@
 // cooperative kernel.
 //   Refusals, p and r untouched: NULL p, A or desc (GrB_UNINITIALIZED_OBJECT); s out
 // of range (GrB_INVALID_INDEX); alpha outside (0, 1] or eps not > 0, NaN included
-// (GrB_INVALID_VALUE); then those of backend::lgcCheck (a dense A, then sizes, then a
-// missing CSC); r the same vector as p (GrB_INVALID_VALUE).
+// (GrB_INVALID_VALUE); then those of backend::graphCheck (a dense A, then sizes, then a
+// missing CSR or CSC); r the same vector as p (GrB_INVALID_VALUE).
 //
 // lgcSweep: the sweep cut of p, the cluster a user of local clustering wants.  The
 // support {v : p[v] > 0 and d[v] > 0} ordered by p[v]/d[v] descending (fp32, ties by
@@ -51,14 +51,10 @@ float lgc(Vector<float>* p, Vector<float>* r, const Matrix<a>* A, Index s, doubl
   if (s < 0 || s >= n) GB_ALGO_STEP(GrB_INVALID_INDEX);
   if (!(alpha > 0.0 && alpha <= 1.0) || !(eps > 0.0)) GB_ALGO_STEP(GrB_INVALID_VALUE);
   backend::Descriptor& d = desc->descriptor_;
-  Desc_value mode;
-  GB_ALGO_STEP(desc->get(GrB_MXVMODE, &mode));
   int count = 0;
   float ms = 0.f;
   GB_ALGO_STEP(backend::lgcRun(&p->vector_, r != NULL ? &r->vector_ : NULL, &A->matrix_, s,
-      alpha, eps, d.max_niter_,
-      mode == GrB_PUSHONLY ? 1 : (mode == GrB_PULLONLY ? 2 : 0), d.switchpoint(),
-      &count, &ms));
+      alpha, eps, d.max_niter_, d.mxvRoute(), d.switchpoint(), &count, &ms));
   if (rounds != NULL) *rounds = count;
   if (d.timing_ > 0) std::cout << "lgc, " << count << " rounds, " << ms << "\n";
   return ms;

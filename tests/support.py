@@ -277,6 +277,15 @@ def launch_count(gb):
     return out.value
 
 
+def launches_per_call(gb, call):
+    """The kernel launches of call(), after one call that lets its vectors take their
+    storage and fills its caches."""
+    call()
+    before = launch_count(gb)
+    call()
+    return launch_count(gb) - before
+
+
 def bfs_pull_model():
     """tools/bfs_pull_model.py, loaded as a module."""
     spec = importlib.util.spec_from_file_location(

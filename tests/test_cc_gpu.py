@@ -20,8 +20,8 @@ import numpy as np
 import pytest
 
 import oracle_binding as orc
-from support import (check_structure, components, directed_csr, gb, make_matrix, mtx_graph,
-                     symmetric_csr)
+from support import (check_structure, components, directed_csr, gb, launches_per_call,
+                     make_matrix, mtx_graph, symmetric_csr)
 
 pytestmark = pytest.mark.gpu
 
@@ -354,6 +354,19 @@ def test_reused_vector_and_repeated_calls(gb):
     for _ in range(3):
         k, _ = algorithm.cc(v, A, gb.Descriptor())
         assert np.array_equal(v.extractTuples().astype(np.int64), want) and k == want_k
+
+
+@pytest.mark.parametrize("graph", ["rmat", "no_entries"])
+def test_launches_per_call(gb, graph):
+    """One cooperative launch per call."""
+    from graphblast_b200 import algorithm
+    if graph == "rmat":
+        rp, ci = orc.rmat_csr(14)
+        A, n = make_matrix(gb, rp, ci), len(rp) - 1
+    else:
+        A, n = gb.Matrix(1000, 1000), 1000
+    v = gb.Vector(n)
+    assert launches_per_call(gb, lambda: algorithm.cc(v, A, gb.Descriptor())) == 1
 
 
 def test_largest_float_size(gb):

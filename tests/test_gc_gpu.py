@@ -12,8 +12,8 @@ import pytest
 
 import greedy_oracle
 import oracle_binding as orc
-from support import (gb, make_matrix, mtx_graph, path_graph, ragged_graph, star_graph,
-                     symmetric_csr)
+from support import (gb, launches_per_call, make_matrix, mtx_graph, path_graph, ragged_graph,
+                     star_graph, symmetric_csr)
 
 pytestmark = pytest.mark.gpu
 
@@ -165,6 +165,19 @@ def test_same_call_twice_is_identical_and_seeds_differ(gb):
     rows = np.repeat(np.arange(n), np.diff(rp))
     for c in (a1, b):
         assert not np.any(c[rows] == c[ci])
+
+
+@pytest.mark.parametrize("graph", ["rmat", "no_entries"])
+def test_launches_per_call(gb, graph):
+    """One cooperative launch per call; zeroing the colours is no launch."""
+    from graphblast_b200 import algorithm
+    if graph == "rmat":
+        rp, ci = orc.rmat_csr(14)
+        A, n = make_matrix(gb, rp, ci), len(rp) - 1
+    else:
+        A, n = gb.Matrix(1000, 1000), 1000
+    v = gb.Vector(n)
+    assert launches_per_call(gb, lambda: algorithm.gc(v, A, 0, gb.Descriptor())) == 1
 
 
 def test_refusals_leave_v_unchanged(gb):

@@ -21,8 +21,8 @@ import pytest
 
 import lgc_reference as L
 import oracle_binding as orc
-from support import (Csr, csr, device_matrix, directed_csr, gb, make_matrix, mtx_graph,
-                     path_graph, star_graph)
+from support import (Csr, csr, device_matrix, directed_csr, gb, launches_per_call,
+                     make_matrix, mtx_graph, path_graph, star_graph)
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
@@ -232,6 +232,26 @@ def test_without_residual(gb):
     for mode in MODES:
         p, _, k = _run(gb, A, len(rp) - 1, 0, 0.15, 1e-6, mode=mode, residual=False)
         assert k == want_k and np.array_equal(_bits(p), _bits(want_p))
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("graph", ["rmat", "no_entries"])
+def test_launches_per_call(gb, graph):
+    """The push is one cooperative launch.  The sweep of a support of more than one
+    vertex runs the keys, the radix sort's eight 8-bit passes, the ranks, the deltas,
+    the two passes of the minimum and the out pass; with no support, the keys and the
+    out pass."""
+    from graphblast_b200 import algorithm
+    if graph == "rmat":
+        rp, ci = orc.rmat_csr(14)
+        A, n, s, sweep = make_matrix(gb, rp, ci), len(rp) - 1, int(np.argmax(np.diff(rp))), 38
+    else:
+        A, n, s, sweep = gb.Matrix(1000, 1000), 1000, 0, 2
+    p, r, cluster = gb.Vector(n), gb.Vector(n), gb.Vector(n)
+    assert launches_per_call(gb, lambda: algorithm.lgc(
+        p, A, s, 0.15, 1e-6, gb.Descriptor(), residual=r)) == 1
+    assert launches_per_call(
+        gb, lambda: algorithm.lgc_sweep(cluster, p, A, gb.Descriptor())) == sweep
 
 
 # ---------------------------------------------------------------------------

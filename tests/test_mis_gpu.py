@@ -13,8 +13,8 @@ import pytest
 
 import greedy_oracle
 import oracle_binding as orc
-from support import (gb, make_matrix, mtx_graph, path_graph, ragged_graph, star_graph,
-                     symmetric_csr)
+from support import (gb, launches_per_call, make_matrix, mtx_graph, path_graph, ragged_graph,
+                     star_graph, symmetric_csr)
 
 pytestmark = pytest.mark.gpu
 
@@ -244,6 +244,29 @@ def test_candidates_aliased_with_v(gb, storage):
     got, k = run_mis(gb, A, n, 5, v, v=v)
     want, want_k, _ = greedy_oracle.mis(rp, ci, 5, cand)
     assert np.array_equal(got, want.astype(np.float32)) and k == want_k
+
+
+@pytest.mark.parametrize("graph", ["rmat", "no_entries"])
+@pytest.mark.parametrize("candidates,launches", [("none", 1), ("dense", 2), ("sparse", 3)])
+def test_launches_per_call(gb, graph, candidates, launches):
+    """The init pass (none for no candidates, one pass over dense ones, a fill and a
+    scatter for sparse ones) and one cooperative launch."""
+    from graphblast_b200 import algorithm
+    if graph == "rmat":
+        rp, ci = orc.rmat_csr(14)
+        A, n = make_matrix(gb, rp, ci), len(rp) - 1
+    else:
+        A, n = gb.Matrix(1000, 1000), 1000
+    c = None
+    if candidates != "none":
+        c = gb.Vector(n)
+        if candidates == "dense":
+            c.build((np.arange(n) % 3 != 0).astype(np.float32))
+        else:
+            c.build(np.arange(0, n, 3, dtype=np.int32), np.ones((n + 2)//3, np.float32))
+    v = gb.Vector(n)
+    assert launches_per_call(
+        gb, lambda: algorithm.mis(v, A, 0, gb.Descriptor(), c)) == launches
 
 
 # ---------------------------------------------------------------------------
