@@ -8,7 +8,7 @@ reference's own tests.
 from .api import (  # noqa: F401
     GraphBLASError, Info, Storage, Desc_field, Desc_value,
     Descriptor, Matrix, Vector,
-    vxm, mxv, mxm, eWiseAdd, eWiseMult, transpose, assign, reduce,
+    vxm, mxv, mxm, eWiseAdd, eWiseMult, transpose, extract, assign, reduce,
     Semiring, Monoid,
     LogicalOrAndSemiring, PlusMultipliesSemiring, MinimumPlusSemiring,
     MaximumMultipliesSemiring, PlusDividesSemiring, PlusGreaterSemiring,

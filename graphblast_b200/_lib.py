@@ -128,6 +128,14 @@ LGC_SIGNATURES = [
     ("gb200_lgc_sweep", _I, [_P, _P, _P, _P, _IP, C.POINTER(_D), C.POINTER(_F)]),
 ]
 
+# (name, restype, argtypes) for every symbol declared in include/graphblast_b200_extract.h,
+# the companion header of extract; load() binds these too.
+EXTRACT_SIGNATURES = [
+    ("gb200_extract_matrix", _I, [_P, _P, _P, _P, _I, _P, _I, _P]),
+    ("gb200_extract_column", _I, [_P, _P, _P, _P, _I, _I, _P]),
+    ("gb200_extract_vector", _I, [_P, _P, _P, _P, _I, _P]),
+]
+
 
 class ExtensionMissing(RuntimeError):
     pass
@@ -144,7 +152,7 @@ def load():
             "`python -c 'import __graft_entry__ as g; g.build()'`; "
             "there is no CPU fallback." % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
-    for name, restype, argtypes in SIGNATURES + LGC_SIGNATURES:
+    for name, restype, argtypes in SIGNATURES + LGC_SIGNATURES + EXTRACT_SIGNATURES:
         fn = getattr(lib, name)   # AttributeError if a declared symbol is missing
         fn.restype = restype
         fn.argtypes = argtypes

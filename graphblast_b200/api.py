@@ -579,6 +579,48 @@ def transpose(C_, mask, accum, A, desc):
            "transpose")
 
 
+def _indices(lst, n):
+    """A host int32 array of an index list of at least n entries (kept alive by the
+    caller), or None for GrB_ALL."""
+    if lst is None:
+        return None
+    arr = np.ascontiguousarray(lst, dtype=np.int32).reshape(-1)
+    if len(arr) < int(n):
+        raise ValueError("extract: an index list of %d entries for a count of %d" % (
+            len(arr), int(n)))
+    return arr
+
+
+def _ptr_or_null(arr):
+    return None if arr is None else _ptr(arr)
+
+
+def extract(out, mask, accum, src, rows, nrows, cols_or_col, ncols, desc):
+    """Submatrix, column or subvector extract, in the reference's argument order.
+
+    Matrix out: out = op(src)(rows, cols), cols_or_col a list, out nrows x ncols.
+    Vector out, Matrix src: out = op(src)(rows, col), cols_or_col the column; ncols
+    is ignored.  Vector out, Vector src: out = src(rows), of size nrows; cols_or_col
+    and ncols are ignored.  op(src) is src' when desc's GrB_INP0 is GrB_TRAN.  None
+    means GrB_ALL; lists are any int sequence or numpy array, sent as int32.  out is
+    replaced: accum is not applied."""
+    lib = _lib.load()
+    r = _indices(rows, nrows)
+    if isinstance(out, Matrix):
+        c = _indices(cols_or_col, ncols)
+        _check(lib.gb200_extract_matrix(out._h, _h(mask), src._h, _ptr_or_null(r),
+                                        int(nrows), _ptr_or_null(c), int(ncols), desc._h),
+               "extract(matrix)")
+    elif isinstance(src, Matrix):
+        _check(lib.gb200_extract_column(out._h, _h(mask), src._h, _ptr_or_null(r), int(nrows),
+                                        int(cols_or_col), desc._h),
+               "extract(column)")
+    else:
+        _check(lib.gb200_extract_vector(out._h, _h(mask), src._h, _ptr_or_null(r), int(nrows),
+                                        desc._h),
+               "extract(vector)")
+
+
 def assign(w, mask, accum, val, indices, nindices, desc):
     if indices is not None:
         raise GraphBLASError(Info.GrB_NOT_IMPLEMENTED, "assign(indices)")

@@ -31,6 +31,7 @@
 
 #include "graphblast_b200.h"
 #include "graphblast_b200_lgc.h"
+#include "graphblast_b200_extract.h"
 
 bool debug_;
 bool memory_;
@@ -139,6 +140,18 @@ template <typename T> T elementOf(const graphblas::Matrix<T>*);
 // f(M) with A's typed matrix M, a graphblas::Matrix<float>* or Matrix<int>*.
 template <typename F>
 auto onMatrix(gb200_matrix_t A, F&& f) { return A->f != NULL ? f(A->f) : f(A->i); }
+
+// A host index list of the extract entries as the frontend takes it: NULL stays
+// GrB_ALL.
+struct HostIndices {
+  std::vector<graphblas::Index> v;
+  const std::vector<graphblas::Index>* list;
+  HostIndices(const int* h, int n) : v(h != NULL ? h : NULL, h != NULL ? h + n : NULL),
+                                     list(h != NULL ? &v : NULL) {}
+};
+
+template <typename T>
+bool denseMatrix(const graphblas::Matrix<T>* M) { return !M->matrix_.isSparse(); }
 
 // Every given handle holds FP32 (allFp32) or INT32 (allInt32) values; NULL, an
 // absent mask, matches either.
@@ -1151,6 +1164,54 @@ int gb200_lgc_sweep(gb200_vector_t cluster, gb200_vector_t p, gb200_matrix_t A,
   if (info == 0 && size) *size = members;
   if (info == 0 && conductance) *conductance = phi;
   return info;
+}
+
+// ---- extract (include/graphblast_b200_extract.h) -------------------------------
+
+int gb200_extract_matrix(gb200_matrix_t C, gb200_matrix_t mask, gb200_matrix_t A,
+                         const int* h_rows, int nrows, const int* h_cols, int ncols,
+                         gb200_desc_t desc) {
+  if (C == NULL || A == NULL || desc == NULL)
+    return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
+  if (nrows < 1 || ncols < 1) return rc(graphblas::GrB_INVALID_VALUE);
+  if (!allFp32(C, A) && !allInt32(C, A)) return rc(graphblas::GrB_DOMAIN_MISMATCH);
+  GB200_REQUIRE_DEVICE();
+  if (mask != NULL || onMatrix(A, [](auto M) { return denseMatrix(M); }))
+    return rc(graphblas::GrB_NOT_IMPLEMENTED);
+  const HostIndices rows(h_rows, nrows), cols(h_cols, ncols);
+  if (A->f != NULL)
+    return rc((graphblas::extract<float, float, float>(C->f,
+        static_cast<graphblas::Matrix<float>*>(NULL), GrB_NULL, A->f, rows.list, nrows,
+        cols.list, ncols, &desc->desc)));
+  return rc((graphblas::extract<int, int, int>(C->i, static_cast<graphblas::Matrix<int>*>(NULL),
+      GrB_NULL, A->i, rows.list, nrows, cols.list, ncols, &desc->desc)));
+}
+
+int gb200_extract_column(gb200_vector_t w, gb200_vector_t mask, gb200_matrix_t A,
+                         const int* h_rows, int nrows, int col, gb200_desc_t desc) {
+  if (w == NULL || A == NULL || desc == NULL)
+    return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
+  if (nrows < 1) return rc(graphblas::GrB_INVALID_VALUE);
+  if (A->f == NULL) return rc(graphblas::GrB_DOMAIN_MISMATCH);
+  GB200_REQUIRE_DEVICE();
+  if (mask != NULL || denseMatrix(A->f)) return rc(graphblas::GrB_NOT_IMPLEMENTED);
+  const HostIndices rows(h_rows, nrows);
+  return rc((graphblas::extract<float, float, float>(w->f,
+      static_cast<graphblas::Vector<float>*>(NULL), GrB_NULL, A->f, rows.list, nrows, col,
+      &desc->desc)));
+}
+
+int gb200_extract_vector(gb200_vector_t w, gb200_vector_t mask, gb200_vector_t u,
+                         const int* h_ind, int nind, gb200_desc_t desc) {
+  if (w == NULL || u == NULL || desc == NULL)
+    return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
+  if (nind < 1) return rc(graphblas::GrB_INVALID_VALUE);
+  GB200_REQUIRE_DEVICE();
+  if (mask != NULL) return rc(graphblas::GrB_NOT_IMPLEMENTED);
+  const HostIndices ind(h_ind, nind);
+  return rc((graphblas::extract<float, float, float>(w->f,
+      static_cast<graphblas::Vector<float>*>(NULL), GrB_NULL, u->f, ind.list, nind,
+      &desc->desc)));
 }
 
 int gb200_pr(gb200_vector_t p, gb200_matrix_t A, float alpha, float eps,

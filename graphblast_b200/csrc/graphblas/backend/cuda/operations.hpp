@@ -33,6 +33,7 @@
 #include "graphblas/backend/cuda/ewiseadd.hpp"
 #include "graphblas/backend/cuda/ewisemult.hpp"
 #include "graphblas/backend/cuda/ewise_matrix.hpp"
+#include "graphblas/backend/cuda/extract.hpp"
 #include "graphblas/backend/cuda/assign.hpp"
 #include "graphblas/backend/cuda/reduce.hpp"
 #include "graphblas/backend/cuda/apply.hpp"
@@ -92,7 +93,6 @@ Info settle(const Vector<X>* x, Rest... rest) {
   template <typename... Named, typename... Args>                            \
   Info name(Args... args) { return notBuilt(what); }
 
-GB_DECLARED_ONLY(extract,           "extract of a vector")
 GB_DECLARED_ONLY(assignIndexed,     "assignIndexed")
 GB_DECLARED_ONLY(traceMxmTranspose, "traceMxmTranspose")
 GB_DECLARED_ONLY(applyVxm,          "applyVxm")
@@ -377,6 +377,48 @@ template <typename TC, typename TA, typename TB, typename TMask,
 Info eWiseAdd(Matrix<TC>* C, const Matrix<TMask>* mask, AccumT accum, SemiringT op,
     const Matrix<TA>* A, const Matrix<TB>* B, Descriptor* desc) {
   return ewiseMatrixDispatch<true>(C, mask, op, A, B, desc);
+}
+
+// ---- extract (extract.hpp) --------------------------------------------------------
+// Host index lists, NULL = GrB_ALL.  A mask and a dense matrix are refused before
+// anything changes; a dense C turns sparse only once the result has replaced it.
+
+// C = op(A)(I, J); C may be A.
+template <typename TC, typename TMask, typename TA, typename AccumT>
+Info extract(Matrix<TC>* C, const Matrix<TMask>* mask, AccumT accum, const Matrix<TA>* A,
+    const std::vector<Index>* row_indices, Index nrows,
+    const std::vector<Index>* col_indices, Index ncols, Descriptor* desc) {
+  if (mask != NULL) return notBuilt("masked extract");
+  if (!A->isSparse()) return notBuilt("extract from a dense matrix");
+  Desc_value inp0_mode;
+  CHECK(desc->get(GrB_INP0, &inp0_mode));
+  const bool was_dense = C->isDense();
+  if (!was_dense) CHECK(C->setStorage(GrB_SPARSE));
+  const Info info = extractMatrix(&C->sparse_, &A->sparse_, inp0_mode == GrB_TRAN,
+      row_indices, nrows, col_indices, ncols);
+  if (info == GrB_SUCCESS && was_dense) CHECK(C->setStorage(GrB_SPARSE));
+  return info;
+}
+
+// w = op(A)(I, j), sparse.
+template <typename TW, typename TMask, typename TA, typename AccumT>
+Info extract(Vector<TW>* w, const Vector<TMask>* mask, AccumT accum, const Matrix<TA>* A,
+    const std::vector<Index>* row_indices, Index nrows, Index col_index, Descriptor* desc) {
+  if (mask != NULL) return notBuilt("masked extract");
+  if (!A->isSparse()) return notBuilt("extract from a dense matrix");
+  Desc_value inp0_mode;
+  CHECK(desc->get(GrB_INP0, &inp0_mode));
+  CHECK(settle(w));
+  return extractColumn(w, &A->sparse_, inp0_mode == GrB_TRAN, row_indices, nrows, col_index);
+}
+
+// w = u(I): dense for a dense u, sparse for a sparse u.
+template <typename TW, typename TMask, typename TU, typename AccumT>
+Info extract(Vector<TW>* w, const Vector<TMask>* mask, AccumT accum, const Vector<TU>* u,
+    const std::vector<Index>* indices, Index nindices, Descriptor* desc) {
+  if (mask != NULL) return notBuilt("masked extract");
+  CHECK(settle(w));
+  return extractVector(w, u, indices, nindices);
 }
 
 // C = Aᵀ (C = A when GrB_INP0 is GrB_TRAN); C may be A.

@@ -163,8 +163,11 @@ class SparseMatrix {
   void dropDerived();
   // The contents replaced by a computed CSR of nnz entries in fresh arrays, which
   // this object takes (with cscptr != NULL, a ready CSC of the same entries too).
+  // symmetric: the entry set is symmetric; the CSC index arrays are the CSR's and
+  // cscval (needed when the format keeps a CSC) holds the column-major values.
   void replaceDevice(Index nnz, Index* rowptr, Index* colind, T* val,
-      Index* cscptr = NULL, Index* cscind = NULL, T* cscval = NULL);
+      Index* cscptr = NULL, Index* cscind = NULL, T* cscval = NULL,
+      bool symmetric = false);
   // The entry set stopped being symmetric (tril): from the next upload on the
   // column-major side owns its index arrays instead of borrowing the CSR's.
   void dropSymmetry() { if (symmetric_) { releaseDevice(); symmetric_ = false; } }
@@ -343,12 +346,13 @@ Info SparseMatrix<T>::dup(const SparseMatrix* rhs) {
 
 // The old arrays, and every cache built on them, go first: stream-ordered after the
 // kernels queued so far, which may still read them through an operand that is this
-// matrix.  Then the CSC, when the format keeps one, is the one given or is built
-// here; a given one is freed when the format is CSR-only.  Nothing is known about
-// the result's symmetry, and the host mirrors follow lazily.
+// matrix.  Then the CSC, when the format keeps one, is the one given, the CSR's
+// index arrays with the given values (symmetric), or is built here; what is given
+// is freed when the format is CSR-only.  Unless the caller says so nothing is
+// known about the result's symmetry.  The host mirrors follow lazily.
 template <typename T>
 void SparseMatrix<T>::replaceDevice(Index nnz, Index* rowptr, Index* colind, T* val,
-    Index* cscptr, Index* cscind, T* cscval) {
+    Index* cscptr, Index* cscind, T* cscval, bool symmetric) {
   clear();
   d_csrRowPtr_ = rowptr;
   d_csrColInd_ = colind;
@@ -356,7 +360,11 @@ void SparseMatrix<T>::replaceDevice(Index nnz, Index* rowptr, Index* colind, T* 
   csr_ownership_ = true;
   nvals_ = nnz;
   ncapacity_ = nnz;
-  symmetric_ = false;
+  symmetric_ = symmetric;
+  if (symmetric) {
+    cscptr = rowptr;
+    cscind = colind;
+  }
   if (format_ == GrB_SPARSE_MATRIX_CSRCSC) {
     if (cscptr == NULL)
       ingestCsrToCsc<T>(nrows_, ncols_, nnz, rowptr, colind, val, &cscptr, &cscind, &cscval);
@@ -366,8 +374,9 @@ void SparseMatrix<T>::replaceDevice(Index nnz, Index* rowptr, Index* colind, T* 
     csc_ownership_ = true;
     cscval_ownership_ = true;
     csc_initialized_ = true;
-  } else if (cscptr != NULL) {
-    gbFree(cscptr); gbFree(cscind); gbFree(cscval);
+  } else {
+    if (cscptr != NULL && !symmetric) { gbFree(cscptr); gbFree(cscind); }
+    if (cscval != NULL) gbFree(cscval);
   }
   csr_initialized_ = true;
   need_update_ = true;

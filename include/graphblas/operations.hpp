@@ -452,25 +452,58 @@ Info extractGather(Vector<TW>* w, const Vector<TMask>* mask, AccumT accum,
   return backend::extractGather(raw(w), raw(mask), accum, raw(u), raw(indices), raw(desc));
 }
 
-// ---- declared by the reference, implemented nowhere -------------------------------------
+// ---- extract ---------------------------------------------------------------------------
+// Host index lists; GrB_ALL (NULL) means every index of that extent.  C (or w) is
+// replaced: accum is not applied.  The backend refuses an index out of range
+// (GrB_INVALID_INDEX) before anything changes.
 
+// w<mask> = u(indices)
 template <typename TW, typename TMask, typename TU, typename AccumT>
 Info extract(Vector<TW>* w, const Vector<TMask>* mask, AccumT accum, const Vector<TU>* u,
              const std::vector<Index>* indices, Index nindices, Descriptor* desc) {
-  return ops_detail::declaredOnly("extract vector variant");
+  using namespace ops_detail;
+  GB_REQUIRE(w, u, desc);
+  GB_SHAPES(Contract()
+      .equal(sizeOf(w), Extent{nindices, true}, "w.size != nindices")
+      .equal(sizeOf(w), sizeOf(mask), "w.size != mask.size"));
+  return backend::extract(raw(w), raw(mask), accum, raw(u), indices, nindices, raw(desc));
 }
+
+// C<mask> = op(A)(row_indices, col_indices), op(A) = Aᵀ when GrB_INP0 is GrB_TRAN
 template <typename TC, typename TMask, typename TA, typename AccumT>
 Info extract(Matrix<TC>* C, const Matrix<TMask>* mask, AccumT accum, const Matrix<TA>* A,
              const std::vector<Index>* row_indices, Index nrows,
              const std::vector<Index>* col_indices, Index ncols, Descriptor* desc) {
-  return ops_detail::declaredOnly("extract matrix variant");
+  using namespace ops_detail;
+  GB_REQUIRE(C, A, desc);
+  GB_SHAPES(Contract()
+      .equal(rowsOf(C), Extent{nrows, true}, "C.nrows != nrows")
+      .equal(colsOf(C), Extent{ncols, true}, "C.ncols != ncols")
+      .alike(C, mask, "C.nrows != mask.nrows", "C.ncols != mask.ncols"));
+  return backend::extract(raw(C), raw(mask), accum, raw(A), row_indices, nrows, col_indices,
+                          ncols, raw(desc));
 }
+
+// w<mask> = op(A)(row_indices, col_index), op(A) = Aᵀ when GrB_INP0 is GrB_TRAN
 template <typename TW, typename TMask, typename TA, typename AccumT>
 Info extract(Vector<TW>* w, const Vector<TMask>* mask, AccumT accum, const Matrix<TA>* A,
              const std::vector<Index>* row_indices, Index nrows, Index col_index,
              Descriptor* desc) {
-  return ops_detail::declaredOnly("extract matrix variant");
+  using namespace ops_detail;
+  GB_REQUIRE(w, A, desc);
+  Desc_value inp0;
+  CHECK(desc->get(GrB_INP0, &inp0));
+  GB_SHAPES(Contract()
+      .equal(sizeOf(w), Extent{nrows, true}, "w.size != nrows")
+      .atMost(Extent{col_index + 1, true}, inp0 == GrB_TRAN ? rowsOf(A) : colsOf(A),
+              "col_index >= op(A).ncols")
+      .equal(sizeOf(w), sizeOf(mask), "w.size != mask.size"));
+  return backend::extract(raw(w), raw(mask), accum, raw(A), row_indices, nrows, col_index,
+                          raw(desc));
 }
+
+// ---- declared by the reference, implemented nowhere -------------------------------------
+
 template <typename TC, typename TMask, typename TA, typename AccumT>
 Info assign(Matrix<TC>* C, const Matrix<TMask>* mask, AccumT accum, const Matrix<TA>* A,
             const std::vector<Index>* row_indices, Index nrows,
