@@ -136,6 +136,12 @@ EXTRACT_SIGNATURES = [
     ("gb200_extract_vector", _I, [_P, _P, _P, _P, _I, _P]),
 ]
 
+# (name, restype, argtypes) for every symbol declared in include/graphblast_b200_bc.h,
+# the companion header of betweenness centrality; load() binds these too.
+BC_SIGNATURES = [
+    ("gb200_bc", _I, [_P, _P, _P, _I, _P, C.POINTER(_F)]),
+]
+
 
 class ExtensionMissing(RuntimeError):
     pass
@@ -152,7 +158,8 @@ def load():
             "`python -c 'import __graft_entry__ as g; g.build()'`; "
             "there is no CPU fallback." % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
-    for name, restype, argtypes in SIGNATURES + LGC_SIGNATURES + EXTRACT_SIGNATURES:
+    for name, restype, argtypes in (SIGNATURES + LGC_SIGNATURES + EXTRACT_SIGNATURES +
+                                    BC_SIGNATURES):
         fn = getattr(lib, name)   # AttributeError if a declared symbol is missing
         fn.restype = restype
         fn.argtypes = argtypes

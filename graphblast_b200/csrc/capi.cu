@@ -28,10 +28,12 @@
 #include "graphblas/algorithm/mis.hpp"
 #include "graphblas/algorithm/cc.hpp"
 #include "graphblas/algorithm/lgc.hpp"
+#include "graphblas/algorithm/bc.hpp"
 
 #include "graphblast_b200.h"
 #include "graphblast_b200_lgc.h"
 #include "graphblast_b200_extract.h"
+#include "graphblast_b200_bc.h"
 
 bool debug_;
 bool memory_;
@@ -1164,6 +1166,26 @@ int gb200_lgc_sweep(gb200_vector_t cluster, gb200_vector_t p, gb200_matrix_t A,
   if (info == 0 && size) *size = members;
   if (info == 0 && conductance) *conductance = phi;
   return info;
+}
+
+// ---- betweenness centrality (include/graphblast_b200_bc.h) ---------------------
+
+int gb200_bc(gb200_vector_t v, gb200_matrix_t A, const int* h_sources, int nsources,
+             gb200_desc_t desc, float* tight_ms) {
+  if (v == NULL || A == NULL || desc == NULL)
+    return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
+  if (A->f == NULL && A->i == NULL) return rc(graphblas::GrB_DOMAIN_MISMATCH);
+  if (nsources < 0) return rc(graphblas::GrB_INVALID_VALUE);
+  int n = 0;
+  onMatrix(A, [&](auto M) { return M->nrows(&n); });
+  if (!graphblas::algorithm::bcSourcesValid(h_sources, nsources, n))
+    return rc(graphblas::GrB_INVALID_INDEX);
+  GB200_REQUIRE_DEVICE();
+  return runAlgorithm(tight_ms, [&] {
+    return onMatrix(A, [&](auto M) {
+      return graphblas::algorithm::bc(v->f, M, h_sources, nsources, &desc->desc);
+    });
+  });
 }
 
 // ---- extract (include/graphblast_b200_extract.h) -------------------------------

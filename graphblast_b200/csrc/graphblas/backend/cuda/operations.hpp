@@ -43,6 +43,7 @@
 #include "graphblas/backend/cuda/mis.hpp"
 #include "graphblas/backend/cuda/cc.hpp"
 #include "graphblas/backend/cuda/lgc.hpp"
+#include "graphblas/backend/cuda/bc.hpp"
 
 namespace graphblas {
 namespace backend {
