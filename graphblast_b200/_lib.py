@@ -142,6 +142,15 @@ BC_SIGNATURES = [
     ("gb200_bc", _I, [_P, _P, _P, _I, _P, C.POINTER(_F)]),
 ]
 
+# (name, restype, argtypes) for every symbol declared in include/graphblast_b200_assign.h,
+# the companion header of assign into a matrix; load() binds these too.
+ASSIGN_SIGNATURES = [
+    ("gb200_assign_matrix", _I, [_P, _P, _I, _P, _P, _I, _P, _I, _P]),
+    ("gb200_assign_matrix_scalar", _I, [_P, _P, _I, _D, _P, _I, _P, _I, _P]),
+    ("gb200_assign_column", _I, [_P, _P, _I, _P, _P, _I, _I, _P]),
+    ("gb200_assign_row", _I, [_P, _P, _I, _P, _I, _P, _I, _P]),
+]
+
 
 class ExtensionMissing(RuntimeError):
     pass
@@ -159,7 +168,7 @@ def load():
             "there is no CPU fallback." % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
     for name, restype, argtypes in (SIGNATURES + LGC_SIGNATURES + EXTRACT_SIGNATURES +
-                                    BC_SIGNATURES):
+                                    BC_SIGNATURES + ASSIGN_SIGNATURES):
         fn = getattr(lib, name)   # AttributeError if a declared symbol is missing
         fn.restype = restype
         fn.argtypes = argtypes

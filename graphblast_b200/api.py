@@ -579,15 +579,15 @@ def transpose(C_, mask, accum, A, desc):
            "transpose")
 
 
-def _indices(lst, n):
+def _indices(lst, n, what="extract"):
     """A host int32 array of an index list of at least n entries (kept alive by the
     caller), or None for GrB_ALL."""
     if lst is None:
         return None
     arr = np.ascontiguousarray(lst, dtype=np.int32).reshape(-1)
     if len(arr) < int(n):
-        raise ValueError("extract: an index list of %d entries for a count of %d" % (
-            len(arr), int(n)))
+        raise ValueError("%s: an index list of %d entries for a count of %d" % (
+            what, len(arr), int(n)))
     return arr
 
 
@@ -621,11 +621,60 @@ def extract(out, mask, accum, src, rows, nrows, cols_or_col, ncols, desc):
                "extract(vector)")
 
 
-def assign(w, mask, accum, val, indices, nindices, desc):
-    if indices is not None:
-        raise GraphBLASError(Info.GrB_NOT_IMPLEMENTED, "assign(indices)")
-    _check(_lib.load().gb200_assign_scalar(w._h, _h(mask), float(val), desc._h),
-           "assign")
+NO_ACCUM = -1
+
+
+def _accum_id(accum):
+    """GB200_NO_ACCUM for None, otherwise the monoid's id."""
+    return NO_ACCUM if accum is None else int(Monoid(accum))
+
+
+def assign(out, mask, accum, src, *args):
+    """Vector out: assign(w, mask, accum, val, indices, nindices, desc), w = val
+    everywhere (indices must be None).
+
+    Matrix out, in the reference's argument order (None means GrB_ALL; lists are any
+    int sequence or numpy array, sent as int32, and may not repeat an index):
+      assign(C, mask, accum, A_or_val, rows, nrows, cols, ncols, desc)
+          C(rows, cols) = accum(C(rows, cols), op(A)), op(A) = A' when desc's
+          GrB_INP0 is GrB_TRAN; or the scalar val at every position of the region;
+      assign(C, mask, accum, u, rows, nrows, col, desc)   C(rows, col) = u;
+      assign(C, mask, accum, u, row, cols, ncols, desc)   C(row, cols) = u.
+    accum is None (C's region takes the source's pattern and values; C's entries in
+    the region that the source does not store are deleted) or a Monoid (the union,
+    accum(c, a) where both store an entry)."""
+    lib = _lib.load()
+    if not isinstance(out, Matrix):
+        indices, nindices, desc = args
+        if indices is not None:
+            raise GraphBLASError(Info.GrB_NOT_IMPLEMENTED, "assign(indices)")
+        _check(lib.gb200_assign_scalar(out._h, _h(mask), float(src), desc._h), "assign")
+        return
+    acc = _accum_id(accum)
+    if len(args) == 5:
+        rows, nrows, cols, ncols, desc = args
+        r, c = _indices(rows, nrows, "assign"), _indices(cols, ncols, "assign")
+        if isinstance(src, Matrix):
+            _check(lib.gb200_assign_matrix(out._h, _h(mask), acc, src._h, _ptr_or_null(r),
+                                           int(nrows), _ptr_or_null(c), int(ncols), desc._h),
+                   "assign(matrix)")
+        else:
+            _check(lib.gb200_assign_matrix_scalar(out._h, _h(mask), acc, float(src),
+                                                  _ptr_or_null(r), int(nrows), _ptr_or_null(c),
+                                                  int(ncols), desc._h),
+                   "assign(matrix, scalar)")
+    elif len(args) == 4 and (args[0] is None or not np.isscalar(args[0])):
+        rows, nrows, col, desc = args
+        r = _indices(rows, nrows, "assign")
+        _check(lib.gb200_assign_column(out._h, _h(mask), acc, src._h, _ptr_or_null(r),
+                                       int(nrows), int(col), desc._h), "assign(column)")
+    elif len(args) == 4:
+        row, cols, ncols, desc = args
+        c = _indices(cols, ncols, "assign")
+        _check(lib.gb200_assign_row(out._h, _h(mask), acc, src._h, int(row), _ptr_or_null(c),
+                                    int(ncols), desc._h), "assign(row)")
+    else:
+        raise TypeError("assign: %d arguments after the source" % len(args))
 
 
 def reduce(accum, op, src, desc, out=None):

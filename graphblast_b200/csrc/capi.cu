@@ -34,6 +34,7 @@
 #include "graphblast_b200_lgc.h"
 #include "graphblast_b200_extract.h"
 #include "graphblast_b200_bc.h"
+#include "graphblast_b200_assign.h"
 
 bool debug_;
 bool memory_;
@@ -133,6 +134,16 @@ int withMonoid(int id, Body&& body) {
     default: return rc(GrB_INVALID_VALUE);
   }
 }
+
+// body(accum) with GrB_NULL for GB200_NO_ACCUM, otherwise with the monoid over T
+// of a GB200_*_MONOID id.
+template <typename T, typename Body>
+int withAccum(int id, Body&& body) {
+  if (id == GB200_NO_ACCUM) return body(GrB_NULL);
+  return withMonoid<T>(id, body);
+}
+
+inline bool validAccum(int id) { return id == GB200_NO_ACCUM || (id >= 0 && id < GB200_NMONOIDS); }
 
 graphblas::Vector<float>* vec(gb200_vector_t v) { return v ? v->f : NULL; }
 
@@ -311,6 +322,27 @@ __global__ void rmatEdgesKernel(int scale, long long nedges,
     src[e] = static_cast<int>(s);
     dst[e] = static_cast<int>(d);
   }
+}
+
+// The column (Column) or row form: u along the list, at the column or row `at`.
+template <bool Column>
+int assignVectorEntry(gb200_matrix_t C, gb200_vector_t mask, int accum, gb200_vector_t u,
+                      const int* h_list, int n, int at, gb200_desc_t desc) {
+  if (C == NULL || u == NULL || desc == NULL)
+    return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
+  if (n < 1 || !validAccum(accum)) return rc(graphblas::GrB_INVALID_VALUE);
+  if (C->f == NULL) return rc(graphblas::GrB_DOMAIN_MISMATCH);
+  GB200_REQUIRE_DEVICE();
+  if (mask != NULL || C->f->matrix_.isDense()) return rc(graphblas::GrB_NOT_IMPLEMENTED);
+  const HostIndices list(h_list, n);
+  return withAccum<float>(accum, [&](auto op) {
+    const graphblas::Vector<float>* no_mask = NULL;
+    if (Column)
+      return rc((graphblas::assign<float, float, float>(C->f, no_mask, op, u->f, list.list,
+          n, at, &desc->desc)));
+    return rc((graphblas::assign<float, float, float>(C->f, no_mask, op, u->f, at,
+        list.list, n, &desc->desc)));
+  });
 }
 
 }  // namespace
@@ -1234,6 +1266,67 @@ int gb200_extract_vector(gb200_vector_t w, gb200_vector_t mask, gb200_vector_t u
   return rc((graphblas::extract<float, float, float>(w->f,
       static_cast<graphblas::Vector<float>*>(NULL), GrB_NULL, u->f, ind.list, nind,
       &desc->desc)));
+}
+
+// ---- assign into a matrix (include/graphblast_b200_assign.h) -------------------
+
+int gb200_assign_matrix(gb200_matrix_t C, gb200_matrix_t mask, int accum, gb200_matrix_t A,
+                        const int* h_rows, int nrows, const int* h_cols, int ncols,
+                        gb200_desc_t desc) {
+  if (C == NULL || A == NULL || desc == NULL)
+    return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
+  if (nrows < 1 || ncols < 1 || !validAccum(accum)) return rc(graphblas::GrB_INVALID_VALUE);
+  if (!allFp32(C, A) && !allInt32(C, A)) return rc(graphblas::GrB_DOMAIN_MISMATCH);
+  GB200_REQUIRE_DEVICE();
+  if (mask != NULL || onMatrix(C, [](auto M) { return M->matrix_.isDense(); }) ||
+      onMatrix(A, [](auto M) { return denseMatrix(M); }) ||
+      (C->i != NULL && accum != GB200_NO_ACCUM && accum != GB200_PLUS_MONOID))
+    return rc(graphblas::GrB_NOT_IMPLEMENTED);
+  const HostIndices rows(h_rows, nrows), cols(h_cols, ncols);
+  if (C->f != NULL)
+    return withAccum<float>(accum, [&](auto op) {
+      return rc((graphblas::assign<float, float, float>(C->f,
+          static_cast<graphblas::Matrix<float>*>(NULL), op,
+          static_cast<const graphblas::Matrix<float>*>(A->f), rows.list, nrows, cols.list,
+          ncols, &desc->desc)));
+    });
+  return withAccum<int>(accum, [&](auto op) {
+    return rc((graphblas::assign<int, int, int>(C->i, static_cast<graphblas::Matrix<int>*>(NULL),
+        op, static_cast<const graphblas::Matrix<int>*>(A->i), rows.list, nrows, cols.list,
+        ncols, &desc->desc)));
+  });
+}
+
+int gb200_assign_matrix_scalar(gb200_matrix_t C, gb200_matrix_t mask, int accum, double val,
+                               const int* h_rows, int nrows, const int* h_cols, int ncols,
+                               gb200_desc_t desc) {
+  if (C == NULL || desc == NULL) return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
+  if (nrows < 1 || ncols < 1 || !validAccum(accum)) return rc(graphblas::GrB_INVALID_VALUE);
+  GB200_REQUIRE_DEVICE();
+  if (mask != NULL || onMatrix(C, [](auto M) { return M->matrix_.isDense(); }) ||
+      (C->i != NULL && accum != GB200_NO_ACCUM && accum != GB200_PLUS_MONOID))
+    return rc(graphblas::GrB_NOT_IMPLEMENTED);
+  const HostIndices rows(h_rows, nrows), cols(h_cols, ncols);
+  if (C->f != NULL)
+    return withAccum<float>(accum, [&](auto op) {
+      return rc((graphblas::assign<float, float, float>(C->f,
+          static_cast<graphblas::Matrix<float>*>(NULL), op, static_cast<float>(val), rows.list,
+          nrows, cols.list, ncols, &desc->desc)));
+    });
+  return withAccum<int>(accum, [&](auto op) {
+    return rc((graphblas::assign<int, int, int>(C->i, static_cast<graphblas::Matrix<int>*>(NULL),
+        op, static_cast<int>(val), rows.list, nrows, cols.list, ncols, &desc->desc)));
+  });
+}
+
+int gb200_assign_column(gb200_matrix_t C, gb200_vector_t mask, int accum, gb200_vector_t u,
+                        const int* h_rows, int nrows, int col, gb200_desc_t desc) {
+  return assignVectorEntry<true>(C, mask, accum, u, h_rows, nrows, col, desc);
+}
+
+int gb200_assign_row(gb200_matrix_t C, gb200_vector_t mask, int accum, gb200_vector_t u,
+                     int row, const int* h_cols, int ncols, gb200_desc_t desc) {
+  return assignVectorEntry<false>(C, mask, accum, u, h_cols, ncols, row, desc);
 }
 
 int gb200_pr(gb200_vector_t p, gb200_matrix_t A, float alpha, float eps,

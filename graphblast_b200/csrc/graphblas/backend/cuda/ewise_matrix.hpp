@@ -61,7 +61,7 @@ Info ewiseMatrix(SparseMatrix<c>* C, SemiringT op, const SparseMatrix<a>* A,
   // 1. count: entries of C per tile, per row and in all
   if (ntiles > 0) {
     ewiseMatrixCountKernel<IsAdd><<<static_cast<unsigned int>(ntiles), GB_EWM_NT, 0, s>>>(
-        Av.ptr, Av.ind, Bv.ptr, Bv.ind, m, total, tiles, rowptr, count);
+        Av.ptr, Av.ind, Bv.ptr, Bv.ind, m, total, tiles, rowptr, count, EwmKeepAll());
     GB_KERNEL_CHECK();
   }
   const unsigned long long nnz64 = runtime().fetch(count);
@@ -81,7 +81,7 @@ Info ewiseMatrix(SparseMatrix<c>* C, SemiringT op, const SparseMatrix<a>* A,
     scanExclusiveAsync(tiles, ntiles, NULL);
     ewiseMatrixFillKernel<IsAdd, c><<<static_cast<unsigned int>(ntiles), GB_EWM_NT, 0, s>>>(
         Av.ptr, Av.ind, Av.val, Bv.ptr, Bv.ind, Bv.val, m, total, tiles, colind, val,
-        extractMul(op), extractAdd(op));
+        extractMul(op), extractAdd(op), EwmKeepAll());
     GB_KERNEL_CHECK();
   }
   C->replaceDevice(nnz, rowptr, colind, val);

@@ -85,6 +85,16 @@ class IndexList {
   bool nonDecreasing() const {
     return h_ == NULL || std::is_sorted(h_->begin(), h_->begin() + n_);
   }
+  // No index appears twice (ALL never repeats); extent bounds the checked list.
+  bool distinct(Index extent) const {
+    if (h_ == NULL) return true;
+    std::vector<bool> seen(static_cast<size_t>(extent), false);
+    for (Index p = 0; p < n_; ++p) {
+      if (seen[(*h_)[p]]) return false;
+      seen[(*h_)[p]] = true;
+    }
+    return true;
+  }
   bool sameAs(const IndexList& o) const {
     if (all() || o.all()) return all() && o.all();
     return n_ == o.n_ && std::equal(h_->begin(), h_->begin() + n_, o.h_->begin());

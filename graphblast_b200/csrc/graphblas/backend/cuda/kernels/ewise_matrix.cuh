@@ -20,6 +20,9 @@
 //   eWiseAdd : it is not a matched A item; a matched B item writes add(a, b),
 //              with A's value first, any other item its own value unchanged;
 //   eWiseMult: it is a matched B item, and writes mul(a, b).
+// An unmatched A item is emitted only where keep(row, column) holds: eWiseAdd
+// passes EwmKeepAll; assign (assign.cuh) drops C's entries inside the region it
+// replaces, and passes its accum (or "take B's value") as add.
 // C's entries are the emitted items in stream order, so an entry's position is
 // the number of items emitted before it.  Two passes over the same tiles:
 //   ewiseMatrixCountKernel: emitted items per tile (and their 64-bit total, the
@@ -129,15 +132,20 @@ __device__ __forceinline__ void ewmTileRows(long long d0, long long d1, Index nr
   __syncthreads();
 }
 
+// The keep test of the eWise operations: every unmatched A item is emitted.
+struct EwmKeepAll {
+  __device__ __forceinline__ bool operator()(Index, Index) const { return true; }
+};
+
 // Emitted items per tile (tile_count[t]), per row (atomics into row_count, zeroed
 // by the caller) and in all (*total, 64-bit).
-template <bool IsAdd>
+template <bool IsAdd, typename Keep>
 __global__ void __launch_bounds__(GB_EWM_NT)
 ewiseMatrixCountKernel(const Index* __restrict__ A_ptr, const Index* __restrict__ A_ind,
                        const Index* __restrict__ B_ptr, const Index* __restrict__ B_ind,
                        Index nrows, long long total, int* __restrict__ tile_count,
                        int* __restrict__ row_count,
-                       unsigned long long* __restrict__ total_count) {
+                       unsigned long long* __restrict__ total_count, Keep keep) {
   __shared__ Index s_rows[2];
   __shared__ int s_sum[GB_EWM_NT/32];
   const long long d0 = static_cast<long long>(blockIdx.x)*GB_EWM_TILE;
@@ -160,7 +168,7 @@ ewiseMatrixCountKernel(const Index* __restrict__ A_ptr, const Index* __restrict_
         in_row = 0;
       }
       if (q.ca <= q.cb) {                         // A item
-        if (IsAdd && q.cb != q.ca) ++in_row;
+        if (IsAdd && q.cb != q.ca && keep(q.r, q.ca)) ++in_row;
         q.last_a = q.ca;
         ++q.a;
         q.ca = q.a < q.a_end ? __ldg(A_ind + q.a) : GB_EWM_END;
@@ -184,14 +192,14 @@ ewiseMatrixCountKernel(const Index* __restrict__ A_ptr, const Index* __restrict_
 // tile_base[t] on (exclusive scan of the count pass's tile counts).  An item's
 // column and value stay in registers between the merge and the staging.
 template <bool IsAdd, typename c, typename a, typename b, typename MulOp,
-          typename AddOp>
+          typename AddOp, typename Keep>
 __global__ void __launch_bounds__(GB_EWM_NT)
 ewiseMatrixFillKernel(const Index* __restrict__ A_ptr, const Index* __restrict__ A_ind,
                       const a* __restrict__ A_val, const Index* __restrict__ B_ptr,
                       const Index* __restrict__ B_ind, const b* __restrict__ B_val,
                       Index nrows, long long total, const int* __restrict__ tile_base,
                       Index* __restrict__ C_ind, c* __restrict__ C_val, MulOp mul_op,
-                      AddOp add_op) {
+                      AddOp add_op, Keep keep) {
   __shared__ Index s_rows[2];
   __shared__ int s_scan[GB_EWM_NT/32 + 1];
   const long long d0 = static_cast<long long>(blockIdx.x)*GB_EWM_TILE;
@@ -212,7 +220,7 @@ ewiseMatrixFillKernel(const Index* __restrict__ A_ptr, const Index* __restrict__
       if (j < n) {
         ewmNextRowIfDone(q, p0 + j, r_hi, A_ptr, A_ind, B_ptr, B_ind);
         if (q.ca <= q.cb) {                       // A item
-          if (IsAdd && q.cb != q.ca) {
+          if (IsAdd && q.cb != q.ca && keep(q.r, q.ca)) {
             col[j] = q.ca;
             val[j] = static_cast<c>(A_val[q.a]);
             emit |= 1u << j;

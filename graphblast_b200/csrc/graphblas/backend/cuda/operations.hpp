@@ -35,6 +35,7 @@
 #include "graphblas/backend/cuda/ewise_matrix.hpp"
 #include "graphblas/backend/cuda/extract.hpp"
 #include "graphblas/backend/cuda/assign.hpp"
+#include "graphblas/backend/cuda/assign_matrix.hpp"
 #include "graphblas/backend/cuda/reduce.hpp"
 #include "graphblas/backend/cuda/apply.hpp"
 #include "graphblas/backend/cuda/indexed.hpp"
@@ -420,6 +421,61 @@ Info extract(Vector<TW>* w, const Vector<TMask>* mask, AccumT accum, const Vecto
   if (mask != NULL) return notBuilt("masked extract");
   CHECK(settle(w));
   return extractVector(w, u, indices, nindices);
+}
+
+// ---- assign into a matrix (assign_matrix.hpp) ----------------------------------------
+// Host index lists, NULL = GrB_ALL.  A mask, a dense C and a dense A are refused
+// before anything changes; C turns sparse once the result has replaced it (a C
+// never built counts as empty).
+
+// Whether a matrix assign can run on C: no mask and a C that is not dense.
+template <typename TC, typename TMask>
+Info assignTarget(const Matrix<TC>* C, const TMask* mask) {
+  if (mask != NULL) return notBuilt("masked assign");
+  if (C->isDense()) return notBuilt("assign into a dense matrix");
+  return GrB_SUCCESS;
+}
+
+// C(I, J) = accum(C(I, J), op(A)); C may be A.
+template <typename TC, typename TMask, typename TA, typename AccumT>
+Info assign(Matrix<TC>* C, const Matrix<TMask>* mask, AccumT accum, const Matrix<TA>* A,
+    const std::vector<Index>* row_indices, Index nrows,
+    const std::vector<Index>* col_indices, Index ncols, Descriptor* desc) {
+  CHECK(assignTarget(C, mask));
+  if (!A->isSparse()) return notBuilt("assign from a dense matrix");
+  Desc_value inp0_mode;
+  CHECK(desc->get(GrB_INP0, &inp0_mode));
+  CHECK(assignMatrix(&C->sparse_, accum, &A->sparse_, inp0_mode == GrB_TRAN, row_indices,
+                     nrows, col_indices, ncols));
+  return C->setStorage(GrB_SPARSE);
+}
+
+// C(I, j) = accum(C(I, j), u).
+template <typename TC, typename TMask, typename TU, typename AccumT>
+Info assign(Matrix<TC>* C, const Vector<TMask>* mask, AccumT accum, const Vector<TU>* u,
+    const std::vector<Index>* row_indices, Index nrows, Index col_index, Descriptor* desc) {
+  CHECK(assignTarget(C, mask));
+  CHECK(assignVector<true>(&C->sparse_, accum, u, row_indices, nrows, col_index));
+  return C->setStorage(GrB_SPARSE);
+}
+
+// C(i, J) = accum(C(i, J), u).
+template <typename TC, typename TMask, typename TU, typename AccumT>
+Info assign(Matrix<TC>* C, const Vector<TMask>* mask, AccumT accum, const Vector<TU>* u,
+    Index row_index, const std::vector<Index>* col_indices, Index ncols, Descriptor* desc) {
+  CHECK(assignTarget(C, mask));
+  CHECK(assignVector<false>(&C->sparse_, accum, u, col_indices, ncols, row_index));
+  return C->setStorage(GrB_SPARSE);
+}
+
+// C(I, J) = accum(C(I, J), val).
+template <typename TC, typename TMask, typename TS, typename AccumT>
+Info assign(Matrix<TC>* C, const Matrix<TMask>* mask, AccumT accum, TS val,
+    const std::vector<Index>* row_indices, Index nrows,
+    const std::vector<Index>* col_indices, Index ncols, Descriptor* desc) {
+  CHECK(assignTarget(C, mask));
+  CHECK(assignConstant(&C->sparse_, accum, val, row_indices, nrows, col_indices, ncols));
+  return C->setStorage(GrB_SPARSE);
 }
 
 // C = Aᵀ (C = A when GrB_INP0 is GrB_TRAN); C may be A.

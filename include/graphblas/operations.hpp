@@ -13,6 +13,7 @@
 #define GRAPHBLAS_OPERATIONS_HPP_
 
 #include <iostream>
+#include <type_traits>
 #include <vector>
 
 #include <graphblas/backend/cuda/operations.hpp>
@@ -502,32 +503,80 @@ Info extract(Vector<TW>* w, const Vector<TMask>* mask, AccumT accum, const Matri
                           raw(desc));
 }
 
-// ---- declared by the reference, implemented nowhere -------------------------------------
+// ---- assign into a matrix -----------------------------------------------------------
+// Host index lists; GrB_ALL (NULL) means every index of that extent, and a list may
+// not repeat an index (GrB_INVALID_VALUE).  Without accum, C(I, J) takes op(A)'s
+// pattern and values (entries of C inside the region that op(A) does not store are
+// deleted); with accum, C(I, J) = accum(C(I, J), op(A)) over the union of the two,
+// C's value first.  Outside the region C is unchanged.  The backend refuses an
+// index out of range (GrB_INVALID_INDEX) before anything changes.
 
+// C<mask>(row_indices, col_indices) = accum(C(..), op(A)), op(A) = Aᵀ when GrB_INP0
+// is GrB_TRAN; op(A) is nrows x ncols
 template <typename TC, typename TMask, typename TA, typename AccumT>
 Info assign(Matrix<TC>* C, const Matrix<TMask>* mask, AccumT accum, const Matrix<TA>* A,
             const std::vector<Index>* row_indices, Index nrows,
             const std::vector<Index>* col_indices, Index ncols, Descriptor* desc) {
-  return ops_detail::declaredOnly("assign matrix variant");
+  using namespace ops_detail;
+  GB_REQUIRE(C, A, desc);
+  Desc_value inp0;
+  CHECK(desc->get(GrB_INP0, &inp0));
+  const bool ta = inp0 == GrB_TRAN;
+  GB_SHAPES(Contract()
+      .equal(ta ? colsOf(A) : rowsOf(A), Extent{nrows, true}, "op(A).nrows != nrows")
+      .equal(ta ? rowsOf(A) : colsOf(A), Extent{ncols, true}, "op(A).ncols != ncols")
+      .alike(C, mask, "C.nrows != mask.nrows", "C.ncols != mask.ncols"));
+  return backend::assign(raw(C), raw(mask), accum, raw(A), row_indices, nrows, col_indices,
+                         ncols, raw(desc));
 }
+
+// C<mask>(row_indices, col_index) = accum(C(..), u), u of size nrows
 template <typename TC, typename TMask, typename TU, typename AccumT>
 Info assign(Matrix<TC>* C, const Vector<TMask>* mask, AccumT accum, const Vector<TU>* u,
             const std::vector<Index>* row_indices, Index nrows, Index col_index,
             Descriptor* desc) {
-  return ops_detail::declaredOnly("assign matrix variant");
+  using namespace ops_detail;
+  GB_REQUIRE(C, u, desc);
+  GB_SHAPES(Contract()
+      .equal(sizeOf(u), Extent{nrows, true}, "u.size != nrows")
+      .atMost(Extent{col_index + 1, true}, colsOf(C), "col_index >= C.ncols")
+      .equal(rowsOf(C), sizeOf(mask), "C.nrows != mask.size"));
+  return backend::assign(raw(C), raw(mask), accum, raw(u), row_indices, nrows, col_index,
+                         raw(desc));
 }
+
+// C<mask>(row_index, col_indices) = accum(C(..), u), u of size ncols
 template <typename TC, typename TMask, typename TU, typename AccumT>
 Info assign(Matrix<TC>* C, const Vector<TMask>* mask, AccumT accum, const Vector<TU>* u,
             Index row_index, const std::vector<Index>* col_indices, Index ncols,
             Descriptor* desc) {
-  return ops_detail::declaredOnly("assign matrix variant");
+  using namespace ops_detail;
+  GB_REQUIRE(C, u, desc);
+  GB_SHAPES(Contract()
+      .equal(sizeOf(u), Extent{ncols, true}, "u.size != ncols")
+      .atMost(Extent{row_index + 1, true}, rowsOf(C), "row_index >= C.nrows")
+      .equal(colsOf(C), sizeOf(mask), "C.ncols != mask.size"));
+  return backend::assign(raw(C), raw(mask), accum, raw(u), row_index, col_indices, ncols,
+                         raw(desc));
 }
+
+// C<mask>(row_indices, col_indices) = accum(C(..), val): every position of the
+// region ends up stored
 template <typename TC, typename TMask, typename TScalar, typename AccumT>
 Info assign(Matrix<TC>* C, const Matrix<TMask>* mask, AccumT accum, TScalar val,
             const std::vector<Index>* row_indices, Index nrows,
             const std::vector<Index>* col_indices, Index ncols, Descriptor* desc) {
-  return ops_detail::declaredOnly("assign matrix variant");
+  static_assert(std::is_arithmetic<TScalar>::value,
+                "assign: val is a scalar; pass the source matrix as const Matrix<T>*");
+  using namespace ops_detail;
+  GB_REQUIRE(C, desc);
+  GB_SHAPES(Contract().alike(C, mask, "C.nrows != mask.nrows", "C.ncols != mask.ncols"));
+  return backend::assign(raw(C), raw(mask), accum, val, row_indices, nrows, col_indices,
+                         ncols, raw(desc));
 }
+
+// ---- declared by the reference, implemented nowhere -------------------------------------
+
 template <typename TB, typename TA, typename TScalar, typename MonoidT>
 Info scale(Matrix<TB>* B, MonoidT op, const Matrix<TA>* A, TScalar val, Descriptor* desc) {
   return ops_detail::declaredOnly("scale matrix variant");
