@@ -151,6 +151,14 @@ ASSIGN_SIGNATURES = [
     ("gb200_assign_row", _I, [_P, _P, _I, _P, _I, _P, _I, _P]),
 ]
 
+# (name, restype, argtypes) for every symbol declared in include/graphblast_b200_ktruss.h,
+# the companion header of k-truss and truss decomposition; load() binds these too.
+KTRUSS_SIGNATURES = [
+    ("gb200_ktruss", _I, [_P, _P, _I, _P, C.POINTER(_LL), C.POINTER(_F)]),
+    ("gb200_trussness", _I, [_P, _P, _P, _IP, C.POINTER(_F)]),
+    ("gb200_ktruss_stats", _I, [_IP, _IP, C.POINTER(_F)]),
+]
+
 
 class ExtensionMissing(RuntimeError):
     pass
@@ -168,7 +176,7 @@ def load():
             "there is no CPU fallback." % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
     for name, restype, argtypes in (SIGNATURES + LGC_SIGNATURES + EXTRACT_SIGNATURES +
-                                    BC_SIGNATURES + ASSIGN_SIGNATURES):
+                                    BC_SIGNATURES + ASSIGN_SIGNATURES + KTRUSS_SIGNATURES):
         fn = getattr(lib, name)   # AttributeError if a declared symbol is missing
         fn.restype = restype
         fn.argtypes = argtypes

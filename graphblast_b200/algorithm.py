@@ -3,10 +3,11 @@
 loops of backend operations (include/graphblas/algorithm/*.hpp), and the graph
 colouring gc, the maximal independent set mis, the connected components cc and the
 local graph clustering lgc, one kernel each on the device, with lgc_sweep, the
-conductance sweep cut of lgc's result, and the betweenness centrality bc, one kernel
-per batch of 32 sources.
+conductance sweep cut of lgc's result, the betweenness centrality bc, one kernel
+per batch of 32 sources, and the k-truss ktruss and truss decomposition trussness, one
+cooperative edge-peeling kernel each.
 
-sssp, pr, tc, gc, mis, cc, lgc, lgc_sweep and bc return the device time of the operation
+sssp, pr, tc, gc, mis, cc, lgc, lgc_sweep, bc, ktruss and trussness return the device time of the operation
 loop in milliseconds ("tight" in the reference drivers, example/gbfs.cu:110-115).  bfs returns it only
 when called with timed=True; otherwise it returns None and, when the traversal runs
 as the fused kernel, only enqueues it, so that back-to-back traversals keep the GPU
@@ -162,3 +163,45 @@ def bc(v, A, desc, sources=None):
                             C.byref(ms))
     _check(code, "algorithm::bc")
     return ms.value
+
+
+
+
+def ktruss(out, A, k, desc):
+    """out = the k-truss (k >= 2) of the undirected simple graph G of A's pattern ({i, j},
+    i != j, when A(i,j) or A(j,i) is stored; values and self-loops ignored): starting
+    from G, every edge in fewer than k - 2 triangles of the remaining graph is deleted
+    until none is left to delete.  out(i,j) = out(j,i) = the number of triangles of the
+    k-truss that contain {i, j}; with k = 2, every edge with its triangle count in G.
+    out is n x n, sorted, installed as symmetric, FP32 or INT32 independently of A, and
+    may be A.  A is FP32 or INT32; a non-symmetric A needs its CSC.  Integers only, so
+    two calls give identical bytes (include/graphblas/algorithm/ktruss.hpp).
+    Returns (nedges, tight_ms), nedges the undirected edges kept."""
+    ms = C.c_float(0)
+    count = C.c_longlong(0)
+    _check(_lib.load().gb200_ktruss(out._h, A._h, int(k), desc._h, C.byref(count),
+                                    C.byref(ms)),
+           "algorithm::ktruss")
+    return count.value, ms.value
+
+
+def trussness(out, A, desc):
+    """out = the truss decomposition of the undirected simple graph G of A's pattern (as
+    in ktruss): G's pattern in both directions, out(i,j) = out(j,i) = the largest k
+    whose k-truss contains {i, j}, 2 for an edge in no triangle.  out is n x n, sorted,
+    installed as symmetric, FP32 or INT32 independently of A, and may be A.  Returns
+    (kmax, tight_ms), kmax the largest value, 0 when G has no edge."""
+    ms = C.c_float(0)
+    kmax = C.c_int(0)
+    _check(_lib.load().gb200_trussness(out._h, A._h, desc._h, C.byref(kmax), C.byref(ms)),
+           "algorithm::trussness")
+    return kmax.value, ms.value
+
+
+def ktruss_stats():
+    """(rounds, levels, support_ms) of the last ktruss or trussness call of this process:
+    the peel rounds that removed edges, the levels that did, and the device time of the
+    support pass alone in milliseconds."""
+    rounds, levels, support = C.c_int(0), C.c_int(0), C.c_float(0)
+    _lib.load().gb200_ktruss_stats(C.byref(rounds), C.byref(levels), C.byref(support))
+    return rounds.value, levels.value, support.value

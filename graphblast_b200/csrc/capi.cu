@@ -29,12 +29,14 @@
 #include "graphblas/algorithm/cc.hpp"
 #include "graphblas/algorithm/lgc.hpp"
 #include "graphblas/algorithm/bc.hpp"
+#include "graphblas/algorithm/ktruss.hpp"
 
 #include "graphblast_b200.h"
 #include "graphblast_b200_lgc.h"
 #include "graphblast_b200_extract.h"
 #include "graphblast_b200_bc.h"
 #include "graphblast_b200_assign.h"
+#include "graphblast_b200_ktruss.h"
 
 bool debug_;
 bool memory_;
@@ -1218,6 +1220,55 @@ int gb200_bc(gb200_vector_t v, gb200_matrix_t A, const int* h_sources, int nsour
       return graphblas::algorithm::bc(v->f, M, h_sources, nsources, &desc->desc);
     });
   });
+}
+
+// ---- k-truss and truss decomposition (include/graphblast_b200_ktruss.h) ----------
+
+int gb200_ktruss(gb200_matrix_t C, gb200_matrix_t A, int k, gb200_desc_t desc,
+                 long long* nedges, float* tight_ms) {
+  if (C == NULL || A == NULL || desc == NULL)
+    return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
+  if ((C->f == NULL && C->i == NULL) || (A->f == NULL && A->i == NULL))
+    return rc(graphblas::GrB_DOMAIN_MISMATCH);
+  if (k < 2) return rc(graphblas::GrB_INVALID_VALUE);
+  GB200_REQUIRE_DEVICE();
+  graphblas::Index count = 0;
+  const int info = runAlgorithm(tight_ms, [&] {
+    return onMatrix(C, [&](auto O) {
+      return onMatrix(A, [&](auto M) {
+        return graphblas::algorithm::ktruss(O, M, k, &desc->desc, &count);
+      });
+    });
+  });
+  if (info == 0 && nedges) *nedges = count;
+  return info;
+}
+
+int gb200_trussness(gb200_matrix_t T, gb200_matrix_t A, gb200_desc_t desc, int* kmax,
+                    float* tight_ms) {
+  if (T == NULL || A == NULL || desc == NULL)
+    return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
+  if ((T->f == NULL && T->i == NULL) || (A->f == NULL && A->i == NULL))
+    return rc(graphblas::GrB_DOMAIN_MISMATCH);
+  GB200_REQUIRE_DEVICE();
+  int top = 0;
+  const int info = runAlgorithm(tight_ms, [&] {
+    return onMatrix(T, [&](auto O) {
+      return onMatrix(A, [&](auto M) {
+        return graphblas::algorithm::trussness(O, M, &desc->desc, &top);
+      });
+    });
+  });
+  if (info == 0 && kmax) *kmax = top;
+  return info;
+}
+
+int gb200_ktruss_stats(int* rounds, int* levels, float* support_ms) {
+  const graphblas::backend::KtrussStats& stats = graphblas::backend::ktrussLastStats();
+  if (rounds) *rounds = stats.rounds;
+  if (levels) *levels = stats.levels;
+  if (support_ms) *support_ms = stats.support_ms;
+  return 0;
 }
 
 // ---- extract (include/graphblast_b200_extract.h) -------------------------------

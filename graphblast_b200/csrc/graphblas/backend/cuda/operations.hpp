@@ -45,6 +45,7 @@
 #include "graphblas/backend/cuda/cc.hpp"
 #include "graphblas/backend/cuda/lgc.hpp"
 #include "graphblas/backend/cuda/bc.hpp"
+#include "graphblas/backend/cuda/ktruss.hpp"
 
 namespace graphblas {
 namespace backend {
