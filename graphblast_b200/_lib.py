@@ -159,6 +159,13 @@ KTRUSS_SIGNATURES = [
     ("gb200_ktruss_stats", _I, [_IP, _IP, C.POINTER(_F)]),
 ]
 
+# (name, restype, argtypes) for every symbol declared in include/graphblast_b200_scc.h,
+# the companion header of strongly connected components; load() binds these too.
+SCC_SIGNATURES = [
+    ("gb200_scc", _I, [_P, _P, _P, _IP, C.POINTER(_F)]),
+    ("gb200_scc_stats", _I, [C.POINTER(_LL), C.POINTER(_LL), _IP, _IP]),
+]
+
 
 class ExtensionMissing(RuntimeError):
     pass
@@ -176,7 +183,8 @@ def load():
             "there is no CPU fallback." % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
     for name, restype, argtypes in (SIGNATURES + LGC_SIGNATURES + EXTRACT_SIGNATURES +
-                                    BC_SIGNATURES + ASSIGN_SIGNATURES + KTRUSS_SIGNATURES):
+                                    BC_SIGNATURES + ASSIGN_SIGNATURES + KTRUSS_SIGNATURES +
+                                    SCC_SIGNATURES):
         fn = getattr(lib, name)   # AttributeError if a declared symbol is missing
         fn.restype = restype
         fn.argtypes = argtypes

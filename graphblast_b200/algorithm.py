@@ -4,10 +4,11 @@ loops of backend operations (include/graphblas/algorithm/*.hpp), and the graph
 colouring gc, the maximal independent set mis, the connected components cc and the
 local graph clustering lgc, one kernel each on the device, with lgc_sweep, the
 conductance sweep cut of lgc's result, the betweenness centrality bc, one kernel
-per batch of 32 sources, and the k-truss ktruss and truss decomposition trussness, one
-cooperative edge-peeling kernel each.
+per batch of 32 sources, the k-truss ktruss and truss decomposition trussness, one
+cooperative edge-peeling kernel each, and the strongly connected components scc, one
+cooperative trim, forward-backward and colouring kernel.
 
-sssp, pr, tc, gc, mis, cc, lgc, lgc_sweep, bc, ktruss and trussness return the device time of the operation
+sssp, pr, tc, gc, mis, cc, lgc, lgc_sweep, bc, ktruss, trussness and scc return the device time of the operation
 loop in milliseconds ("tight" in the reference drivers, example/gbfs.cu:110-115).  bfs returns it only
 when called with timed=True; otherwise it returns None and, when the traversal runs
 as the fused kernel, only enqueues it, so that back-to-back traversals keep the GPU
@@ -205,3 +206,30 @@ def ktruss_stats():
     rounds, levels, support = C.c_int(0), C.c_int(0), C.c_float(0)
     _lib.load().gb200_ktruss_stats(C.byref(rounds), C.byref(levels), C.byref(support))
     return rounds.value, levels.value, support.value
+
+
+def scc(v, A, desc):
+    """v[i] = the smallest vertex id in the strongly connected component of i, over the
+    arcs i -> j with A(i,j) stored and i != j (values and self-loops ignored), one
+    cooperative trim, forward-backward and colouring kernel
+    (include/graphblas/algorithm/scc.hpp).  The result depends only on A's pattern, so
+    there is no seed.  A is FP32 or INT32; out-lists come from its CSR and in-lists from
+    its CSC, so a non-symmetric A needs its CSC.  An A marked symmetric (or whose CSC
+    aliases its CSR) takes cc, whose components are then the strong ones.  v becomes
+    dense and is overwritten.  A float v holds ids exactly only up to 2^24, so
+    nrows(A) > 2^24 + 1 raises GrB_INVALID_VALUE.  Returns (ncomponents, tight_ms)."""
+    ms = C.c_float(0)
+    k = C.c_int(0)
+    _check(_lib.load().gb200_scc(v._h, A._h, desc._h, C.byref(k), C.byref(ms)),
+           "algorithm::scc")
+    return k.value, ms.value
+
+
+def scc_stats():
+    """(trimmed, pivot_size, colour_iterations, barriers) of the last scc call of this
+    process: the vertices settled by the trim, the size of the pivot's component, the
+    colouring iterations and the grid barriers of the kernel.  After an A marked
+    symmetric (cc's kernel) all are 0 except barriers, which is -1."""
+    t, p, c, b = C.c_longlong(0), C.c_longlong(0), C.c_int(0), C.c_int(0)
+    _lib.load().gb200_scc_stats(C.byref(t), C.byref(p), C.byref(c), C.byref(b))
+    return t.value, p.value, c.value, b.value

@@ -30,6 +30,7 @@
 #include "graphblas/algorithm/lgc.hpp"
 #include "graphblas/algorithm/bc.hpp"
 #include "graphblas/algorithm/ktruss.hpp"
+#include "graphblas/algorithm/scc.hpp"
 
 #include "graphblast_b200.h"
 #include "graphblast_b200_lgc.h"
@@ -37,6 +38,7 @@
 #include "graphblast_b200_bc.h"
 #include "graphblast_b200_assign.h"
 #include "graphblast_b200_ktruss.h"
+#include "graphblast_b200_scc.h"
 
 bool debug_;
 bool memory_;
@@ -1268,6 +1270,34 @@ int gb200_ktruss_stats(int* rounds, int* levels, float* support_ms) {
   if (rounds) *rounds = stats.rounds;
   if (levels) *levels = stats.levels;
   if (support_ms) *support_ms = stats.support_ms;
+  return 0;
+}
+
+// ---- strongly connected components (include/graphblast_b200_scc.h) ---------------
+
+int gb200_scc(gb200_vector_t v, gb200_matrix_t A, gb200_desc_t desc, int* ncomponents,
+              float* tight_ms) {
+  if (v == NULL || A == NULL || desc == NULL)
+    return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
+  if (A->f == NULL && A->i == NULL) return rc(graphblas::GrB_DOMAIN_MISMATCH);
+  GB200_REQUIRE_DEVICE();
+  int count = 0;
+  const int info = runAlgorithm(tight_ms, [&] {
+    return onMatrix(A, [&](auto M) {
+      return graphblas::algorithm::scc(v->f, M, &desc->desc, &count);
+    });
+  });
+  if (info == 0 && ncomponents) *ncomponents = count;
+  return info;
+}
+
+int gb200_scc_stats(long long* trimmed, long long* pivot_size, int* colour_iterations,
+                    int* barriers) {
+  const graphblas::backend::SccStats& stats = graphblas::backend::sccLastStats();
+  if (trimmed) *trimmed = stats.trimmed;
+  if (pivot_size) *pivot_size = stats.pivot_size;
+  if (colour_iterations) *colour_iterations = stats.colour_iterations;
+  if (barriers) *barriers = stats.barriers;
   return 0;
 }
 

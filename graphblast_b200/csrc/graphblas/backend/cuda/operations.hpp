@@ -46,6 +46,7 @@
 #include "graphblas/backend/cuda/lgc.hpp"
 #include "graphblas/backend/cuda/bc.hpp"
 #include "graphblas/backend/cuda/ktruss.hpp"
+#include "graphblas/backend/cuda/scc.hpp"
 
 namespace graphblas {
 namespace backend {
