@@ -150,11 +150,14 @@ Info bfsFused(Vector<float>* v, const Matrix<a>* A, Index s, Descriptor* desc, i
         cells[GB_BFS_CELL_LEVELS] < GB_BFS_TIMED_LEVELS - 1 ? cells[GB_BFS_CELL_LEVELS]
                                                             : GB_BFS_TIMED_LEVELS - 1);
     fprintf(stderr, "bfs trace: set-up %.1fus",
-            1e-3*static_cast<double>((clock[0] >> 1) - cells[GB_BFS_CELL_START_CLOCK]));
+            1e-3*static_cast<double>((clock[0] >> 2) - cells[GB_BFS_CELL_START_CLOCK]));
+    int second_phases = 0;
     for (int l = 1; l <= levels; ++l) {
-      const unsigned long long start = clock[l - 1] >> 1, end = clock[l] >> 1;
+      const unsigned long long start = clock[l - 1] >> 2, end = clock[l] >> 2;
       const unsigned long long scan = cells[GB_BFS_CELL_SCAN_CLOCK + l];
-      if (clock[l] & 1ull)               // pull: scan, walk, rows walked, chunks listed
+      second_phases += static_cast<int>((clock[l] >> 1) & 1ull);
+      // pull: scan, walk (0 without a second phase), rows walked, chunks listed
+      if (clock[l] & 1ull)
         fprintf(stderr, " L%d pull %.1fus (scan %.1f walk %.1f, %llu walked, %llu listed)",
                 l, 1e-3*static_cast<double>(end - start),
                 1e-3*static_cast<double>(scan - start),
@@ -166,6 +169,14 @@ Info bfsFused(Vector<float>* v, const Matrix<a>* A, Index s, Descriptor* desc, i
     fprintf(stderr, " end-pass %.1fus\n",
             1e-3*static_cast<double>(cells[GB_BFS_CELL_END_PASS_CLOCK] -
                                      cells[GB_BFS_CELL_LAST_LEVEL_CLOCK]));
+    // Grid barriers: the set-up's, one per level and one per second phase.  Each level
+    // marks in its clock cell whether it ran a second phase: a counter cell added to
+    // after the barriers costs the push-only instantiation spill reloads.  Levels past
+    // the traced ones are counted as if they ran none.
+    fprintf(stderr, "bfs barriers: %llu (second phases %d%s)\n",
+            1ull + cells[GB_BFS_CELL_LEVELS] + second_phases, second_phases,
+            cells[GB_BFS_CELL_LEVELS] > static_cast<unsigned long long>(levels)
+                ? ", later levels not traced" : "");
   }
   if (depth != NULL) {
     const unsigned long long levels = runtime().fetch(args.counters + GB_BFS_CELL_LEVELS);

@@ -14,15 +14,20 @@
 // State: visited bitmap (two copies, ping-pong on pull levels), frontier bitmap F,
 // next-frontier bitmap N, a byte per row holding its level while the traversal runs,
 // float levels v (the result, 1-based, 0 = unreached).
+//   A level is a main phase and one grid barrier.  A second phase, and a second
+//   barrier, follow only when the main phase left work for the whole grid (heavy
+//   vertices pushing, listed chunks pulling); the count of that work is complete at
+//   the barrier, so every thread takes the same branch.
 //   push level (frontier small): warps scan F; a vertex of moderate degree is
 //     expanded by its warp, lanes striding the adjacency; vertices with more than
-//     GB_BFS_HEAVY neighbours go to a list that the WHOLE grid expands after a
-//     barrier (an R-MAT source has 10^5..10^6 neighbours).  Discoveries set the
-//     visited bit with atomicOr immediately (same level either way), the winner
-//     writes v and the N bit.
+//     GB_BFS_HEAVY neighbours go to a list that the WHOLE grid expands in the second
+//     phase (an R-MAT source has 10^5..10^6 neighbours).  Level 1 scans nothing: its
+//     frontier is the source, whose list the grid expands in the main phase.
+//     Discoveries set the visited bit with atomicOr immediately (same level either
+//     way), the winner writes v and the N bit.
 //   pull level (frontier large): the fused Boolean pull of kernels/spmv_pull.cuh,
 //     probing the visited bitmap AS OF THE LEVEL'S START (operand reuse, reference
-//     kernels/spmv.hpp:35-41), in two phases separated by a grid barrier:
+//     kernels/spmv.hpp:35-41), a scan and, when it listed chunks, a walk of them:
 //     scan  — warps take chunks of 32 bitmap words (1024 rows) round-robin; a
 //             lane per word, fully visited words only move their bitmap words on.
 //             Every open row probes one neighbour, its highest-degree one (the
@@ -38,8 +43,9 @@
 //             a chunk with more goes to a list of such chunks.
 //             The owner of a word writes N, the merged visited word of the other
 //             copy, the level bytes of the discovered rows and clears F.
-//     walk  — warps claim listed chunks from a counter and walk their rows by the
-//             same rules; discoveries are ORed into N and the other visited copy.
+//     walk  — (second phase) warps claim listed chunks from a counter and walk their
+//             rows by the same rules; discoveries are ORed into N and the other
+//             visited copy.
 //   The walk (bfsWalkRows): a lane walks its row's list from entry 0 (the probed
 //   entry is looked at again), GB_BFS_WALK_STEP entries per step, a list still
 //   longer than GB_BFS_WALK_WARP after the first step is walked by the whole warp,
@@ -129,8 +135,15 @@ struct BfsFusedArgs {
 #define GB_BFS_TIMED_LEVELS 16
 
 // The cells of BfsFusedArgs::counters.  A rotating cell is a triple used by level L
-// as cell L % 3 (bfsLevelCell): it is zeroed during level L-1, filled during L and
-// read after L's barrier, when slow threads may still be reading the cell of L-1.
+// as cell L % 3 (bfsLevelCell): thread 0 zeroes it at the start of level L-1, it is
+// added to during L and read after L's first barrier (heavy, listed: their counts
+// come from the main phase) or its last (the frontier count).  One barrier per level
+// is enough to keep the triples race-free.  Level L zeroes cell L+1, which is cell
+// L-2: every read of L-2's cells happens after L-2's last barrier and before the
+// reading thread arrives at L-1's first barrier, which thread 0 has passed when it
+// starts level L.  The first add to cell L+1 comes after L's first barrier, when the
+// zero store of level L is ordered before it.  With two cells a thread still reading
+// level L-1's count after L-1's barrier would meet level L+1's zeroing.
 // Clocks are %globaltimer nanoseconds.
 enum BfsCell {
   // zeroed at the start of a traversal
@@ -145,8 +158,8 @@ enum BfsCell {
   GB_BFS_CELL_FOUND_PUSHING,                          // vertices discovered pushing
   // clocks
   GB_BFS_CELL_LEVEL_CLOCK,                            // per level: end of the set-up
-                                                      // (0) and of every level, ns << 1
-                                                      // | pulled
+                                                      // (0) and of every level, ns << 2
+                                                      // | second phase << 1 | pulled
   GB_BFS_CELL_START_CLOCK = GB_BFS_CELL_LEVEL_CLOCK + GB_BFS_TIMED_LEVELS,
   GB_BFS_CELL_END_PASS_CLOCK,                         // end of the pass that writes v
                                                       // (GB200_BFS_TRACE only)
@@ -154,7 +167,7 @@ enum BfsCell {
   // pull levels, zeroed at the start of a traversal
   GB_BFS_CELL_WALK_CLAIM = 35,                        // rotating: walk-chunk claims
   GB_BFS_CELL_LISTED = GB_BFS_CELL_WALK_CLAIM + 3,    // rotating: chunks in walk_chunks
-  GB_BFS_CELL_SCAN_CLOCK = 44,                        // per level: the scan barrier
+  GB_BFS_CELL_SCAN_CLOCK = 44,                        // per pull level: the scan barrier
   // per level, GB200_BFS_TRACE only: rows the scan left to walk (inline and listed,
   // zeroed at the start of a traversal) and chunks it listed
   GB_BFS_CELL_WALKED = GB_BFS_CELL_SCAN_CLOCK + GB_BFS_TIMED_LEVELS,
@@ -233,6 +246,38 @@ __device__ __forceinline__ unsigned int* bfsN(const BfsFusedArgs& a, int fsel) {
 // as visited from the start and are unreached unless one is the source.
 __device__ __forceinline__ unsigned int bfsIsolated(const BfsFusedArgs& a, Index w) {
   return a.pull_empty[w] & (a.push_empty != NULL ? a.push_empty[w] : 0xffffffffu);
+}
+
+// Adds a phase's discoveries to the level's count (and, pushing, to the vertices
+// discovered pushing), one atomic per CTA.
+template <int NT>
+__device__ __forceinline__ void bfsAddFound(const BfsFusedArgs& a,
+                                            unsigned long long* count_cell, int found_here,
+                                            bool pushing, int* s_red) {
+  const int block_found = blockSum<NT>(found_here, s_red);
+  if (threadIdx.x == 0 && block_found) {
+    atomicAdd(count_cell, static_cast<unsigned long long>(block_found));
+    if (pushing)
+      atomicAdd(a.counters + GB_BFS_CELL_FOUND_PUSHING,
+                static_cast<unsigned long long>(block_found));
+  }
+}
+
+// The whole grid expands vertex u's list, a thread per entry; returns its length.
+__device__ __forceinline__ Index bfsExpandGrid(const BfsFusedArgs& a, int vsel, int fsel,
+                                               int level, Index u, Index gtid,
+                                               Index gthreads, int& found_here) {
+  const Index beg = __ldg(a.push_ptr + u);
+  const Index deg = __ldg(a.push_ptr + u + 1) - beg;
+  for (Index k = gtid; k < deg; k += gthreads) {
+    const Index nbr = __ldg(a.push_ind + beg + k);
+    if (bfsClaim(bfsVis(a, vsel), nbr)) {
+      bfsSetLevel(a, nbr, level + 1);
+      atomicOr(bfsN(a, fsel) + (nbr >> 5), 1u << (nbr & 31));
+      ++found_here;
+    }
+  }
+  return deg;
 }
 
 // The pull walk of one row per lane (warp-collective; a lane without a row passes
@@ -321,22 +366,27 @@ bfsFusedKernel(BfsFusedArgs a) {
   const Index nchunks = (nwords + 31) >> 5;               // pull chunks of 32 words
 
   if (gtid == 0) a.counters[GB_BFS_CELL_START_CLOCK] = bfsClockNs();
-  // ---- level 0: clear the bitmaps, seed the source (v is written once per row, after
-  // the last level) ---------------------------------------------------------------------
+  // ---- level 0: clear the bitmaps, mark the source visited (v is written once per
+  // row, after the last level) ------------------------------------------------------------
+  // F is not seeded: a push at level 1 expands the source without reading F, a pull
+  // only clears it, and the end pass adds the source back to what it reaches.
+  // visited[1] is not cleared: it is read (as visited[vsel], and by the end pass)
+  // only once vsel is 1, after a pull level whose owners' stores wrote every word of
+  // it, and it is never read in a push-only traversal.
   if (gtid == 0) a.level8[a.source] = 1;
   for (Index w = gtid; w < nwords; w += gthreads) {
     const unsigned int seed = (w == (a.source >> 5)) ? (1u << (a.source & 31)) : 0u;
     // rows nothing points at count as visited from the start: no level can discover
     // them, and the pull levels would look at them every time
     a.visited[0][w] = seed | bfsIsolated(a, w);
-    a.visited[1][w] = 0u; a.frontier[w] = seed; a.next[w] = 0u;
+    a.frontier[w] = 0u; a.next[w] = 0u;
   }
   if (gtid <= GB_BFS_CELL_FOUND_PUSHING) a.counters[gtid] = 0ull;
   if (gtid >= GB_BFS_CELL_WALK_CLAIM && gtid < GB_BFS_CELL_LISTED + 3) a.counters[gtid] = 0ull;
   if (gtid >= GB_BFS_CELL_WALKED && gtid < GB_BFS_CELL_WALKED + GB_BFS_TIMED_LEVELS)
     a.counters[gtid] = 0ull;
   grid.sync();
-  if (gtid == 0) a.counters[GB_BFS_CELL_LEVEL_CLOCK] = bfsClockNs() << 1;
+  if (gtid == 0) a.counters[GB_BFS_CELL_LEVEL_CLOCK] = bfsClockNs() << 2;
 
   int vsel = 0;                           // bfsVis / bfsVisOther
   int fsel = 0;                           // bfsF / bfsN
@@ -344,7 +394,8 @@ bfsFusedKernel(BfsFusedArgs a) {
   bool dense = PULL && (a.mode == 2);             // direction state (storage of the frontier)
   float prev_ratio = 0.f;
   int inspected = 0;                      // colind entries looked at by this thread
-  int pushed_vertices = 0;                // frontier entries expanded (lane 0 counts)
+  int pushed_vertices = 0;                // frontier entries expanded (lane 0 counts,
+                                          // thread 0 the source at level 1)
   unsigned int pushed_edges = 0u;         // their adjacency lengths (a vertex is pushed
                                           // once: at most nnz < 2^31 per thread)
   int pull_levels = 0;
@@ -370,7 +421,13 @@ bfsFusedKernel(BfsFusedArgs a) {
     }
     int found_here = 0;
 
-    if (!dense) {
+    if (!dense && level == 1) {
+      // ---------------- push from the source: the grid expands its list ----------
+      // (no scan of F for its one vertex, no barrier before a heavy source's list)
+      const Index deg = bfsExpandGrid(a, vsel, fsel, level, a.source, gtid, gthreads,
+                                      found_here);
+      if (gtid == 0) { ++pushed_vertices; pushed_edges += deg; }
+    } else if (!dense) {
       // ---------------- push: expand the frontier --------------------------------
       // A warp reads 32 frontier words at once (the frontier is sparse here: most
       // words are zero and a word-at-a-time scan is a chain of dependent loads),
@@ -393,8 +450,8 @@ bfsFusedKernel(BfsFusedArgs a) {
             const Index deg = __ldg(a.push_ptr + u + 1) - beg;
             if (lane == 0) { ++pushed_vertices; pushed_edges += deg; }
             if (deg > GB_BFS_HEAVY) {
-              // the whole grid expands it after the barrier; a full list falls back
-              // to this warp (slow, still correct)
+              // the whole grid expands it in the second phase; a full list falls
+              // back to this warp (slow, still correct)
               unsigned long long slot = 0ull;
               if (lane == 0) slot = atomicAdd(heavy_cell, 1ull);
               slot = __shfl_sync(GB_FULL_MASK, slot, 0);
@@ -414,31 +471,9 @@ bfsFusedKernel(BfsFusedArgs a) {
           }
         }
       }
-      grid.sync();
-      const unsigned long long listed =
-          *reinterpret_cast<volatile unsigned long long*>(heavy_cell);
-      const int nheavy = (listed > GB_BFS_HEAVY_CAP) ? GB_BFS_HEAVY_CAP
-                                                     : static_cast<int>(listed);
-      if (nheavy > 0) {
-        for (int h = 0; h < nheavy; ++h) {
-          const Index u = a.heavy[h];
-          const Index beg = __ldg(a.push_ptr + u);
-          const Index deg = __ldg(a.push_ptr + u + 1) - beg;
-          for (Index k = gtid; k < deg; k += gthreads) {
-            const Index nbr = __ldg(a.push_ind + beg + k);
-            if (bfsClaim(bfsVis(a, vsel), nbr)) {
-              bfsSetLevel(a, nbr, level + 1);
-              atomicOr(bfsN(a, fsel) + (nbr >> 5), 1u << (nbr & 31));
-              ++found_here;
-            }
-          }
-        }
-      }
     } else if (PULL) {
       ++pull_levels;
       // ---------------- pull: every unvisited row looks for a visited neighbour ----
-      unsigned long long* const walk_cell =
-          bfsLevelCell(a.counters, GB_BFS_CELL_WALK_CLAIM, level);
       unsigned long long* const list_cell = bfsLevelCell(a.counters, GB_BFS_CELL_LISTED, level);
       // scan: a lane per bitmap word of the chunk, chunks dealt round-robin (the
       // grid has ~4 chunks per warp at RMAT-24 and they cost about the same); the
@@ -629,44 +664,61 @@ bfsFusedKernel(BfsFusedArgs a) {
         }
         c = c_next;
       }
+    }
+    // ---- the level's barrier, then the second phase when there is one ---------------
+    // One barrier and one count for each phase, from one place in the code: written
+    // twice, the push-only instantiation reloads more spilled values after them.
+    for (int phase = 0; ; ++phase) {
+      bfsAddFound<NT>(a, count_cell, found_here, !dense, s_red);
       grid.sync();
-      const Index nlisted = static_cast<Index>(
-          *reinterpret_cast<volatile unsigned long long*>(list_cell));
+      // After the main phase: heavy vertices listed pushing, chunks listed pulling.
+      // Every add to the cell came before the barrier, so every thread reads the
+      // same value and takes the same branch.
+      const unsigned long long listed = phase ? 0ull : *reinterpret_cast<volatile unsigned long long*>(
+          bfsLevelCell(a.counters, dense ? GB_BFS_CELL_LISTED : GB_BFS_CELL_HEAVY, level));
       if (gtid == 0 && level < GB_BFS_TIMED_LEVELS) {
-        a.counters[GB_BFS_CELL_SCAN_CLOCK + level] = bfsClockNs();
-        if (a.trace)
-          a.counters[GB_BFS_CELL_LISTED_CHUNKS + level] = static_cast<unsigned long long>(nlisted);
-      }
-      // walk: the heavy chunks' rows, chunks claimed from a counter, a lane per row
-      for (Index i = gwarp; i < nlisted; ) {
-        const Index i_next = gwarps + bfsClaimChunk(walk_cell, lane);
-        const Index c = a.walk_chunks[i];
-        const int nwalk = a.walk_count[c];
-        for (int i0 = 0; i0 < nwalk; i0 += 32) {
-          const bool active = i0 + lane < nwalk;
-          const Index row = active ? a.walk[c*GB_BFS_CHUNK + i0 + lane] : 0;
-          if (bfsWalkRows(a, vsel, row, active, lane, inspected)) {
-            const unsigned int bit = 1u << (row & 31);
-            atomicOr(bfsN(a, fsel) + (row >> 5), bit);
-            atomicOr(bfsVisOther(a, vsel) + (row >> 5), bit);
-            bfsSetLevel(a, row, level + 1);
-            ++found_here;
-          }
+        const unsigned long long t = bfsClockNs();
+        if (dense && phase == 0) {
+          a.counters[GB_BFS_CELL_SCAN_CLOCK + level] = t;
+          if (a.trace) a.counters[GB_BFS_CELL_LISTED_CHUNKS + level] = listed;
         }
-        i = i_next;
+        if (listed == 0ull)
+          a.counters[GB_BFS_CELL_LEVEL_CLOCK + level] =
+              (t << 2) | (static_cast<unsigned long long>(phase) << 1) | (dense ? 1ull : 0ull);
+      }
+      if (listed == 0ull) break;
+      found_here = 0;                       // the main phase's are counted
+      if (!dense) {
+        // the heavy vertices' lists, each by the whole grid
+        const int nheavy = (listed > GB_BFS_HEAVY_CAP) ? GB_BFS_HEAVY_CAP
+                                                       : static_cast<int>(listed);
+        for (int h = 0; h < nheavy; ++h)
+          bfsExpandGrid(a, vsel, fsel, level, a.heavy[h], gtid, gthreads, found_here);
+      } else if (PULL) {
+        // walk: the heavy chunks' rows, chunks claimed from a counter, a lane per row
+        unsigned long long* const walk_cell =
+            bfsLevelCell(a.counters, GB_BFS_CELL_WALK_CLAIM, level);
+        const Index nlisted = static_cast<Index>(listed);
+        for (Index i = gwarp; i < nlisted; ) {
+          const Index i_next = gwarps + bfsClaimChunk(walk_cell, lane);
+          const Index c = a.walk_chunks[i];
+          const int nwalk = a.walk_count[c];
+          for (int i0 = 0; i0 < nwalk; i0 += 32) {
+            const bool active = i0 + lane < nwalk;
+            const Index row = active ? a.walk[c*GB_BFS_CHUNK + i0 + lane] : 0;
+            if (bfsWalkRows(a, vsel, row, active, lane, inspected)) {
+              const unsigned int bit = 1u << (row & 31);
+              atomicOr(bfsN(a, fsel) + (row >> 5), bit);
+              atomicOr(bfsVisOther(a, vsel) + (row >> 5), bit);
+              bfsSetLevel(a, row, level + 1);
+              ++found_here;
+            }
+          }
+          i = i_next;
+        }
       }
     }
     // ---- frontier size of the next level ------------------------------------------
-    const int block_found = blockSum<NT>(found_here, s_red);
-    if (threadIdx.x == 0 && block_found) {
-      atomicAdd(count_cell, static_cast<unsigned long long>(block_found));
-      if (!dense)
-        atomicAdd(a.counters + GB_BFS_CELL_FOUND_PUSHING,
-                  static_cast<unsigned long long>(block_found));
-    }
-    grid.sync();
-    if (gtid == 0 && level < GB_BFS_TIMED_LEVELS)
-      a.counters[GB_BFS_CELL_LEVEL_CLOCK + level] = (bfsClockNs() << 1) | (dense ? 1ull : 0ull);
     fcount = static_cast<unsigned int>(
         *reinterpret_cast<volatile unsigned long long*>(count_cell));
     if (dense) vsel ^= 1;
@@ -806,7 +858,7 @@ bfsFusedKernel(BfsFusedArgs a) {
     }
   }
   if (a.trace) {
-    grid.sync();
+    grid.sync();                  // only to time the end pass: not counted in the barriers
     if (gtid == 0) a.counters[GB_BFS_CELL_END_PASS_CLOCK] = bfsClockNs();
   }
   // ---- results: the work counters, the algorithmic bytes of SURVEY.md §8d --------
