@@ -345,7 +345,10 @@ class Vector(object):
         _check(self._lib.gb200_vector_dup(self._h, rhs._h), "Vector::dup")
 
     def swap(self, rhs):
+        """Trades contents with rhs, and with them the device tensors either one
+        adopted (build_device), which must live as long as the contents do."""
         _check(self._lib.gb200_vector_swap(self._h, rhs._h), "Vector::swap")
+        self._keep, rhs._keep = rhs._keep, self._keep
 
     def getStorage(self):
         out = C.c_int(0)
