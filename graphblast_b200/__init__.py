@@ -20,6 +20,6 @@ from .api import (  # noqa: F401
     PlusMonoid, MultipliesMonoid, MinimumMonoid, MaximumMonoid,
     LogicalOrMonoid, LogicalAndMonoid, GreaterMonoid, CustomLessMonoid,
     NotEqualToMonoid,
-    init, sync, sm_count,
+    init, sync, sm_count, set_stream,
 )
 from . import algorithm  # noqa: F401

@@ -1480,7 +1480,7 @@ int gb200_vector_export_bits(gb200_vector_t v, uint32_t* d_bits,
 int gb200_profile_enable(int on) {
   GB200_REQUIRE_DEVICE();
   graphblas::backend::profiler().enabled = (on != 0);
-  if (on) graphblas::backend::profiler().ensureCells();
+  if (on) graphblas::backend::profiler().ensureCells(graphblas::backend::gbStream());
   return 0;
 }
 

@@ -126,7 +126,7 @@ Info bfsFused(Vector<float>* v, const Matrix<a>* A, Index s, Descriptor* desc, i
   args.trace = bfsTrace();
   args.prof_bytes = NULL;               // the kernel adds its bytes when profiling
   if (profiler().enabled) {
-    profiler().ensureCells();
+    profiler().ensureCells(gbStream());
     args.prof_bytes = profiler().d_cells + GB_PROF_PULL_BOOL;
   }
 

@@ -123,7 +123,7 @@ Info spgemmMasked(SparseMatrix<c>* C, const Matrix<m>* mask, BinaryOpT accum,
       const int grid = runtime().sm_count*8;
       unsigned long long* prof_cell = NULL;
       if (profiler().enabled) {
-        profiler().ensureCells();
+        profiler().ensureCells(gbStream());
         prof_cell = profiler().d_cells + GB_PROF_SPGEMM;
       }
       profiler().begin(GB_PROF_SPGEMM, s);

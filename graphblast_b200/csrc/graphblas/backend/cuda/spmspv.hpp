@@ -193,7 +193,7 @@ Info spmspvMerge(SparseVector<W>* w, const Vector<M>* mask, BinaryOpT accum,
   const int add_kind = static_cast<int>(extractAdd(op)(3, 5));
   unsigned long long* prof_cell = NULL;
   if (profiler().enabled) {
-    profiler().ensureCells();
+    profiler().ensureCells(gbStream());
     prof_cell = profiler().d_cells + GB_PROF_PUSH;
   }
   profiler().begin(GB_PROF_PUSH, s);

@@ -164,7 +164,7 @@ Info spmv(DenseVector<W>* w, const Vector<M>* mask, BinaryOpT accum, SemiringT o
 
       unsigned long long* prof_cell = NULL;
       if (profiler().enabled) {
-        profiler().ensureCells();
+        profiler().ensureCells(gbStream());
         prof_cell = profiler().d_cells + GB_PROF_PULL_BOOL;
       }
 

@@ -71,10 +71,12 @@ struct Profiler {
     for (int k = 0; k < GB_PROF_NKINDS; ++k) { used[k] = 0; host_bytes[k] = 0; }
   }
 
-  void ensureCells() {
+  // The cells are cleared on the stream whose kernels add into them: a clear on the
+  // legacy stream would be unordered with those kernels under a non-blocking stream.
+  void ensureCells(cudaStream_t s) {
     if (d_cells == NULL) {
       CUDA_CALL(cudaMalloc(&d_cells, GB_PROF_NKINDS*sizeof(unsigned long long)));
-      CUDA_CALL(cudaMemset(d_cells, 0, GB_PROF_NKINDS*sizeof(unsigned long long)));
+      CUDA_CALL(cudaMemsetAsync(d_cells, 0, GB_PROF_NKINDS*sizeof(unsigned long long), s));
     }
   }
 
@@ -98,14 +100,16 @@ struct Profiler {
   }
 
   void reset(cudaStream_t s) {
-    ensureCells();
+    ensureCells(s);
     for (int k = 0; k < GB_PROF_NKINDS; ++k) { used[k] = 0; host_bytes[k] = 0; }
     CUDA_CALL(cudaMemsetAsync(d_cells, 0, GB_PROF_NKINDS*sizeof(unsigned long long), s));
   }
 
   // Total milliseconds, launches and bytes of one kind (synchronises).
   void read(int kind, cudaStream_t s, double* ms, long long* launches, double* bytes) {
-    ensureCells();
+    ensureCells(s);
+    unsigned long long cell = 0;
+    CUDA_CALL(cudaMemcpyAsync(&cell, d_cells + kind, sizeof(cell), cudaMemcpyDeviceToHost, s));
     CUDA_CALL(cudaStreamSynchronize(s));
     double total = 0;
     for (size_t i = 0; i < used[kind]; ++i) {
@@ -113,8 +117,6 @@ struct Profiler {
       CUDA_CALL(cudaEventElapsedTime(&t, start[kind][i], stop[kind][i]));
       total += t;
     }
-    unsigned long long cell = 0;
-    CUDA_CALL(cudaMemcpy(&cell, d_cells + kind, sizeof(cell), cudaMemcpyDeviceToHost));
     *ms = total;
     *launches = static_cast<long long>(used[kind]);
     *bytes = host_bytes[kind] + static_cast<double>(cell);
