@@ -166,6 +166,13 @@ SCC_SIGNATURES = [
     ("gb200_scc_stats", _I, [C.POINTER(_LL), C.POINTER(_LL), _IP, _IP]),
 ]
 
+# (name, restype, argtypes) for every symbol declared in include/graphblast_b200_msf.h,
+# the companion header of the minimum spanning forest; load() binds these too.
+MSF_SIGNATURES = [
+    ("gb200_msf", _I, [_P, _P, _P, C.POINTER(_LL), C.POINTER(_D), C.POINTER(_F)]),
+    ("gb200_msf_stats", _I, [_IP, _IP, C.POINTER(_F)]),
+]
+
 
 class ExtensionMissing(RuntimeError):
     pass
@@ -184,7 +191,7 @@ def load():
     lib = C.CDLL(LIB_PATH)
     for name, restype, argtypes in (SIGNATURES + LGC_SIGNATURES + EXTRACT_SIGNATURES +
                                     BC_SIGNATURES + ASSIGN_SIGNATURES + KTRUSS_SIGNATURES +
-                                    SCC_SIGNATURES):
+                                    SCC_SIGNATURES + MSF_SIGNATURES):
         fn = getattr(lib, name)   # AttributeError if a declared symbol is missing
         fn.restype = restype
         fn.argtypes = argtypes

@@ -5,10 +5,11 @@ colouring gc, the maximal independent set mis, the connected components cc and t
 local graph clustering lgc, one kernel each on the device, with lgc_sweep, the
 conductance sweep cut of lgc's result, the betweenness centrality bc, one kernel
 per batch of 32 sources, the k-truss ktruss and truss decomposition trussness, one
-cooperative edge-peeling kernel each, and the strongly connected components scc, one
-cooperative trim, forward-backward and colouring kernel.
+cooperative edge-peeling kernel each, the strongly connected components scc, one
+cooperative trim, forward-backward and colouring kernel, and the minimum spanning
+forest msf, one cooperative Boruvka kernel.
 
-sssp, pr, tc, gc, mis, cc, lgc, lgc_sweep, bc, ktruss, trussness and scc return the device time of the operation
+sssp, pr, tc, gc, mis, cc, lgc, lgc_sweep, bc, ktruss, trussness, scc and msf return the device time of the operation
 loop in milliseconds ("tight" in the reference drivers, example/gbfs.cu:110-115).  bfs returns it only
 when called with timed=True; otherwise it returns None and, when the traversal runs
 as the fused kernel, only enqueues it, so that back-to-back traversals keep the GPU
@@ -233,3 +234,36 @@ def scc_stats():
     t, p, c, b = C.c_longlong(0), C.c_longlong(0), C.c_int(0), C.c_int(0)
     _lib.load().gb200_scc_stats(C.byref(t), C.byref(p), C.byref(c), C.byref(b))
     return t.value, p.value, c.value, b.value
+
+
+def msf(F, A, desc):
+    """F = the minimum spanning forest of the undirected graph G with the edge {i, j},
+    i != j, when A(i,j) or A(j,i) is stored, weighted by the smaller of the stored
+    values among A(i,j) and A(j,i).  Self-loops are ignored; stored zeros are edges of
+    weight 0 (scipy treats explicit zeros as missing).  Only A's CSR is read.  Edges are
+    ranked by (w, min(i,j), max(i,j)): numbers compare as numbers, -0.0 equal to +0.0,
+    +-inf allowed, INT32 as signed integers.  The order is strict and total, so the
+    forest is unique: Kruskal's forest under it.  F is n x n, replaced, a sorted CSR
+    installed as symmetric with F(i,j) = F(j,i) = w({i,j}) (-0.0 written as +0.0), of
+    A's element type, and may be A; two calls give identical bytes.  An FP32 A with a
+    NaN on a stored off-diagonal entry raises GrB_INVALID_VALUE
+    (include/graphblas/algorithm/msf.hpp).  Returns (nedges, weight, tight_ms): the
+    undirected forest edges (n minus the number of trees) and their fp64 sum, taken in
+    an order that depends only on the forest (exact while every partial sum is an
+    integer below 2^53)."""
+    ms = C.c_float(0)
+    count = C.c_longlong(0)
+    weight = C.c_double(0)
+    _check(_lib.load().gb200_msf(F._h, A._h, desc._h, C.byref(count), C.byref(weight),
+                                 C.byref(ms)),
+           "algorithm::msf")
+    return count.value, weight.value, ms.value
+
+
+def msf_stats():
+    """(rounds, barriers, canon_ms) of the last msf call of this process: the Boruvka
+    rounds, at most ceil(log2 n) + 1, the grid barriers of the kernel, and the device
+    time of building the canonical edge list in milliseconds."""
+    rounds, barriers, canon = C.c_int(0), C.c_int(0), C.c_float(0)
+    _lib.load().gb200_msf_stats(C.byref(rounds), C.byref(barriers), C.byref(canon))
+    return rounds.value, barriers.value, canon.value

@@ -31,6 +31,7 @@
 #include "graphblas/algorithm/bc.hpp"
 #include "graphblas/algorithm/ktruss.hpp"
 #include "graphblas/algorithm/scc.hpp"
+#include "graphblas/algorithm/msf.hpp"
 
 #include "graphblast_b200.h"
 #include "graphblast_b200_lgc.h"
@@ -39,6 +40,7 @@
 #include "graphblast_b200_assign.h"
 #include "graphblast_b200_ktruss.h"
 #include "graphblast_b200_scc.h"
+#include "graphblast_b200_msf.h"
 
 bool debug_;
 bool memory_;
@@ -1298,6 +1300,35 @@ int gb200_scc_stats(long long* trimmed, long long* pivot_size, int* colour_itera
   if (pivot_size) *pivot_size = stats.pivot_size;
   if (colour_iterations) *colour_iterations = stats.colour_iterations;
   if (barriers) *barriers = stats.barriers;
+  return 0;
+}
+
+// ---- minimum spanning forest (include/graphblast_b200_msf.h) ----------------------
+
+int gb200_msf(gb200_matrix_t F, gb200_matrix_t A, gb200_desc_t desc, long long* nedges,
+              double* weight, float* tight_ms) {
+  if (F == NULL || A == NULL || desc == NULL)
+    return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
+  if ((F->f == NULL && F->i == NULL) || (A->f == NULL && A->i == NULL) ||
+      (F->f == NULL) != (A->f == NULL))
+    return rc(graphblas::GrB_DOMAIN_MISMATCH);
+  GB200_REQUIRE_DEVICE();
+  graphblas::Index count = 0;
+  double total = 0.0;
+  const int info = runAlgorithm(tight_ms, [&] {
+    return A->f != NULL ? graphblas::algorithm::msf(F->f, A->f, &desc->desc, &count, &total)
+                        : graphblas::algorithm::msf(F->i, A->i, &desc->desc, &count, &total);
+  });
+  if (info == 0 && nedges) *nedges = count;
+  if (info == 0 && weight) *weight = total;
+  return info;
+}
+
+int gb200_msf_stats(int* rounds, int* barriers, float* canon_ms) {
+  const graphblas::backend::MsfStats& stats = graphblas::backend::msfLastStats();
+  if (rounds) *rounds = stats.rounds;
+  if (barriers) *barriers = stats.barriers;
+  if (canon_ms) *canon_ms = stats.canon_ms;
   return 0;
 }
 

@@ -47,6 +47,7 @@
 #include "graphblas/backend/cuda/bc.hpp"
 #include "graphblas/backend/cuda/ktruss.hpp"
 #include "graphblas/backend/cuda/scc.hpp"
+#include "graphblas/backend/cuda/msf.hpp"
 
 namespace graphblas {
 namespace backend {
