@@ -1268,7 +1268,7 @@ int gb200_trussness(gb200_matrix_t T, gb200_matrix_t A, gb200_desc_t desc, int* 
 }
 
 int gb200_ktruss_stats(int* rounds, int* levels, float* support_ms) {
-  const graphblas::backend::KtrussStats& stats = graphblas::backend::ktrussLastStats();
+  const auto& stats = graphblas::backend::lastStats<graphblas::backend::KtrussStats>();
   if (rounds) *rounds = stats.rounds;
   if (levels) *levels = stats.levels;
   if (support_ms) *support_ms = stats.support_ms;
@@ -1295,7 +1295,7 @@ int gb200_scc(gb200_vector_t v, gb200_matrix_t A, gb200_desc_t desc, int* ncompo
 
 int gb200_scc_stats(long long* trimmed, long long* pivot_size, int* colour_iterations,
                     int* barriers) {
-  const graphblas::backend::SccStats& stats = graphblas::backend::sccLastStats();
+  const auto& stats = graphblas::backend::lastStats<graphblas::backend::SccStats>();
   if (trimmed) *trimmed = stats.trimmed;
   if (pivot_size) *pivot_size = stats.pivot_size;
   if (colour_iterations) *colour_iterations = stats.colour_iterations;
@@ -1325,7 +1325,7 @@ int gb200_msf(gb200_matrix_t F, gb200_matrix_t A, gb200_desc_t desc, long long* 
 }
 
 int gb200_msf_stats(int* rounds, int* barriers, float* canon_ms) {
-  const graphblas::backend::MsfStats& stats = graphblas::backend::msfLastStats();
+  const auto& stats = graphblas::backend::lastStats<graphblas::backend::MsfStats>();
   if (rounds) *rounds = stats.rounds;
   if (barriers) *barriers = stats.barriers;
   if (canon_ms) *canon_ms = stats.canon_ms;

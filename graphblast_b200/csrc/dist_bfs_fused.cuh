@@ -100,7 +100,7 @@ static_assert((GBX_CELL_TRACE + GBX_TRACE_STRIDE*(GBX_TRACE_LEVELS - 1) + GBX_T_
 
 #define GBX_TRACE(slot) do {                                                         \
   if (gtid == 0 && level < GBX_TRACE_LEVELS)                                         \
-    a.cells[GBX_CELL_TRACE + GBX_TRACE_STRIDE*level + (slot)] = bfsClockNs();        \
+    a.cells[GBX_CELL_TRACE + GBX_TRACE_STRIDE*level + (slot)] = globalTimerNs();     \
 } while (0)
 
 __global__ void __launch_bounds__(GBX_BFS_NT, 2)
@@ -211,7 +211,7 @@ bfsFusedDistKernel(BfsDistArgs a) {
         }
       }
       grid.sync();
-      unsigned long long nheavy = *reinterpret_cast<volatile unsigned long long*>(heavy_cell);
+      unsigned long long nheavy = loadCell(heavy_cell);
       if (nheavy > GB_BFS_HEAVY_CAP) nheavy = GB_BFS_HEAVY_CAP;
       for (unsigned long long h = 0; h < nheavy; ++h) {
         const Index u = a.heavy[h];
@@ -328,8 +328,7 @@ bfsFusedDistKernel(BfsDistArgs a) {
       if (atomicAdd(done_cell, 1ull) == gridDim.x - 1) {
         bfsZeroNextCell(a.cells, GBX_CELL_CHECKIN, level);
         __threadfence();
-        const unsigned long long mine =
-            *reinterpret_cast<volatile unsigned long long*>(found_cell);
+        const unsigned long long mine = loadCell(found_cell);
         // one word per rank carries the epoch and this rank's count
         const unsigned long long word = (epoch << 32) | (mine & 0xffffffffull);
         for (int p = 0; p < a.world; ++p)

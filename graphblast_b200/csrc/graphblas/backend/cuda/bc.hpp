@@ -71,8 +71,8 @@ Info bcRun(Vector<float>* v, const Matrix<a>* A, const Index* sources, Index nso
                                 cudaMemcpyHostToDevice, stream));
     BcArgs args;
     args.row_ptr = g.row_ptr;  args.row_ind = g.row_ind;
-    args.in_ptr = g.col_ptr != NULL ? g.col_ptr : g.row_ptr;
-    args.in_ind = g.col_ptr != NULL ? g.col_ind : g.row_ind;
+    args.in_ptr = g.in_ptr();
+    args.in_ind = g.in_ind();
     args.n = n;
     args.sources = sources != NULL ? block.at<Index>(src) : NULL;
     args.seen = block.at<unsigned int>(seen);

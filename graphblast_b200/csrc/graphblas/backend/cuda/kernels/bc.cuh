@@ -54,7 +54,7 @@
 
 #include <cooperative_groups.h>
 
-#include "graphblas/backend/cuda/kernels/common.cuh"
+#include "graphblas/backend/cuda/kernels/cooperative.cuh"
 
 namespace graphblas {
 namespace backend {
@@ -90,10 +90,6 @@ struct BcArgs {
   int* ticket;                   // [partial slots] chunks done; 0 between uses
   unsigned long long* counters;  // [BC_NCELLS] BcCell
 };
-
-__device__ __forceinline__ unsigned long long bcCell(const BcArgs& a, int cell) {
-  return *reinterpret_cast<volatile unsigned long long*>(a.counters + cell);
-}
 
 // The number of entries a level list gives v: one per GB_BC_CHUNK of its longer list.
 __device__ __forceinline__ int bcChunks(const BcArgs& a, Index v) {
@@ -197,7 +193,7 @@ bcKernel(BcArgs a) {
   grid.sync();
 
   Index lo = 0;
-  Index hi = static_cast<Index>(bcCell(a, BC_ENTRIES));
+  Index hi = static_cast<Index>(loadCell(a.counters + BC_ENTRIES));
   if (gtid == 0) {
     a.level_start[0] = 0;
     a.counters[BC_PSLOTS] = 0ull;
@@ -240,7 +236,7 @@ bcKernel(BcArgs a) {
       }
     }
     grid.sync();
-    const Index next = static_cast<Index>(bcCell(a, BC_ENTRIES));
+    const Index next = static_cast<Index>(loadCell(a.counters + BC_ENTRIES));
     if (next == hi) break;
     if (gtid == 0) {
       a.level_start[d + 1] = hi;

@@ -63,7 +63,7 @@
 
 #include <cooperative_groups.h>
 
-#include "graphblas/backend/cuda/kernels/common.cuh"
+#include "graphblas/backend/cuda/kernels/cooperative.cuh"
 
 namespace graphblas {
 namespace backend {
@@ -186,12 +186,6 @@ __device__ __forceinline__ unsigned long long* bfsLevelCell(unsigned long long* 
 __device__ __forceinline__ void bfsZeroNextCell(unsigned long long* cells, int first,
                                                 int level) {
   cells[first + (level + 1) % 3] = 0ull;
-}
-
-__device__ __forceinline__ unsigned long long bfsClockNs() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return t;
 }
 
 // Sets vertex vtx's bit in visited; true for the one thread that set it.  V: the
@@ -365,7 +359,7 @@ bfsFusedKernel(BfsFusedArgs a) {
   const Index gwarps = gthreads >> 5;
   const Index nchunks = (nwords + 31) >> 5;               // pull chunks of 32 words
 
-  if (gtid == 0) a.counters[GB_BFS_CELL_START_CLOCK] = bfsClockNs();
+  if (gtid == 0) a.counters[GB_BFS_CELL_START_CLOCK] = globalTimerNs();
   // ---- level 0: clear the bitmaps, mark the source visited (v is written once per
   // row, after the last level) ------------------------------------------------------------
   // F is not seeded: a push at level 1 expands the source without reading F, a pull
@@ -386,7 +380,7 @@ bfsFusedKernel(BfsFusedArgs a) {
   if (gtid >= GB_BFS_CELL_WALKED && gtid < GB_BFS_CELL_WALKED + GB_BFS_TIMED_LEVELS)
     a.counters[gtid] = 0ull;
   grid.sync();
-  if (gtid == 0) a.counters[GB_BFS_CELL_LEVEL_CLOCK] = bfsClockNs() << 2;
+  if (gtid == 0) a.counters[GB_BFS_CELL_LEVEL_CLOCK] = globalTimerNs() << 2;
 
   int vsel = 0;                           // bfsVis / bfsVisOther
   int fsel = 0;                           // bfsF / bfsN
@@ -674,10 +668,10 @@ bfsFusedKernel(BfsFusedArgs a) {
       // After the main phase: heavy vertices listed pushing, chunks listed pulling.
       // Every add to the cell came before the barrier, so every thread reads the
       // same value and takes the same branch.
-      const unsigned long long listed = phase ? 0ull : *reinterpret_cast<volatile unsigned long long*>(
+      const unsigned long long listed = phase ? 0ull : loadCell(
           bfsLevelCell(a.counters, dense ? GB_BFS_CELL_LISTED : GB_BFS_CELL_HEAVY, level));
       if (gtid == 0 && level < GB_BFS_TIMED_LEVELS) {
-        const unsigned long long t = bfsClockNs();
+        const unsigned long long t = globalTimerNs();
         if (dense && phase == 0) {
           a.counters[GB_BFS_CELL_SCAN_CLOCK + level] = t;
           if (a.trace) a.counters[GB_BFS_CELL_LISTED_CHUNKS + level] = listed;
@@ -719,12 +713,11 @@ bfsFusedKernel(BfsFusedArgs a) {
       }
     }
     // ---- frontier size of the next level ------------------------------------------
-    fcount = static_cast<unsigned int>(
-        *reinterpret_cast<volatile unsigned long long*>(count_cell));
+    fcount = static_cast<unsigned int>(loadCell(count_cell));
     if (dense) vsel ^= 1;
     fsel ^= 1;
   }
-  if (gtid == 0) a.counters[GB_BFS_CELL_LAST_LEVEL_CLOCK] = bfsClockNs();
+  if (gtid == 0) a.counters[GB_BFS_CELL_LAST_LEVEL_CLOCK] = globalTimerNs();
   // ---- v, every row once, in full lines ----------------------------------------
   // A row is reached when it is visited now and not only because nothing points at
   // it (the source is reached).  A traversal cut off after max_levels (the frontier
@@ -859,7 +852,7 @@ bfsFusedKernel(BfsFusedArgs a) {
   }
   if (a.trace) {
     grid.sync();                  // only to time the end pass: not counted in the barriers
-    if (gtid == 0) a.counters[GB_BFS_CELL_END_PASS_CLOCK] = bfsClockNs();
+    if (gtid == 0) a.counters[GB_BFS_CELL_END_PASS_CLOCK] = globalTimerNs();
   }
   // ---- results: the work counters, the algorithmic bytes of SURVEY.md §8d --------
   const int block_insp = blockSum<NT>(inspected, s_red);
@@ -896,8 +889,7 @@ bfsFusedKernel(BfsFusedArgs a) {
       if (blockIdx.x == 0)
         bytes += static_cast<unsigned long long>(pull_levels)*
                      (12ull*static_cast<unsigned long long>(n) + 4ull) +
-                 8ull*(*reinterpret_cast<volatile unsigned long long*>(
-                           a.counters + GB_BFS_CELL_FOUND_PUSHING));
+                 8ull*loadCell(a.counters + GB_BFS_CELL_FOUND_PUSHING);
       if (bytes) atomicAdd(a.prof_bytes, bytes);
     }
   }

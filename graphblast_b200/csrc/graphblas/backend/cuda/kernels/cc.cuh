@@ -19,8 +19,8 @@
 //     only if it still holds p); g is in x's tree, so no tree is cut.
 //   compress — parent[v] = root(v), plain (relaxed) stores, between grid barriers with
 //     no link in flight.
-// parent[] is read with ld.relaxed.gpu (L2), never through the non-coherent path: a
-// word other SMs hook or halve while the kernel runs must not be read stale from L1.
+// parent[] is read with ldRelaxed: other SMs hook and halve it while the kernel runs
+// (the memory model of cooperative.cuh).
 //
 // Phases (grid barriers between them):
 //   init      parent[v] = v.
@@ -51,7 +51,7 @@
 
 #include <cooperative_groups.h>
 
-#include "graphblas/backend/cuda/kernels/common.cuh"
+#include "graphblas/backend/cuda/kernels/cooperative.cuh"
 
 namespace graphblas {
 namespace backend {
@@ -79,22 +79,12 @@ struct CcArgs {
   unsigned long long* counters;  // [CC_NCELLS] CcCell
 };
 
-__device__ __forceinline__ Index ccLoad(const Index* p) {
-  Index x;
-  asm volatile("ld.relaxed.gpu.global.s32 %0, [%1];" : "=r"(x) : "l"(p));
-  return x;
-}
-
-__device__ __forceinline__ void ccStore(Index* p, Index x) {
-  asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" :: "l"(p), "r"(x) : "memory");
-}
-
 // The root of x, halving the path on the way by CAS.
 __device__ __forceinline__ Index ccFind(Index* parent, Index x) {
   while (true) {
-    const Index p = ccLoad(parent + x);
+    const Index p = ldRelaxed(parent + x);
     if (p == x) return x;
-    const Index g = ccLoad(parent + p);
+    const Index g = ldRelaxed(parent + p);
     if (g == p) return p;
     atomicCAS(parent + x, p, g);       // only if parent[x] still holds p
     x = g;
@@ -116,12 +106,12 @@ __device__ __forceinline__ void ccLink(Index* parent, Index u, Index v) {
   }
 }
 
-// parent[v] = root(v) for v = first, first + stride, ...; no link is in flight.
-__device__ __forceinline__ void ccCompress(const CcArgs& a, Index first, Index stride) {
-  for (Index v = first; v < a.n; v += stride) {
-    Index r = ccLoad(a.parent + v);
-    for (Index p = ccLoad(a.parent + r); p != r; p = ccLoad(a.parent + r)) r = p;
-    ccStore(a.parent + v, r);
+// parent[v] = root(v) for v = first, first + stride, ... below n; no link is in flight.
+__device__ __forceinline__ void ccCompress(Index* parent, Index n, Index first, Index stride) {
+  for (Index v = first; v < n; v += stride) {
+    Index r = ldRelaxed(parent + v);
+    for (Index p = ldRelaxed(parent + r); p != r; p = ldRelaxed(parent + r)) r = p;
+    stRelaxed(parent + v, r);
   }
 }
 
@@ -138,7 +128,7 @@ __device__ __forceinline__ Index ccSample(const CcArgs& a) {
   for (int i = threadIdx.x; i < GB_CC_SAMPLES; i += GB_CC_NT) {
     const Index v = static_cast<Index>(fmix32(static_cast<unsigned int>(i)) %
                                        static_cast<unsigned int>(a.n));
-    const Index r = ccLoad(a.parent + v);
+    const Index r = ldRelaxed(a.parent + v);
     unsigned int slot = fmix32(static_cast<unsigned int>(r)) & (GB_CC_SLOTS - 1);
     while (true) {
       const Index k = atomicCAS(keys + slot, -1, r);
@@ -167,7 +157,7 @@ ccKernel(CcArgs a, W* out) {
   const Index gwarps = gthreads >> 5;
 
   // ---- init --------------------------------------------------------------------------
-  for (Index v = gtid; v < a.n; v += gthreads) ccStore(a.parent + v, v);
+  for (Index v = gtid; v < a.n; v += gthreads) stRelaxed(a.parent + v, v);
   grid.sync();
 
   if (a.row_ptr != NULL) {
@@ -178,7 +168,7 @@ ccKernel(CcArgs a, W* out) {
         if (__ldg(a.row_ptr + v + 1) - b > r) ccLink(a.parent, v, __ldg(a.row_ind + b + r));
       }
       grid.sync();
-      ccCompress(a, gtid, gthreads);
+      ccCompress(a.parent, a.n, gtid, gthreads);
       grid.sync();
     }
 
@@ -188,14 +178,13 @@ ccKernel(CcArgs a, W* out) {
       if (threadIdx.x == 0) a.counters[CC_LARGEST] = static_cast<unsigned long long>(L);
     }
     if (a.skip) grid.sync();
-    const Index L = a.skip ? static_cast<Index>(
-        *reinterpret_cast<volatile unsigned long long*>(a.counters + CC_LARGEST)) : -1;
+    const Index L = a.skip ? static_cast<Index>(loadCell(a.counters + CC_LARGEST)) : -1;
 
     // ---- finish: entries from position 2 on, a lane or a warp per list ---------------
     for (Index i0 = gwarp*32; i0 < a.n; i0 += gwarps*32) {
       const Index v = i0 + lane;
       Index b = 0, e = 0;
-      if (v < a.n && (L < 0 || ccLoad(a.parent + v) != L)) {
+      if (v < a.n && (L < 0 || ldRelaxed(a.parent + v) != L)) {
         b = __ldg(a.row_ptr + v) + 2;
         e = __ldg(a.row_ptr + v + 1);
         if (e < b) e = b;
@@ -240,7 +229,7 @@ ccKernel(CcArgs a, W* out) {
   unsigned int roots = 0u;
   for (Index v = gtid; v < a.n; v += gthreads) {
     Index r = v;
-    for (Index p = ccLoad(a.parent + r); p != r; p = ccLoad(a.parent + r)) r = p;
+    for (Index p = ldRelaxed(a.parent + r); p != r; p = ldRelaxed(a.parent + r)) r = p;
     out[v] = static_cast<W>(r);
     roots += r == v ? 1u : 0u;
   }

@@ -36,7 +36,7 @@ namespace backend {
 
 struct ColorStep {
   static __device__ __forceinline__ int poll(const GreedyArgs a, Index v, Index waiting) {
-    return waiting >= 0 && gcLoadState(a.state + waiting) == 0u ? GREEDY_BLOCKED
+    return waiting >= 0 && ldRelaxed(a.state + waiting) == 0u ? GREEDY_BLOCKED
                                                                  : GREEDY_ATTEMPT;
   }
 
@@ -55,7 +55,7 @@ struct ColorStep {
       if (k < len) {
         const Index x = gcEntry(a, l, k);
         if (gcAbove(gcHash(a.seed, static_cast<unsigned int>(x)), x, hv, v) &&
-            gcLoadState(a.state + x) == 0u)
+            ldRelaxed(a.state + x) == 0u)
           u = x;
       }
       int src = 0;
@@ -78,7 +78,7 @@ struct ColorStep {
 #pragma unroll 4
       for (Index k = me; k < len; k += G) {
         const Index x = gcEntry(a, l, k);
-        const unsigned int c = gcLoadState(a.state + x);
+        const unsigned int c = ldRelaxed(a.state + x);
         if (c == 0u && base == 0u &&
             gcAbove(gcHash(a.seed, static_cast<unsigned int>(x)), x, hv, v))
           stale = x;
@@ -105,7 +105,7 @@ struct ColorStep {
       }
       if (~used != 0ull) {
         if (me == 0)
-          gcStoreState(a.state + v, base + static_cast<unsigned int>(
+          stRelaxed(a.state + v, base + static_cast<unsigned int>(
                                                __ffsll(static_cast<long long>(~used))));
         return true;
       }

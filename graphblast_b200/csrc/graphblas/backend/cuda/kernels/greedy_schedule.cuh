@@ -36,12 +36,14 @@
 //     each), and attempts the ones that poll ATTEMPT together, one at a time, until all
 //     its vertices are decided; it sleeps briefly only when none is ready.
 //   out — after one more barrier, the step's out pass.
+// Steps read and write the per-vertex state with ldRelaxed / stRelaxed (the memory model
+// of cooperative.cuh): a blocked vertex re-reads states that other SMs store.
 #ifndef GRAPHBLAS_BACKEND_CUDA_KERNELS_GREEDY_SCHEDULE_CUH_
 #define GRAPHBLAS_BACKEND_CUDA_KERNELS_GREEDY_SCHEDULE_CUH_
 
 #include <cooperative_groups.h>
 
-#include "graphblas/backend/cuda/kernels/common.cuh"
+#include "graphblas/backend/cuda/kernels/cooperative.cuh"
 
 namespace graphblas {
 namespace backend {
@@ -79,21 +81,6 @@ __host__ __device__ __forceinline__ unsigned int gcHash(unsigned int seed, unsig
 // p(u) > p(v)
 __device__ __forceinline__ bool gcAbove(unsigned int hu, Index u, unsigned int hv, Index v) {
   return hu > hv || (hu == hv && u > v);
-}
-
-// State loads MUST NOT go through the non-coherent path (__ldg, ld.global.nc): a
-// vertex re-reads states that other SMs store while the kernel runs, and a
-// non-coherent load may keep returning a stale 0 from L1 for as long as the line
-// stays there, so a blocked vertex would never see its blocker decided.
-// ld.relaxed.gpu reads at GPU scope (L2); volatile keeps every re-read in the loop.
-__device__ __forceinline__ unsigned int gcLoadState(const unsigned int* p) {
-  unsigned int c;
-  asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(c) : "l"(p));
-  return c;
-}
-
-__device__ __forceinline__ void gcStoreState(unsigned int* p, unsigned int c) {
-  asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" :: "l"(p), "r"(c) : "memory");
 }
 
 // A vertex's list: its CSR row, then its CSC column (dc = 0 when symmetric).
@@ -171,7 +158,7 @@ __device__ __forceinline__ void greedySchedule(const GreedyArgs a, W* out) {
       }
     }
     grid.sync();
-    m = static_cast<Index>(*reinterpret_cast<volatile unsigned long long*>(count));
+    m = static_cast<Index>(loadCell(count));
     in = next;
     ++s;
   }

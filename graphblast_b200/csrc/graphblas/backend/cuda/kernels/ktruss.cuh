@@ -48,7 +48,7 @@
 
 #include <cooperative_groups.h>
 
-#include "graphblas/backend/cuda/kernels/common.cuh"
+#include "graphblas/backend/cuda/kernels/cooperative.cuh"
 
 namespace graphblas {
 namespace backend {
@@ -150,18 +150,6 @@ __device__ __forceinline__ void ktAppend(const KtArgs& a, bool want, Index f, in
   for (int c = 0; c < nch; ++c) a.items[base + c] = make_int2(f, c);
 }
 
-// The items counted for the frontier of `round`; read after the barrier that ends its
-// appends.
-__device__ __forceinline__ Index ktCount(const KtArgs& a, int round) {
-  return *reinterpret_cast<volatile int*>(a.cells + KT_COUNT + round % 3);
-}
-
-__device__ __forceinline__ unsigned long long ktNow() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
-
 // Decrements the support of f; true when f crossed below k - 2 here.
 __device__ __forceinline__ bool ktDrop(const KtArgs& a, Index f, int k) {
   return atomicSub(a.sup + f, 1) == k - 2;
@@ -176,7 +164,7 @@ ktrussKernel(KtArgs a) {
   const Index gthreads = gridDim.x*GB_KT_NT;
   const Index gwarp = gtid >> 5;
   const Index gwarps = gthreads >> 5;
-  const unsigned long long t0 = gtid == 0 ? ktNow() : 0ull;
+  const unsigned long long t0 = gtid == 0 ? globalTimerNs() : 0ull;
 
   // ---- support: every item of every edge ---------------------------------------------
   for (Index t = gwarp; t < a.nitems; t += gwarps) {
@@ -190,7 +178,7 @@ ktrussKernel(KtArgs a) {
     if (lane == 0 && count > 0) atomicAdd(a.sup + e.x, count);
   }
   grid.sync();
-  if (gtid == 0) a.cells[KT_SUPPORT_US] = static_cast<int>((ktNow() - t0)/1000ull);
+  if (gtid == 0) a.cells[KT_SUPPORT_US] = static_cast<int>((globalTimerNs() - t0)/1000ull);
 
   // ---- peel ----------------------------------------------------------------------------
   const bool truss = a.k == 0;
@@ -210,7 +198,7 @@ ktrussKernel(KtArgs a) {
       if (lane == 0 && m != INT_MAX) atomicMin(a.cells + KT_MIN + (level & 1), m);
       if (gtid == 0) a.cells[KT_MIN + ((level + 1) & 1)] = INT_MAX;
       grid.sync();
-      m = *reinterpret_cast<volatile int*>(a.cells + KT_MIN + (level & 1));
+      m = loadCell(a.cells + KT_MIN + (level & 1));
       if (m == INT_MAX) break;
       k = m + 3;
     }
@@ -221,7 +209,7 @@ ktrussKernel(KtArgs a) {
       ktAppend(a, want, p, r, lo);
     }
     grid.sync();
-    Index hi = lo + ktCount(a, r);
+    Index hi = lo + loadCell(a.cells + KT_COUNT + r % 3);
     if (hi > lo && gtid == 0) {
       a.cells[KT_LEVELS] += 1;
       a.cells[KT_KMAX] = k - 1;
@@ -257,7 +245,7 @@ ktrussKernel(KtArgs a) {
       grid.sync();
       ++r;
       lo = hi;
-      hi = lo + ktCount(a, r);
+      hi = lo + loadCell(a.cells + KT_COUNT + r % 3);
     }
     ++level;
     if (!truss) break;

@@ -55,7 +55,7 @@
 
 #include <cooperative_groups.h>
 
-#include "graphblas/backend/cuda/kernels/common.cuh"
+#include "graphblas/backend/cuda/kernels/cooperative.cuh"
 
 namespace graphblas {
 namespace backend {
@@ -94,10 +94,6 @@ struct LgcArgs {
   Index* touched;                // [n] the touched list of a sparse round
   unsigned long long* counters;  // [LGC_NCELLS] LgcCell
 };
-
-__device__ __forceinline__ unsigned long long lgcCell(const LgcArgs& a, int cell) {
-  return *reinterpret_cast<volatile unsigned long long*>(a.counters + cell);
-}
 
 // The lanes with `want` append x to list at counter *count, one atomic per warp; every
 // lane of the warp calls it.  Returns nothing; *count grows by the number of wanting lanes.
@@ -235,9 +231,9 @@ lgcKernel(LgcArgs a) {
 
   int k = 0;
   for (; k < a.max_rounds; ++k) {
-    const Index nf = static_cast<Index>(lgcCell(a, LGC_FCOUNT + k % 3));
+    const Index nf = static_cast<Index>(loadCell(a.counters + LGC_FCOUNT + k % 3));
     if (nf == 0) break;
-    const unsigned long long vol = lgcCell(a, LGC_FVOL + k % 3);
+    const unsigned long long vol = loadCell(a.counters + LGC_FVOL + k % 3);
     const bool dense = a.mode == 2 ||
         (a.mode == 0 && static_cast<double>(vol) >
                         static_cast<double>(a.switchpoint)*static_cast<double>(a.nnz));
@@ -286,7 +282,7 @@ lgcKernel(LgcArgs a) {
     if (dense)
       lgcPull<true>(a, k, a.n, gwarp, gwarps, lane);
     else
-      lgcPull<false>(a, k, static_cast<Index>(lgcCell(a, LGC_TCOUNT + (k & 1))),
+      lgcPull<false>(a, k, static_cast<Index>(loadCell(a.counters + LGC_TCOUNT + (k & 1))),
                      gwarp, gwarps, lane);
     grid.sync();
   }

@@ -68,12 +68,12 @@ __global__ void misInitSparseKernel(unsigned int* __restrict__ state,
 
 struct MisStep {
   static __device__ __forceinline__ int poll(const GreedyArgs a, Index v, Index waiting) {
-    if (gcLoadState(a.state + v) != MIS_UNDECIDED) return GREEDY_DONE;
+    if (ldRelaxed(a.state + v) != MIS_UNDECIDED) return GREEDY_DONE;
     if (waiting >= 0) {
-      const unsigned int b = gcLoadState(a.state + waiting);
+      const unsigned int b = ldRelaxed(a.state + waiting);
       if (b == MIS_UNDECIDED) return GREEDY_BLOCKED;
       if (b == MIS_IN) {
-        gcStoreState(a.state + v, MIS_OUT);
+        stRelaxed(a.state + v, MIS_OUT);
         return GREEDY_DONE;
       }
     }
@@ -95,12 +95,12 @@ struct MisStep {
       if (k < len) {
         x = gcEntry(a, l, k);
         if (gcAbove(gcHash(a.seed, static_cast<unsigned int>(x)), x, hv, v))
-          s = gcLoadState(a.state + x);
+          s = ldRelaxed(a.state + x);
       }
       int src = 0;
       if (G == 32) {
         if (__ballot_sync(GB_FULL_MASK, s == MIS_IN) != 0u) {
-          if (me == 0) gcStoreState(a.state + v, MIS_OUT);
+          if (me == 0) stRelaxed(a.state + v, MIS_OUT);
           return true;
         }
         const unsigned int m = __ballot_sync(GB_FULL_MASK, s == MIS_UNDECIDED);
@@ -108,7 +108,7 @@ struct MisStep {
         src = __ffs(m) - 1;
         x = __shfl_sync(GB_FULL_MASK, x, src);
       } else if (s == MIS_IN) {
-        gcStoreState(a.state + v, MIS_OUT);
+        stRelaxed(a.state + v, MIS_OUT);
         return true;
       } else if (s != MIS_UNDECIDED) {
         continue;
@@ -117,11 +117,11 @@ struct MisStep {
       resume = k0 + src;
       return false;
     }
-    if (me == 0) gcStoreState(a.state + v, MIS_IN);
+    if (me == 0) stRelaxed(a.state + v, MIS_IN);
     for (Index k = me; k < len; k += G) {
       const Index x = gcEntry(a, l, k);
       if (gcAbove(hv, v, gcHash(a.seed, static_cast<unsigned int>(x)), x))
-        gcStoreState(a.state + x, MIS_OUT);
+        stRelaxed(a.state + x, MIS_OUT);
     }
     return true;
   }

@@ -30,17 +30,17 @@
 // to cell (r + 1) % 3, and clears cell (r + 2) % 3, which no thread reads again before
 // round r + 2's appends.  So every thread runs the same rounds.
 //
-// Memory model.  parent[] is read with ccLoad (ld.relaxed.gpu) and best[] with __ldcg,
-// both from L2, never through L1: other SMs write them while the kernel runs, and a
-// stale best word would skip a smaller pick.  The canonical list, which nothing writes,
-// is read through the non-coherent path.
+// Memory model (cooperative.cuh).  parent[] is read with ldRelaxed and best[] with
+// __ldcg, both from L2: other SMs write them while the kernel runs, and a stale best
+// word would skip a smaller pick.  The canonical list, which nothing writes, is read
+// through the non-coherent path.
 #ifndef GRAPHBLAS_BACKEND_CUDA_KERNELS_MSF_CUH_
 #define GRAPHBLAS_BACKEND_CUDA_KERNELS_MSF_CUH_
 
 #include <cooperative_groups.h>
 
 #include "graphblas/backend/cuda/kernels/cc.cuh"
-#include "graphblas/backend/cuda/kernels/scc.cuh"
+#include "graphblas/backend/cuda/kernels/cooperative.cuh"
 
 namespace graphblas {
 namespace backend {
@@ -69,10 +69,6 @@ struct MsfArgs {
   int* forest;                         // [m] 1 on the slots of forest edges
   unsigned long long* counters;        // [MSF_NCELLS] MsfCell
 };
-
-__device__ __forceinline__ unsigned long long msfCell(const MsfArgs& a, int cell) {
-  return *reinterpret_cast<volatile unsigned long long*>(a.counters + cell);
-}
 
 // Order-preserving bits of a weight: the unsigned order of the bits is the numeric
 // order of the weights.  Floats: -0.0 is +0.0 first; negative values have every bit
@@ -162,21 +158,18 @@ msfKernel(MsfArgs a) {
   const Index gtid = blockIdx.x*GB_MSF_NT + threadIdx.x;
   const Index gthreads = gridDim.x*GB_MSF_NT;
   const bool leader = gtid == 0;
-  CcArgs cc = {};
-  cc.n = a.n;
-  cc.parent = a.parent;
   int barriers = 0, rounds = 0;
 
   // ---- init --------------------------------------------------------------------------
   for (Index v = gtid; v < a.n; v += gthreads) {
-    ccStore(a.parent + v, v);
+    stRelaxed(a.parent + v, v);
     a.best[v] = MSF_NONE;
   }
   grid.sync();
   ++barriers;
 
   for (int r = 0;; ++r) {
-    const Index len = static_cast<Index>(msfCell(a, MSF_LIVE + r % 3));
+    const Index len = static_cast<Index>(loadCell(a.counters + MSF_LIVE + r % 3));
     if (len == 0) break;
     ++rounds;
     const Index* in = (r & 1) ? a.live1 : a.live0;
@@ -187,10 +180,10 @@ msfKernel(MsfArgs a) {
     // ---- pick --------------------------------------------------------------------------
     for (Index i = gtid; i < len; i += gthreads) {
       const Index s = r == 0 ? i : __ldcg(in + i);
-      const Index ru = ccLoad(a.parent + __ldg(a.eu + s));
-      const Index rv = ccLoad(a.parent + __ldg(a.ev + s));
+      const Index ru = ldRelaxed(a.parent + __ldg(a.eu + s));
+      const Index rv = ldRelaxed(a.parent + __ldg(a.ev + s));
       if (ru == rv) continue;
-      sccAppend(out, 0, next, s);
+      warpAppend(out, 0, next, s);
       const unsigned long long key =
           (static_cast<unsigned long long>(__ldg(a.ew + s)) << 32) | static_cast<unsigned int>(s);
       if (key < __ldcg(a.best + ru)) atomicMin(a.best + ru, key);
@@ -198,7 +191,7 @@ msfKernel(MsfArgs a) {
     }
     grid.sync();
     ++barriers;
-    if (msfCell(a, MSF_LIVE + (r + 1) % 3) == 0ull) break;   // no root picked
+    if (loadCell(a.counters + MSF_LIVE + (r + 1) % 3) == 0ull) break;   // no root picked
 
     // ---- link --------------------------------------------------------------------------
     for (Index v = gtid; v < a.n; v += gthreads) {
@@ -213,7 +206,7 @@ msfKernel(MsfArgs a) {
     ++barriers;
 
     // ---- compress ----------------------------------------------------------------------
-    ccCompress(cc, gtid, gthreads);
+    ccCompress(a.parent, a.n, gtid, gthreads);
     grid.sync();
     ++barriers;
   }

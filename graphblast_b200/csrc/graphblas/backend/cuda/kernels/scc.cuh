@@ -47,18 +47,15 @@
 // lay their frontiers one after another in qa; the pivot's reaches do the same in qb
 // and qc; the colour work lists alternate between qb and qc.
 //
-// Memory model.  label, colour, degrees, marks, stamps, queue entries and the cells are
-// written by other SMs while the kernel runs: they are read with ld.relaxed.gpu (ccLoad,
-// the L2), never through __ldg or L1, where a line read earlier in the kernel could be
-// stale.  Writes before a grid barrier are visible to every thread after it.  Only the
-// CSR and CSC, which nothing writes, are read through the non-coherent path.
+// Memory model (cooperative.cuh).  label, colour, degrees, marks, stamps and queue
+// entries are written by other SMs while the kernel runs and are read with ldRelaxed;
+// only the CSR and CSC are read through the non-coherent path.
 #ifndef GRAPHBLAS_BACKEND_CUDA_KERNELS_SCC_CUH_
 #define GRAPHBLAS_BACKEND_CUDA_KERNELS_SCC_CUH_
 
 #include <cooperative_groups.h>
 
-#include "graphblas/backend/cuda/kernels/cc.cuh"
-#include "graphblas/backend/cuda/kernels/common.cuh"
+#include "graphblas/backend/cuda/kernels/cooperative.cuh"
 
 namespace graphblas {
 namespace backend {
@@ -110,27 +107,12 @@ struct SccFront {
   int dirs;
 };
 
-__device__ __forceinline__ unsigned long long sccCell(const SccArgs& a, int cell) {
-  return *reinterpret_cast<volatile unsigned long long*>(a.counters + cell);
-}
-
 // The length of v's list without its self-loop.
 __device__ __forceinline__ Index sccDegree(const Index* ptr, const Index* ind, Index v) {
   const Index b = __ldg(ptr + v), e = __ldg(ptr + v + 1);
   if (e == b) return 0;
   const Index k = findSorted(ind, b, e, v);
   return e - b - (k < e && __ldg(ind + k) == v ? 1 : 0);
-}
-
-// Appends y at q[base + the cell's count], one atomic for the lanes that append together.
-__device__ __forceinline__ void sccAppend(Index* q, Index base, unsigned long long* cell,
-                                          Index y) {
-  namespace cg = cooperative_groups;
-  cg::coalesced_group g = cg::coalesced_threads();
-  unsigned long long at = 0ull;
-  if (g.thread_rank() == 0) at = atomicAdd(cell, static_cast<unsigned long long>(g.size()));
-  at = g.shfl(at, 0);
-  q[base + static_cast<Index>(at) + static_cast<Index>(g.thread_rank())] = y;
 }
 
 // The light part of a level: visit(dir, x, y) for every entry y of each list of f,
@@ -149,7 +131,7 @@ __device__ __forceinline__ void sccLight(const SccArgs& a, const SccFront& f,
       const Index i = i0 + lane;
       Index x = 0, b = 0, e = 0;
       if (i < f.hi) {
-        x = ccLoad(f.q + i);
+        x = ldRelaxed(f.q + i);
         b = __ldg(ptr + x);
         e = __ldg(ptr + x + 1);
       }
@@ -181,7 +163,7 @@ __device__ __forceinline__ void sccHeavy(const SccArgs& a, Index nh, Visit& visi
   const Index gwarps = (gridDim.x*GB_SCC_NT) >> 5;
   Index before = 0;                    // chunks of the lists before h, modulo warps
   for (Index h = 0; h < nh; ++h) {
-    const Index entry = ccLoad(a.heavy + h);
+    const Index entry = ldRelaxed(a.heavy + h);
     const int dir = entry >= 0 ? SCC_OUT : SCC_IN;
     const Index x = entry >= 0 ? entry : ~entry;
     const Index* ptr = dir == SCC_OUT ? a.row_ptr : a.col_ptr;
@@ -228,7 +210,7 @@ sccKernel(SccArgs a, W* out) {
     advance();
   };
   auto count = [&](int cell) {         // the appends of the level before this one
-    return static_cast<Index>(sccCell(a, cell + (lv + 2) % 3));
+    return static_cast<Index>(loadCell(cells + cell + (lv + 2) % 3));
   };
   // One frontier level over f and g: the light part, a barrier, and the grid pass with
   // its own barrier when a list was deferred.
@@ -237,7 +219,7 @@ sccKernel(SccArgs a, W* out) {
     sccLight(a, g, cells + SCC_HEAVY + lv % 3, visit);
     grid.sync();
     ++barriers;
-    const Index nh = static_cast<Index>(sccCell(a, SCC_HEAVY + lv % 3));
+    const Index nh = static_cast<Index>(loadCell(cells + SCC_HEAVY + lv % 3));
     if (nh > 0) {
       sccHeavy(a, nh, visit);
       grid.sync();
@@ -253,27 +235,27 @@ sccKernel(SccArgs a, W* out) {
     const Index dout = sccDegree(a.row_ptr, a.row_ind, v);
     const Index din = sccDegree(a.col_ptr, a.col_ind, v);
     const bool dead = dout == 0 || din == 0;
-    ccStore(a.label + v, -1);
-    ccStore(a.dout + v, dout);
-    ccStore(a.din + v, din);
-    ccStore(a.mark + v, dead ? SCC_QUEUED : 0);
-    ccStore(a.stamp + v, -1);
-    if (dead) sccAppend(a.qa, 0, cells + SCC_FRONT + lv % 3, v);
+    stRelaxed(a.label + v, -1);
+    stRelaxed(a.dout + v, dout);
+    stRelaxed(a.din + v, din);
+    stRelaxed(a.mark + v, dead ? SCC_QUEUED : 0);
+    stRelaxed(a.stamp + v, -1);
+    if (dead) warpAppend(a.qa, 0, cells + SCC_FRONT + lv % 3, v);
   }
   next();
 
   // ---- trim, to its fixpoint -----------------------------------------------------------
   Index lo = 0, hi = count(SCC_FRONT);
   auto trim = [&](int dir, Index x, Index y) {
-    if (y == x || (ccLoad(a.mark + y) & SCC_QUEUED) != 0) return;
+    if (y == x || (ldRelaxed(a.mark + y) & SCC_QUEUED) != 0) return;
     Index* deg = dir == SCC_OUT ? a.din : a.dout;    // x -> y, or y -> x
     if (atomicSub(deg + y, 1) == 1 && (atomicOr(a.mark + y, SCC_QUEUED) & SCC_QUEUED) == 0)
-      sccAppend(a.qa, hi, cells + SCC_FRONT + lv % 3, y);
+      warpAppend(a.qa, hi, cells + SCC_FRONT + lv % 3, y);
   };
   while (lo < hi) {
     for (Index i = lo + gtid; i < hi; i += gthreads) {
-      const Index x = ccLoad(a.qa + i);
-      ccStore(a.label + x, x);
+      const Index x = ldRelaxed(a.qa + i);
+      stRelaxed(a.label + x, x);
     }
     level({a.qa, lo, hi, SCC_OUT | SCC_IN}, none, trim);
     lo = hi;
@@ -284,10 +266,10 @@ sccKernel(SccArgs a, W* out) {
   // ---- pivot: the largest (out + 1)(in + 1) among the live, ties to the smallest id -----
   unsigned long long best = 0ull;
   for (Index v = gtid; v < a.n; v += gthreads) {
-    if (ccLoad(a.label + v) != -1) continue;
+    if (ldRelaxed(a.label + v) != -1) continue;
     const unsigned long long score =
-        static_cast<unsigned long long>(ccLoad(a.dout + v) + 1) *
-        static_cast<unsigned long long>(ccLoad(a.din + v) + 1);
+        static_cast<unsigned long long>(ldRelaxed(a.dout + v) + 1) *
+        static_cast<unsigned long long>(ldRelaxed(a.din + v) + 1);
     const unsigned long long key =
         ((score < 0xFFFFFFFFull ? score : 0xFFFFFFFFull) << 32) |
         (0xFFFFFFFFull - static_cast<unsigned int>(v));
@@ -296,7 +278,7 @@ sccKernel(SccArgs a, W* out) {
   best = warpReduce(best, [](unsigned long long x, unsigned long long y) { return x > y ? x : y; });
   if (lane == 0 && best != 0ull) atomicMax(cells + SCC_PIVOT, best);
   next();
-  const unsigned long long pivot_key = sccCell(a, SCC_PIVOT);
+  const unsigned long long pivot_key = loadCell(cells + SCC_PIVOT);
   Index pivot_min = -1;
 
   if (pivot_key != 0ull) {
@@ -310,11 +292,11 @@ sccKernel(SccArgs a, W* out) {
     next();
     Index flo = 0, fhi = 1, blo = 0, bhi = 1;
     auto reach = [&](int dir, Index x, Index y) {
-      if (y == x || ccLoad(a.label + y) != -1) return;
+      if (y == x || ldRelaxed(a.label + y) != -1) return;
       const int bit = dir == SCC_OUT ? SCC_FW : SCC_BW;
-      if ((ccLoad(a.mark + y) & bit) != 0 || (atomicOr(a.mark + y, bit) & bit) != 0) return;
-      if (dir == SCC_OUT) sccAppend(a.qb, fhi, cells + SCC_FRONT + lv % 3, y);
-      else                sccAppend(a.qc, bhi, cells + SCC_BACK + lv % 3, y);
+      if ((ldRelaxed(a.mark + y) & bit) != 0 || (atomicOr(a.mark + y, bit) & bit) != 0) return;
+      if (dir == SCC_OUT) warpAppend(a.qb, fhi, cells + SCC_FRONT + lv % 3, y);
+      else                warpAppend(a.qc, bhi, cells + SCC_BACK + lv % 3, y);
     };
     while (flo < fhi || blo < bhi) {
       level({a.qb, flo, fhi, SCC_OUT}, {a.qc, blo, bhi, SCC_IN}, reach);
@@ -327,8 +309,8 @@ sccKernel(SccArgs a, W* out) {
     // ---- the pivot's component: both reaches; its size and smallest id -----------------
     unsigned int size = 0u;
     for (Index i = gtid; i < fhi; i += gthreads) {
-      const Index x = ccLoad(a.qb + i);
-      if ((ccLoad(a.mark + x) & (SCC_FW | SCC_BW)) == (SCC_FW | SCC_BW)) {
+      const Index x = ldRelaxed(a.qb + i);
+      if ((ldRelaxed(a.mark + x) & (SCC_FW | SCC_BW)) == (SCC_FW | SCC_BW)) {
         atomicMin(cells + SCC_MIN, static_cast<unsigned long long>(x));
         ++size;
       }
@@ -336,7 +318,7 @@ sccKernel(SccArgs a, W* out) {
     size = __reduce_add_sync(GB_FULL_MASK, size);
     if (lane == 0 && size != 0u) atomicAdd(cells + SCC_SIZE, static_cast<unsigned long long>(size));
     next();
-    pivot_min = static_cast<Index>(sccCell(a, SCC_MIN));
+    pivot_min = static_cast<Index>(loadCell(cells + SCC_MIN));
   }
 
   // ---- colouring, while live vertices remain -------------------------------------------
@@ -347,13 +329,13 @@ sccKernel(SccArgs a, W* out) {
       // init: colour[v] = v for every live v, all of them the first work list; the first
       // init also settles the pivot's component
       for (Index v = gtid; v < a.n; v += gthreads) {
-        if (ccLoad(a.label + v) != -1) continue;
-        if ((ccLoad(a.mark + v) & (SCC_FW | SCC_BW)) == (SCC_FW | SCC_BW)) {
-          ccStore(a.label + v, pivot_min);
+        if (ldRelaxed(a.label + v) != -1) continue;
+        if ((ldRelaxed(a.mark + v) & (SCC_FW | SCC_BW)) == (SCC_FW | SCC_BW)) {
+          stRelaxed(a.label + v, pivot_min);
           continue;
         }
-        ccStore(a.colour + v, v);
-        sccAppend(a.qb, 0, cells + SCC_FRONT + lv % 3, v);
+        stRelaxed(a.colour + v, v);
+        warpAppend(a.qb, 0, cells + SCC_FRONT + lv % 3, v);
       }
       next();
       Index len = count(SCC_FRONT);
@@ -365,10 +347,10 @@ sccKernel(SccArgs a, W* out) {
       Index* cur = a.qb;
       Index* nxt = a.qc;
       auto push = [&](int, Index x, Index y) {
-        if (y == x || ccLoad(a.label + y) != -1) return;
-        const Index c = ccLoad(a.colour + x);
+        if (y == x || ldRelaxed(a.label + y) != -1) return;
+        const Index c = ldRelaxed(a.colour + x);
         if (atomicMin(a.colour + y, c) > c && atomicExch(a.stamp + y, lv) != lv)
-          sccAppend(nxt, 0, cells + SCC_FRONT + lv % 3, y);
+          warpAppend(nxt, 0, cells + SCC_FRONT + lv % 3, y);
       };
       while (len > 0) {
         level({cur, 0, len, SCC_OUT}, none, push);
@@ -380,18 +362,18 @@ sccKernel(SccArgs a, W* out) {
 
       // settle: the roots, then backward through live vertices of their colour
       for (Index v = gtid; v < a.n; v += gthreads) {
-        if (ccLoad(a.label + v) == -1 && ccLoad(a.colour + v) == v) {
-          ccStore(a.label + v, v);
-          sccAppend(a.qa, settled, cells + SCC_FRONT + lv % 3, v);
+        if (ldRelaxed(a.label + v) == -1 && ldRelaxed(a.colour + v) == v) {
+          stRelaxed(a.label + v, v);
+          warpAppend(a.qa, settled, cells + SCC_FRONT + lv % 3, v);
         }
       }
       next();
       Index slo = settled, shi = settled + count(SCC_FRONT);
       auto settle = [&](int, Index x, Index y) {
-        if (y == x || ccLoad(a.label + y) != -1) return;
-        const Index c = ccLoad(a.colour + x);
-        if (ccLoad(a.colour + y) != c) return;
-        if (atomicCAS(a.label + y, -1, c) == -1) sccAppend(a.qa, shi, cells + SCC_FRONT + lv % 3, y);
+        if (y == x || ldRelaxed(a.label + y) != -1) return;
+        const Index c = ldRelaxed(a.colour + x);
+        if (ldRelaxed(a.colour + y) != c) return;
+        if (atomicCAS(a.label + y, -1, c) == -1) warpAppend(a.qa, shi, cells + SCC_FRONT + lv % 3, y);
       };
       while (slo < shi) {
         level({a.qa, slo, shi, SCC_IN}, none, settle);
@@ -405,7 +387,7 @@ sccKernel(SccArgs a, W* out) {
   // ---- out: the label of every vertex, and the number of components --------------------
   unsigned int roots = 0u;
   for (Index v = gtid; v < a.n; v += gthreads) {
-    const Index r = ccLoad(a.label + v);
+    const Index r = ldRelaxed(a.label + v);
     out[v] = static_cast<W>(r);
     roots += r == v ? 1u : 0u;
   }

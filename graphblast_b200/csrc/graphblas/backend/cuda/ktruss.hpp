@@ -23,11 +23,6 @@ struct KtrussStats {
   float support_ms = 0.f;
 };
 
-inline KtrussStats& ktrussLastStats() {
-  static KtrussStats stats;
-  return stats;
-}
-
 // k >= 2: C = the k-truss of the undirected simple graph G of A's pattern, C(i,j) =
 // C(j,i) = the number of triangles of the k-truss that contain {i, j}; *count (when not
 // NULL) = its undirected edges.  k == 0: C = the truss decomposition, C(i,j) = C(j,i) =
@@ -51,14 +46,8 @@ template <typename c, typename a>
 Info ktrussRun(Matrix<c>* C, const Matrix<a>* A, int k, long long* count, float* ms = NULL) {
   static_assert(std::is_same<c, int>::value || std::is_same<c, float>::value,
                 "ktruss writes int or float matrices");
-  Vector<float>* const no_vector = NULL;
-  if (!A->isSparse()) return graphCheck("k-truss", A, true, no_vector);
+  CHECK(graphCheck("k-truss", A, true, C));
   const SparseMatrix<a>& S = A->sparse_;
-  Index cr = 0, cn = 0;
-  CHECK(C->nrows(&cr));
-  CHECK(C->ncols(&cn));
-  if (S.nrows_ != S.ncols_ || cr != S.nrows_ || cn != S.nrows_) return GrB_DIMENSION_MISMATCH;
-  CHECK(graphCheck("k-truss", A, true, no_vector));
   const Index n = S.nrows_;
   if (std::is_same<c, float>::value && n > (1 << 24)) return GrB_INVALID_VALUE;
 
@@ -90,8 +79,7 @@ Info ktrussRun(Matrix<c>* C, const Matrix<a>* A, int k, long long* count, float*
   const size_t offset = l.place(nz*sizeof(int));
   const DeviceBlock block(gbMalloc(l.bytes));
   CUDA_CALL(cudaMemsetAsync(block.at<void>(cells), 0, KT_NCELLS*sizeof(int), s));
-  int nitems = 0;
-  int2* items = NULL;
+  DeviceBlock items(NULL);              // the support items, then the peel list
   if (nnz > 0) {
     CUDA_CALL(cudaMemsetAsync(block.at<void>(sup), 0, nz*sizeof(int), s));
     ktrussPrepKernel<<<gridFor(nz, 256), 256, 0, s>>>(ptr, ind, n, nnz, block.at<Index>(erow),
@@ -99,10 +87,11 @@ Info ktrussRun(Matrix<c>* C, const Matrix<a>* A, int k, long long* count, float*
     GB_KERNEL_CHECK();
     const unsigned long long total = scanExclusiveInPlace(block.at<int>(offset), nnz);
     if (total > static_cast<unsigned long long>(INT_MAX)) return GrB_OUT_OF_MEMORY;
-    nitems = static_cast<int>(total);
-    items = reinterpret_cast<int2*>(gbMalloc(static_cast<size_t>(nitems)*sizeof(int2)));
+    const int nitems = static_cast<int>(total);
+    DeviceBlock list(gbMalloc(static_cast<size_t>(nitems)*sizeof(int2)));
+    items.swap(list);
     ktrussItemsKernel<<<gridFor(nz, 256), 256, 0, s>>>(ptr, ind, block.at<Index>(erow),
-        block.at<int>(state), block.at<int>(offset), nnz, items);
+        block.at<int>(state), block.at<int>(offset), nnz, items.at<int2>());
     GB_KERNEL_CHECK();
     const int min_cell = INT_MAX;
     CUDA_CALL(cudaMemcpyAsync(block.at<int>(cells) + KT_MIN, &min_cell, sizeof(int),
@@ -116,15 +105,11 @@ Info ktrussRun(Matrix<c>* C, const Matrix<a>* A, int k, long long* count, float*
     args.nnz = nnz;
     args.sup = block.at<int>(sup);
     args.state = block.at<int>(state);
-    args.items = items;
+    args.items = items.at<int2>();
     args.nitems = nitems;
     args.k = k;
     args.cells = block.at<int>(cells);
-    const Info launched = launchCooperative<ktrussKernel, GB_KT_NT>(s, args);
-    if (launched != GrB_SUCCESS) {
-      gbFree(items);
-      return launched;
-    }
+    CHECK((launchCooperative<ktrussKernel, GB_KT_NT>(s, args)));
   }
 
   // the result: every kept entry of the view, in stored order
@@ -149,15 +134,13 @@ Info ktrussRun(Matrix<c>* C, const Matrix<a>* A, int k, long long* count, float*
   CUDA_CALL(cudaMemcpyAsync(host_cells, block.at<int>(cells), sizeof(host_cells),
                             cudaMemcpyDeviceToHost, s));
   CUDA_CALL(cudaStreamSynchronize(s));
-  gbFree(items);
-  // the values are symmetric too, so the column-major values are a copy of the CSR's
-  c* cscval = C->sparse_.format_ == GrB_SPARSE_MATRIX_CSRCSC ? copyOnDevice(val, kept) : NULL;
-  C->sparse_.replaceDevice(kept, rowptr, colind, val, NULL, NULL, cscval, true);
-  CHECK(C->setStorage(GrB_SPARSE));
+  DeviceBlock(NULL).swap(items);       // the items are freed before C takes the result
+  CHECK(installSymmetric(C, kept, rowptr, colind, val));
   clock.Stop();
-  ktrussLastStats().rounds = host_cells[KT_ROUNDS];
-  ktrussLastStats().levels = host_cells[KT_LEVELS];
-  ktrussLastStats().support_ms = host_cells[KT_SUPPORT_US]*1e-3f;
+  KtrussStats& stats = lastStats<KtrussStats>();
+  stats.rounds = host_cells[KT_ROUNDS];
+  stats.levels = host_cells[KT_LEVELS];
+  stats.support_ms = host_cells[KT_SUPPORT_US]*1e-3f;
   if (count != NULL) *count = keep_all ? host_cells[KT_KMAX] : kept/2;
   if (ms != NULL) *ms = clock.ElapsedMillis();
   return GrB_SUCCESS;

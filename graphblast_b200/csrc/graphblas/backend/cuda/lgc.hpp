@@ -67,8 +67,8 @@ Info lgcRun(Vector<float>* p, Vector<float>* r, const Matrix<a>* A, Index s, dou
   args.front[1] = block.at<Index>(front1);
   args.touched  = block.at<Index>(touched);
   args.row_ptr = g.row_ptr;  args.row_ind = g.row_ind;
-  args.in_ptr = g.col_ptr != NULL ? g.col_ptr : g.row_ptr;
-  args.in_ind = g.col_ptr != NULL ? g.col_ind : g.row_ind;
+  args.in_ptr = g.in_ptr();
+  args.in_ind = g.in_ind();
   CUDA_CALL(cudaMemsetAsync(args.counters, 0, LGC_NCELLS*sizeof(unsigned long long), stream));
 
   CHECK(p->setStorage(GrB_DENSE));

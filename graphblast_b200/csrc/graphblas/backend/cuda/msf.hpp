@@ -22,11 +22,6 @@ struct MsfStats {
   float canon_ms = 0.f;
 };
 
-inline MsfStats& msfLastStats() {
-  static MsfStats stats;
-  return stats;
-}
-
 // F = the minimum spanning forest of the undirected graph G of A: the edge {i, j}, i !=
 // j, when A(i,j) or A(j,i) is stored, weighted by the smaller stored value; edges ranked
 // by (w, min(i,j), max(i,j)).  F(i,j) = F(j,i) = w({i,j}) on every forest edge, -0.0
@@ -48,14 +43,8 @@ Info msfRun(Matrix<T>* F, const Matrix<T>* A, long long* nedges, double* weight,
             float* ms = NULL) {
   static_assert(std::is_same<T, int>::value || std::is_same<T, float>::value,
                 "msf reads int or float matrices");
-  Vector<float>* const no_vector = NULL;
-  if (!A->isSparse()) return graphCheck("msf", A, false, no_vector);
+  CHECK(graphCheck("msf", A, false, F));
   const SparseMatrix<T>& S = A->sparse_;
-  Index fr = 0, fc = 0;
-  CHECK(F->nrows(&fr));
-  CHECK(F->ncols(&fc));
-  if (S.nrows_ != S.ncols_ || fr != S.nrows_ || fc != S.nrows_) return GrB_DIMENSION_MISMATCH;
-  CHECK(graphCheck("msf", A, false, no_vector));
   const Index n = S.nrows_;
   const Index nnz = hasEntries(S) ? S.nvals_ : 0;
   const size_t nz = static_cast<size_t>(nnz);
@@ -73,47 +62,52 @@ Info msfRun(Matrix<T>* F, const Matrix<T>* A, long long* nedges, double* weight,
   const int bits = ingestBitsFor(n);
   const unsigned long long loop = (1ull << (2*bits)) - 1ull;
   Index m = 0;
-  unsigned long long* keys = NULL;
-  unsigned int* pay = NULL;
-  int* first = NULL;
-  if (nnz > 0) {
-    keys = reinterpret_cast<unsigned long long*>(gbMalloc(nz*8));
-    pay = reinterpret_cast<unsigned int*>(gbMalloc(nz*4));
-    msfEmitKernel<T><<<gridFor(nz, 256), 256, 0, s>>>(S.d_csrRowPtr_, S.d_csrColInd_,
-        S.d_csrVal_, n, nnz, bits, loop, keys, pay, cells);
-    GB_KERNEL_CHECK();
-    if (std::is_same<T, float>::value && runtime().fetch(cells + MSF_NAN) != 0ull) {
-      gbFree(pay);
-      gbFree(keys);
-      return GrB_INVALID_VALUE;
-    }
-    unsigned long long* keys_tmp = reinterpret_cast<unsigned long long*>(gbMalloc(nz*8));
-    unsigned int* pay_tmp = reinterpret_cast<unsigned int*>(gbMalloc(nz*4));
-    radixSortPairs(&keys, &pay, &keys_tmp, &pay_tmp, nnz, 2*bits);
-    gbFree(keys_tmp);
-    gbFree(pay_tmp);
-    first = reinterpret_cast<int*>(gbMalloc((nz + 1)*sizeof(int)));
-    msfFirstKernel<<<gridFor(nz + 1, 256), 256, 0, s>>>(keys, nnz, loop, first);
-    GB_KERNEL_CHECK();
-    m = static_cast<Index>(scanExclusiveInPlace(first, static_cast<long long>(nnz) + 1));
-  }
-  const size_t mm = static_cast<size_t>(m);
   ScratchLayout edges;
-  const size_t eu_at = edges.place(mm*sizeof(Index));
-  const size_t ev_at = edges.place(mm*sizeof(Index));
-  const size_t ew_at = edges.place(mm*sizeof(unsigned int));
-  const DeviceBlock list(m > 0 ? gbMalloc(edges.bytes) : NULL);
+  size_t eu_at = 0, ev_at = 0, ew_at = 0;
+  DeviceBlock list(NULL);
+  if (nnz > 0) {
+    DeviceBlock keys(gbMalloc(nz*8));
+    DeviceBlock pay(gbMalloc(nz*4));
+    msfEmitKernel<T><<<gridFor(nz, 256), 256, 0, s>>>(S.d_csrRowPtr_, S.d_csrColInd_,
+        S.d_csrVal_, n, nnz, bits, loop, keys.at<unsigned long long>(), pay.at<unsigned int>(),
+        cells);
+    GB_KERNEL_CHECK();
+    if (std::is_same<T, float>::value && runtime().fetch(cells + MSF_NAN) != 0ull)
+      return GrB_INVALID_VALUE;
+    {  // freed before `first` is allocated: the sort's peak stays 24 bytes per entry
+      DeviceBlock keys_tmp(gbMalloc(nz*8));
+      DeviceBlock pay_tmp(gbMalloc(nz*4));
+      unsigned long long* k = keys.at<unsigned long long>();
+      unsigned long long* k_tmp = keys_tmp.at<unsigned long long>();
+      unsigned int* p = pay.at<unsigned int>();
+      unsigned int* p_tmp = pay_tmp.at<unsigned int>();
+      radixSortPairs(&k, &p, &k_tmp, &p_tmp, nnz, 2*bits);
+      // the sort may have left its output in the other buffers: ownership follows it
+      if (k != keys.at<unsigned long long>()) keys.swap(keys_tmp);
+      if (p != pay.at<unsigned int>()) pay.swap(pay_tmp);
+    }
+    DeviceBlock first(gbMalloc((nz + 1)*sizeof(int)));
+    msfFirstKernel<<<gridFor(nz + 1, 256), 256, 0, s>>>(keys.at<unsigned long long>(), nnz,
+        loop, first.at<int>());
+    GB_KERNEL_CHECK();
+    m = static_cast<Index>(scanExclusiveInPlace(first.at<int>(), static_cast<long long>(nnz) + 1));
+    const size_t slots = static_cast<size_t>(m);
+    eu_at = edges.place(slots*sizeof(Index));
+    ev_at = edges.place(slots*sizeof(Index));
+    ew_at = edges.place(slots*sizeof(unsigned int));
+    DeviceBlock canonical(m > 0 ? gbMalloc(edges.bytes) : NULL);
+    list.swap(canonical);
+    if (m > 0) {
+      msfCanonKernel<<<gridFor(nz, 256), 256, 0, s>>>(keys.at<unsigned long long>(),
+          pay.at<unsigned int>(), first.at<int>(), nnz, bits, list.at<Index>(eu_at),
+          list.at<Index>(ev_at), list.at<unsigned int>(ew_at));
+      GB_KERNEL_CHECK();
+    }
+  }  // first, pay and keys are freed here
+  const size_t mm = static_cast<size_t>(m);
   const Index* eu = list.at<Index>(eu_at);
   const Index* ev = list.at<Index>(ev_at);
   const unsigned int* ew = list.at<unsigned int>(ew_at);
-  if (m > 0) {
-    msfCanonKernel<<<gridFor(nz, 256), 256, 0, s>>>(keys, pay, first, nnz, bits,
-        list.at<Index>(eu_at), list.at<Index>(ev_at), list.at<unsigned int>(ew_at));
-    GB_KERNEL_CHECK();
-  }
-  gbFree(first);
-  gbFree(pay);
-  gbFree(keys);
   canon.Stop();
 
   // ---- Borůvka rounds ------------------------------------------------------------------
@@ -170,13 +164,10 @@ Info msfRun(Matrix<T>* F, const Matrix<T>* A, long long* nedges, double* weight,
   T* val = NULL;
   const Index kept = ingestCooToCsr<T>(n, n, out.at<Index>(src_at), out.at<Index>(dst_at),
       out.at<T>(val_at), nf, GB_INGEST_SYMMETRIZE, &rowptr, &colind, &val);
-  // the values are symmetric too, so the column-major values are a copy of the CSR's
-  T* cscval = F->sparse_.format_ == GrB_SPARSE_MATRIX_CSRCSC ? copyOnDevice(val, kept) : NULL;
-  F->sparse_.replaceDevice(kept, rowptr, colind, val, NULL, NULL, cscval, true);
-  CHECK(F->setStorage(GrB_SPARSE));
+  CHECK(installSymmetric(F, kept, rowptr, colind, val));
   clock.Stop();
   CUDA_CALL(cudaStreamSynchronize(s));
-  MsfStats& stats = msfLastStats();
+  MsfStats& stats = lastStats<MsfStats>();
   stats.rounds = static_cast<int>(host_cells[MSF_ROUNDS]);
   stats.barriers = static_cast<int>(host_cells[MSF_BARRIERS]);
   stats.canon_ms = canon.ElapsedMillis();

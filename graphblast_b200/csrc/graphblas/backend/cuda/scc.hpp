@@ -23,11 +23,6 @@ struct SccStats {
   int barriers = 0;
 };
 
-inline SccStats& sccLastStats() {
-  static SccStats stats;
-  return stats;
-}
-
 // v[i] = the smallest vertex id in the strongly connected component of i, over the arcs
 // i -> j with A(i,j) stored and i != j; *ncomponents (when not NULL) = the number of
 // components, 0 when A has no rows; *ms (when not NULL) = the device time, from CUDA
@@ -50,8 +45,8 @@ Info sccRun(Vector<W>* v, const Matrix<a>* A, int* ncomponents, float* ms = NULL
   if (std::is_same<W, float>::value && n > (1 << 24) + 1) return GrB_INVALID_VALUE;
   if (S.sameStructure()) {
     CHECK(ccRun(v, A, ncomponents, ms));
-    sccLastStats() = SccStats();
-    sccLastStats().barriers = -1;
+    lastStats<SccStats>() = SccStats();
+    lastStats<SccStats>().barriers = -1;
     return GrB_SUCCESS;
   }
 
@@ -61,7 +56,7 @@ Info sccRun(Vector<W>* v, const Matrix<a>* A, int* ncomponents, float* ms = NULL
   CHECK(v->setStorage(GrB_DENSE));
   if (n == 0) {
     clock.Stop();
-    sccLastStats() = SccStats();
+    lastStats<SccStats>() = SccStats();
     if (ms != NULL) *ms = clock.ElapsedMillis();
     return GrB_SUCCESS;
   }
@@ -79,8 +74,8 @@ Info sccRun(Vector<W>* v, const Matrix<a>* A, int* ncomponents, float* ms = NULL
   args.n = n;
   args.row_ptr = g.row_ptr;
   args.row_ind = g.row_ind;
-  args.col_ptr = g.stored() ? g.col_ptr : g.row_ptr;   // no entry: every list is empty
-  args.col_ind = g.col_ind;
+  args.col_ptr = g.in_ptr();
+  args.col_ind = g.in_ind();
   args.counters = block.at<unsigned long long>(counters);
   Index* w = block.at<Index>(words);
   args.label = w;
@@ -102,7 +97,7 @@ Info sccRun(Vector<W>* v, const Matrix<a>* A, int* ncomponents, float* ms = NULL
   clock.Stop();
   CUDA_CALL(cudaStreamSynchronize(stream));
   v->dense_.touched();
-  SccStats& stats = sccLastStats();
+  SccStats& stats = lastStats<SccStats>();
   stats.trimmed = static_cast<long long>(cells[SCC_TRIMMED]);
   stats.pivot_size = static_cast<long long>(cells[SCC_SIZE]);
   stats.colour_iterations = static_cast<int>(cells[SCC_COLOURS]);

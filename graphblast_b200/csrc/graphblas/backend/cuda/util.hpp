@@ -16,6 +16,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <iostream>
+#include <utility>
 #include <vector>
 
 #define CUDA_SAFE_CALL_NO_SYNC(call) do {                                    \
@@ -257,6 +258,7 @@ class DeviceBlock {
   DeviceBlock& operator=(const DeviceBlock&) = delete;
   // The array at byte offset `off` of the block.
   template <typename T> T* at(size_t off = 0) const { return reinterpret_cast<T*>(p_ + off); }
+  void swap(DeviceBlock& other) { std::swap(p_, other.p_); }   // exchanges the blocks
 
  private:
   unsigned char* p_;

@@ -45,7 +45,7 @@ float ktruss(Matrix<T>* C, const Matrix<a>* A, int k, Descriptor* desc, Index* n
   if (nedges != NULL) *nedges = static_cast<Index>(count);
   if (desc->descriptor_.timing_ > 0)
     std::cout << "ktruss, k " << k << ", " << count << " edges, "
-              << backend::ktrussLastStats().rounds << " rounds, " << ms << "\n";
+              << backend::lastStats<backend::KtrussStats>().rounds << " rounds, " << ms << "\n";
   return ms;
 }
 
@@ -56,9 +56,11 @@ float trussness(Matrix<T>* C, const Matrix<a>* A, Descriptor* desc, int* kmax) {
   float ms = 0.f;
   GB_ALGO_STEP(backend::ktrussRun(&C->matrix_, &A->matrix_, 0, &count, &ms));
   if (kmax != NULL) *kmax = static_cast<int>(count);
-  if (desc->descriptor_.timing_ > 0)
-    std::cout << "trussness, kmax " << count << ", " << backend::ktrussLastStats().levels
-              << " levels, " << backend::ktrussLastStats().rounds << " rounds, " << ms << "\n";
+  if (desc->descriptor_.timing_ > 0) {
+    const backend::KtrussStats& stats = backend::lastStats<backend::KtrussStats>();
+    std::cout << "trussness, kmax " << count << ", " << stats.levels << " levels, "
+              << stats.rounds << " rounds, " << ms << "\n";
+  }
   return ms;
 }
 

@@ -47,7 +47,7 @@ float msf(Matrix<T>* F, const Matrix<T>* A, Descriptor* desc, Index* nedges,
   if (weight != NULL) *weight = total;
   if (desc->descriptor_.timing_ > 0)
     std::cout << "msf, " << count << " edges, weight " << total << ", "
-              << backend::msfLastStats().rounds << " rounds, " << ms << "\n";
+              << backend::lastStats<backend::MsfStats>().rounds << " rounds, " << ms << "\n";
   return ms;
 }
 

@@ -34,10 +34,11 @@ float scc(Vector<float>* v, const Matrix<a>* A, Descriptor* desc, int* ncomponen
   float ms = 0.f;
   GB_ALGO_STEP(backend::sccRun(&v->vector_, &A->matrix_, &count, &ms));
   if (ncomponents != NULL) *ncomponents = count;
-  if (desc->descriptor_.timing_ > 0)
-    std::cout << "scc, " << count << " components, " << backend::sccLastStats().trimmed
-              << " trimmed, " << backend::sccLastStats().colour_iterations
-              << " colourings, " << ms << "\n";
+  if (desc->descriptor_.timing_ > 0) {
+    const backend::SccStats& stats = backend::lastStats<backend::SccStats>();
+    std::cout << "scc, " << count << " components, " << stats.trimmed << " trimmed, "
+              << stats.colour_iterations << " colourings, " << ms << "\n";
+  }
   return ms;
 }
 
