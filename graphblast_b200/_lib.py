@@ -174,6 +174,15 @@ MSF_SIGNATURES = [
 ]
 
 
+# (name, restype, argtypes) for every symbol declared in include/graphblast_b200_cdlp.h,
+# the companion header of community detection by label propagation; load() binds these too.
+CDLP_SIGNATURES = [
+    ("gb200_cdlp", _I, [_P, _P, _I, _P, _IP, _IP, C.POINTER(_F)]),
+    ("gb200_cdlp_stats", _I, [C.POINTER(_LL), C.POINTER(_LL), C.POINTER(_LL),
+                              C.POINTER(_LL), _IP]),
+]
+
+
 class ExtensionMissing(RuntimeError):
     pass
 
@@ -191,7 +200,7 @@ def load():
     lib = C.CDLL(LIB_PATH)
     for name, restype, argtypes in (SIGNATURES + LGC_SIGNATURES + EXTRACT_SIGNATURES +
                                     BC_SIGNATURES + ASSIGN_SIGNATURES + KTRUSS_SIGNATURES +
-                                    SCC_SIGNATURES + MSF_SIGNATURES):
+                                    SCC_SIGNATURES + MSF_SIGNATURES + CDLP_SIGNATURES):
         fn = getattr(lib, name)   # AttributeError if a declared symbol is missing
         fn.restype = restype
         fn.argtypes = argtypes

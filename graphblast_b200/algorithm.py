@@ -6,10 +6,11 @@ local graph clustering lgc, one kernel each on the device, with lgc_sweep, the
 conductance sweep cut of lgc's result, the betweenness centrality bc, one kernel
 per batch of 32 sources, the k-truss ktruss and truss decomposition trussness, one
 cooperative edge-peeling kernel each, the strongly connected components scc, one
-cooperative trim, forward-backward and colouring kernel, and the minimum spanning
-forest msf, one cooperative Boruvka kernel.
+cooperative trim, forward-backward and colouring kernel, the minimum spanning
+forest msf, one cooperative Boruvka kernel, and the community detection by label
+propagation cdlp, one cooperative kernel for every iteration.
 
-sssp, pr, tc, gc, mis, cc, lgc, lgc_sweep, bc, ktruss, trussness, scc and msf return the device time of the operation
+sssp, pr, tc, gc, mis, cc, lgc, lgc_sweep, bc, ktruss, trussness, scc, msf and cdlp return the device time of the operation
 loop in milliseconds ("tight" in the reference drivers, example/gbfs.cu:110-115).  bfs returns it only
 when called with timed=True; otherwise it returns None and, when the traversal runs
 as the fused kernel, only enqueues it, so that back-to-back traversals keep the GPU
@@ -267,3 +268,39 @@ def msf_stats():
     rounds, barriers, canon = C.c_int(0), C.c_int(0), C.c_float(0)
     _lib.load().gb200_msf_stats(C.byref(rounds), C.byref(barriers), C.byref(canon))
     return rounds.value, barriers.value, canon.value
+
+
+def cdlp(v, A, max_iter, desc):
+    """v[i] = the label of i after synchronous label propagation (LDBC Graphalytics CDLP,
+    include/graphblas/algorithm/cdlp.hpp).  The arc i -> j when A(i,j) is stored and
+    i != j (values and self-loops ignored; FP32 and INT32 A give the same result).
+    L_0(v) = v; iteration k gives v the smallest label of highest multiplicity among the
+    labels of its out-neighbours (A's CSR) and in-neighbours (A's CSC), an arc stored
+    both ways counted twice; a vertex without neighbours keeps its label.  An A marked
+    symmetric (or whose CSC aliases its CSR) is read through its CSR alone, with the same
+    answer; a non-symmetric A needs its CSC.  max_iter >= 0 iterations, stopping early
+    after the first iteration that changes no label (a fixpoint, so the result is the
+    same).  v becomes dense and is overwritten; two calls give identical bytes.  A float
+    v holds ids exactly only up to 2^24, so nrows(A) > 2^24 + 1 raises
+    GrB_INVALID_VALUE, as does max_iter < 0.  Returns (ncommunities, iterations,
+    tight_ms): the distinct labels and the iterations run, including the one that changed
+    nothing."""
+    ms = C.c_float(0)
+    k = C.c_int(0)
+    it = C.c_int(0)
+    _check(_lib.load().gb200_cdlp(v._h, A._h, int(max_iter), desc._h, C.byref(k), C.byref(it),
+                                  C.byref(ms)),
+           "algorithm::cdlp")
+    return k.value, it.value, ms.value
+
+
+def cdlp_stats():
+    """(short_vertices, warp_vertices, long_vertices, long_items, barriers) of the last cdlp
+    call of this process: the vertices whose list (out- plus in-list, self-loops
+    included) has at most 32 entries, at most 128, and more; the (vertex, partition)
+    items of the long lists, one per 2048 entries or part of it; and the grid barriers of
+    the kernel, 2 per iteration and 2 more."""
+    s, w, lv, li, b = (C.c_longlong(0), C.c_longlong(0), C.c_longlong(0), C.c_longlong(0),
+                       C.c_int(0))
+    _lib.load().gb200_cdlp_stats(C.byref(s), C.byref(w), C.byref(lv), C.byref(li), C.byref(b))
+    return s.value, w.value, lv.value, li.value, b.value

@@ -32,6 +32,7 @@
 #include "graphblas/algorithm/ktruss.hpp"
 #include "graphblas/algorithm/scc.hpp"
 #include "graphblas/algorithm/msf.hpp"
+#include "graphblas/algorithm/cdlp.hpp"
 
 #include "graphblast_b200.h"
 #include "graphblast_b200_lgc.h"
@@ -41,6 +42,7 @@
 #include "graphblast_b200_ktruss.h"
 #include "graphblast_b200_scc.h"
 #include "graphblast_b200_msf.h"
+#include "graphblast_b200_cdlp.h"
 
 bool debug_;
 bool memory_;
@@ -1329,6 +1331,36 @@ int gb200_msf_stats(int* rounds, int* barriers, float* canon_ms) {
   if (rounds) *rounds = stats.rounds;
   if (barriers) *barriers = stats.barriers;
   if (canon_ms) *canon_ms = stats.canon_ms;
+  return 0;
+}
+
+// ---- community detection by label propagation (include/graphblast_b200_cdlp.h) ----
+
+int gb200_cdlp(gb200_vector_t v, gb200_matrix_t A, int max_iter, gb200_desc_t desc,
+               int* ncommunities, int* iterations, float* tight_ms) {
+  if (v == NULL || A == NULL || desc == NULL)
+    return rc(graphblas::GrB_UNINITIALIZED_OBJECT);
+  if (A->f == NULL && A->i == NULL) return rc(graphblas::GrB_DOMAIN_MISMATCH);
+  GB200_REQUIRE_DEVICE();
+  int count = 0, iters = 0;
+  const int info = runAlgorithm(tight_ms, [&] {
+    return onMatrix(A, [&](auto M) {
+      return graphblas::algorithm::cdlp(v->f, M, max_iter, &desc->desc, &count, &iters);
+    });
+  });
+  if (info == 0 && ncommunities) *ncommunities = count;
+  if (info == 0 && iterations) *iterations = iters;
+  return info;
+}
+
+int gb200_cdlp_stats(long long* short_vertices, long long* warp_vertices,
+                     long long* long_vertices, long long* long_items, int* barriers) {
+  const auto& stats = graphblas::backend::lastStats<graphblas::backend::CdlpStats>();
+  if (short_vertices) *short_vertices = stats.short_vertices;
+  if (warp_vertices) *warp_vertices = stats.warp_vertices;
+  if (long_vertices) *long_vertices = stats.long_vertices;
+  if (long_items) *long_items = stats.long_items;
+  if (barriers) *barriers = stats.barriers;
   return 0;
 }
 

@@ -1,7 +1,7 @@
 // graphblast_b200 backend — the input and output of the cooperative graph algorithms
-// (cc.hpp, greedy_schedule.hpp, lgc.hpp, bc.hpp, ktruss.hpp, scc.hpp, msf.hpp): one check
-// of A and the results, one view of A's pattern as their kernels read it, one installer
-// of a symmetric result matrix and the statistics of the last call.
+// (cc.hpp, greedy_schedule.hpp, lgc.hpp, bc.hpp, ktruss.hpp, scc.hpp, msf.hpp, cdlp.hpp):
+// one check of A and the results, one view of A's pattern as their kernels read it, one
+// installer of a symmetric result matrix and the statistics of the last call.
 #ifndef GRAPHBLAS_BACKEND_CUDA_GRAPH_INPUT_HPP_
 #define GRAPHBLAS_BACKEND_CUDA_GRAPH_INPUT_HPP_
 

@@ -48,6 +48,7 @@
 #include "graphblas/backend/cuda/ktruss.hpp"
 #include "graphblas/backend/cuda/scc.hpp"
 #include "graphblas/backend/cuda/msf.hpp"
+#include "graphblas/backend/cuda/cdlp.hpp"
 
 namespace graphblas {
 namespace backend {
