@@ -182,6 +182,26 @@ __device__ __forceinline__ void atomicCombine(T* addr, T val, AddOp add_op) {
   }
 }
 
+// atomicAdd on a float cell, returning the old value, with IEEE subnormals.  The
+// native float atomic add of global memory (atom.add.f32) flushes subnormal
+// operands and results to zero.  It is taken only when |v| > 2^-102: then a
+// subnormal cell lies below half an ulp of v on both sides (ulp(v) >= 2^-125), so
+// flushing it cannot change the rounded sum, and a nonzero sum is a multiple of
+// 2^-126 at least, so it is not subnormal either.  (At |v| = 2^-102 exactly the ulp
+// below v is 2^-126 and a cell of nearly -2^-126 would move the sum.)  Every
+// other v, NaN included, takes a CAS loop around a plain add.
+__device__ __forceinline__ float atomicAddIeee(float* addr, float v) {
+  if (fabsf(v) > 0x1p-102f) return atomicAdd(addr, v);
+  unsigned int* a = reinterpret_cast<unsigned int*>(addr);
+  unsigned int old = *a;
+  while (true) {
+    const unsigned int next = __float_as_uint(__fadd_rn(__uint_as_float(old), v));
+    const unsigned int prev = atomicCAS(a, old, next);
+    if (prev == old) return __uint_as_float(old);
+    old = prev;
+  }
+}
+
 // Same combine, returning the cell's value BEFORE this update.  `kind` is what
 // the semiring's add answers for add(3, 5) — the reference's own way of telling
 // monoids apart (spmv.hpp:76-85): 3 = minimum, 5 = maximum, 8 = plus.  For float
@@ -190,6 +210,9 @@ __device__ __forceinline__ void atomicCombine(T* addr, T val, AddOp add_op) {
 // set like reversed unsigned ints); everything else takes the CAS loop.  The
 // branch goes by the sign bit, not by `>= 0`: -0.0 compares equal to 0 but is
 // INT_MIN as a signed int, so atomicMin(int) would overwrite a negative cell.
+// A NaN is the largest signed int (positive NaN) or unsigned int (negative NaN)
+// and would win those atomics, where min / max (fminf / fmaxf) ignore it: a NaN
+// value leaves the cell alone, and the cell's value is returned.
 template <typename T, typename AddOp>
 __device__ __forceinline__ T atomicCombineFetch(T* addr, T val, AddOp add_op,
                                                 int kind) {
@@ -200,7 +223,9 @@ __device__ __forceinline__ T atomicCombineFetch(T* addr, T val, AddOp add_op,
     memcpy(&fv, &val, 4);
     float old;
     if (kind == 8) {
-      old = atomicAdd(fa, fv);
+      old = atomicAddIeee(fa, fv);
+    } else if (fv != fv) {
+      old = *reinterpret_cast<volatile float*>(fa);
     } else {
       const bool neg = (__float_as_uint(fv) >> 31) != 0u;
       const bool as_signed = (kind == 3) ? !neg : neg;

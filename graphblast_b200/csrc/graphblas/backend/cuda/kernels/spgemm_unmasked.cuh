@@ -291,10 +291,14 @@ mxmSymbolicDenseKernel(const Index* __restrict__ rows, const MxmCells* cells, in
   }
 }
 
-// Semiring add of v into a 32-bit cell: native for plus, CAS loop otherwise.
+// Semiring add of v into a 32-bit cell: native for plus (keeping float subnormals,
+// atomicAddIeee), CAS loop otherwise.
+__device__ __forceinline__ void mxmAdd(float* cell, float v) { atomicAddIeee(cell, v); }
+__device__ __forceinline__ void mxmAdd(int* cell, int v) { atomicAdd(cell, v); }
+
 template <bool PLUS, typename T, typename AddOp>
 __device__ __forceinline__ void mxmCombine(T* cell, T v, AddOp add_op) {
-  if (PLUS) atomicAdd(cell, v);
+  if (PLUS) mxmAdd(cell, v);
   else atomicCombine(cell, v, add_op);
 }
 

@@ -1,6 +1,8 @@
 // graphblast_b200 backend — hub-cached, TMA-staged generic-semiring pull SpMV.
 //
-// Same contract as spmvMergeKernelT (kernels/spmv_pull.cuh; replaces
+// Same contract as spmvMergeKernelT, bit for bit wherever the fold's order does
+// not matter: every product is rounded before it is added, as there (the
+// multiplies functor's __fmul_rn; no FFMA).  (kernels/spmv_pull.cuh; replaces
 // mgpu::SpmvCsrBinary, reference spmv.hpp:188-190 and
 // ext/moderngpu/include/kernels/spmvcsr.cuh:334-413,489-587), built for what
 // bounds that kernel: every gathered u[col] of a power-law graph is its own L1

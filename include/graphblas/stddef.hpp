@@ -29,7 +29,23 @@ struct NAME {                                                                 \
 #define GB_NONE
 
 namespace graphblas {
-GB_DEFINE_BINARY_OP(logical_or,    GB_BOOL, GB_BOOL, GB_BOOL, lhs || rhs)
+// A float product is rounded before anything adds it: on the device __fmul_rn
+// keeps the compiler from contracting mul_op and add_op into one FFMA, which
+// would round a kernel's sums differently from another route's (and turn an
+// overflowing product next to -FLT_MAX into a finite sum).
+template <typename T_in1, typename T_in2>
+inline GRB_HOST_DEVICE auto gbMul(T_in1 lhs, T_in2 rhs) -> decltype(lhs * rhs) {
+  return lhs * rhs;
+}
+inline GRB_HOST_DEVICE float gbMul(float lhs, float rhs) {
+#ifdef __CUDA_ARCH__
+  return __fmul_rn(lhs, rhs);
+#else
+  return lhs * rhs;
+#endif
+}
+
+GB_DEFINE_BINARY_OP(logical_or,   GB_BOOL, GB_BOOL, GB_BOOL, lhs || rhs)
 GB_DEFINE_BINARY_OP(logical_and,   GB_BOOL, GB_BOOL, GB_BOOL, lhs && rhs)
 GB_DEFINE_BINARY_OP(logical_xor,   GB_BOOL, GB_BOOL, GB_BOOL,
                     (lhs && !rhs) || (!lhs && rhs))
@@ -45,7 +61,7 @@ GB_DEFINE_BINARY_OP(minimum,       GB_NONE, GB_SAME, GB_SAME, min(lhs, rhs))
 GB_DEFINE_BINARY_OP(maximum,       GB_NONE, GB_SAME, GB_SAME, max(lhs, rhs))
 GB_DEFINE_BINARY_OP(plus,          GB_NONE, GB_SAME, GB_SAME, lhs + rhs)
 GB_DEFINE_BINARY_OP(minus,         GB_NONE, GB_SAME, GB_SAME, lhs - rhs)
-GB_DEFINE_BINARY_OP(multiplies,    GB_NONE, GB_SAME, GB_SAME, lhs * rhs)
+GB_DEFINE_BINARY_OP(multiplies,    GB_NONE, GB_SAME, GB_SAME, gbMul(lhs, rhs))
 GB_DEFINE_BINARY_OP(divides,       GB_NONE, GB_SAME, GB_SAME, lhs / rhs)
 GB_DEFINE_BINARY_OP(select_second, GB_NONE, GB_SAME, GB_SAME, rhs)
 }  // namespace graphblas

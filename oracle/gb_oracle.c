@@ -25,8 +25,8 @@ static float apply_op(int op, float a, float b) {
     case OP_MINUS:  return a - b;
     case OP_MUL:    return a * b;
     case OP_DIV:    return a / b;
-    case OP_MIN:    return a < b ? a : b;      /* CUDA/C++ min(a,b) */
-    case OP_MAX:    return a > b ? a : b;
+    case OP_MIN:    return fminf(a, b);      /* CUDA min(a,b): a NaN operand is ignored */
+    case OP_MAX:    return fmaxf(a, b);
     case OP_GT:     return a > b ? 1.f : 0.f;
     case OP_LT:     return a < b ? 1.f : 0.f;
     case OP_NE:     return a != b ? 1.f : 0.f;

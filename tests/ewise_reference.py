@@ -243,10 +243,8 @@ def reduce(monoid, x):
         return float(x64.sum()), (len(x) + 1)*2.0**-24*float(np.abs(x64).sum())
     if op == "mul":
         return F32(np.prod(x.astype(np.float64))), None
-    if op == "min":
-        return F32(min(F32(ident), x.min())), None
-    if op == "max":
-        return F32(max(F32(ident), x.max())), None
+    if op in ("min", "max"):
+        return F32(OPS[op](F32(ident), OPS[op].reduce(x))), None   # NaN ignored
     if op == "or":
         return F32(bool(np.any(x != 0))), None
     return F32(0), None                            # and: and(false, ...) is false

@@ -19,6 +19,30 @@ def _flag(x):
     return x.astype(F32)
 
 
+class _NanIgnoring(object):
+    """np.fmin / np.fmax on operands multiplied by 1 first: numpy's fmin returns NaN
+    for a signaling NaN operand, where fminf and the device's min ignore it as they
+    ignore a quiet one.  x * 1 quiets a signaling NaN and leaves every other value,
+    a zero's sign included, as it is."""
+
+    def __init__(self, ufunc):
+        self.ufunc = ufunc
+
+    def __call__(self, a, b):
+        return self.ufunc(_quiet(a), _quiet(b))
+
+    def reduce(self, x):
+        return self.ufunc.reduce(_quiet(x))
+
+    def reduceat(self, x, at):
+        return self.ufunc.reduceat(_quiet(x), at)
+
+
+def _quiet(x):
+    x = np.asarray(x)
+    return x*x.dtype.type(1)
+
+
 OPS = {
     "or": lambda a, b: _flag((a != 0) | (b != 0)),
     "and": lambda a, b: _flag((a != 0) & (b != 0)),
@@ -26,8 +50,8 @@ OPS = {
     "minus": lambda a, b: a - b,
     "mul": lambda a, b: a * b,
     "div": lambda a, b: a / b,
-    "min": lambda a, b: np.where(a < b, a, b),
-    "max": lambda a, b: np.where(a > b, a, b),
+    "min": _NanIgnoring(np.fmin),     # a NaN operand is ignored (fminf; ieee_reference)
+    "max": _NanIgnoring(np.fmax),
     "gt": lambda a, b: _flag(a > b),
     "lt": lambda a, b: _flag(a < b),
     "ne": lambda a, b: _flag(a != b),

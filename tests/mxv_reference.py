@@ -67,7 +67,7 @@ def pull(semiring, ptr, ind, val, u, mask=None, scmp=False, w_old=None):
                 mag[nonempty] = np.add.reduceat(np.abs(p64), starts)
             bound = (np.diff(ptr) + 1)*2.0**-24*mag
         elif add_name in ("min", "max"):
-            red = np.minimum if add_name == "min" else np.maximum
+            red = add                 # np.fmin / np.fmax: NaN products are ignored
             w = np.full(n, ident, F32)
             if nonempty.any():
                 part = red.reduceat(prods, ptr[:-1][nonempty])
