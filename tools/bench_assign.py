@@ -27,44 +27,26 @@ written,
 "ewise_add_ms" times gb.eWiseAdd of C with the embedded source E built on the host
 (C ∪ E, the merge assign runs after building E), on the same CSR-only C.
 """
-import argparse
 import json
-import os
-import sys
 
 import numpy as np
 import torch
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, HERE)
-sys.path.insert(0, os.path.join(os.path.dirname(HERE), "tests"))
-
-from bench_ewise import hbm_peak_gbps             # noqa: E402
-from bench_mxm import card, timed                 # noqa: E402
-import graphblast_b200 as gb                      # noqa: E402
-from graphblast_b200 import graphs                # noqa: E402
-import assign_reference as R                      # noqa: E402
+# benchlib first: it puts the repository root and tests/ on sys.path
+from benchlib import (event_ms, hbm_peak_gbps, header, new_matrix, parser, rmat_csr,
+                      selected)
+import graphblast_b200 as gb
+from graphblast_b200 import graphs
+import assign_reference as R
 
 
 def compulsory_bytes(m, nnz_c, n_i, nnz_a, nnz_out):
     return 4*(m + 1) + 8*nnz_c + 4*(n_i + 1) + 8*nnz_a + 4*(m + 1) + 8*nnz_out
 
 
-def rmat(scale, seed):
-    src, dst = graphs.rmat_edges(scale, seed=seed)
-    rp, ci = graphs.build_csr(1 << scale, src, dst, True)
-    del src, dst
-    return rp, ci
-
-
 def matrix(n, ncols, rp, ci, val, csr_only, symmetric):
     """A Matrix over copies of the device CSR (rp, ci, val)."""
-    if csr_only:
-        os.environ["GRB_SPARSE_MATRIX_FORMAT"] = "1"
-    try:
-        M = gb.Matrix(n, ncols)
-    finally:
-        os.environ.pop("GRB_SPARSE_MATRIX_FORMAT", None)
+    M = new_matrix(n, ncols, csr_only)
     M.build_device_csr(rp.clone(), ci.clone(), val.clone(), ci.numel(), None, None, None,
                        symmetric=symmetric)
     return M
@@ -104,7 +86,7 @@ def measure(case, args, peak):
     e_rows, e_cols, e_vals = want[3]
     del got, want
 
-    def timed_call(csr_only):
+    def rebuilt_c_ms(csr_only):
         ts = []
         for it in range(args.warmup + args.iters):
             C_ = matrix(n, n, rp, ci, val, csr_only, case.symmetric)
@@ -118,20 +100,17 @@ def measure(case, args, peak):
                 ts.append(a.elapsed_time(b))
             del C_
         return float(np.median(ts))
-    rec["ms"] = timed_call(True)
-    rec["ms_with_csc"] = timed_call(False)
+    rec["ms"] = rebuilt_c_ms(True)
+    rec["ms_with_csc"] = rebuilt_c_ms(False)
     # yardstick: C ∪ E through the matrix eWiseAdd on a CSR-only C
     E = gb.Matrix(n, n)
     E.build(e_rows, e_cols, e_vals)
     C_ = matrix(n, n, rp, ci, val, True, case.symmetric)
-    os.environ["GRB_SPARSE_MATRIX_FORMAT"] = "1"
-    try:
-        out = gb.Matrix(n, n)
-    finally:
-        os.environ.pop("GRB_SPARSE_MATRIX_FORMAT", None)
-    rec["ewise_add_ms"] = timed(lambda: gb.eWiseAdd(out, None, None, gb.Semiring.PlusMultiplies,
-                                                    C_, E, gb.Descriptor()),
-                                args.iters, args.warmup)
+    out = new_matrix(n, n, True)
+    rec["ewise_add_ms"] = event_ms(lambda: gb.eWiseAdd(out, None, None,
+                                                       gb.Semiring.PlusMultiplies, C_, E,
+                                                       gb.Descriptor()),
+                                   args.iters, args.warmup)
     del E, C_, out
     cb = compulsory_bytes(n, rec["nnz_C"], case.n_i, case.nnz_a, rec["nnz_out"])
     rec["compulsory_GB"] = cb/1e9
@@ -152,11 +131,11 @@ def embedded(I, J, src, n):
 
 def workloads(scale, rng, sets):
     n = 1 << scale
-    rp, ci = rmat(scale, 1)
+    _, rp, ci = rmat_csr(scale, seed=1)
     val = torch.ones(ci.numel(), dtype=torch.float32, device="cuda")
     c_arrays = (rp, ci, val)
     h_c = (rp.cpu().numpy(), ci.cpu().numpy(), np.ones(ci.numel(), np.float32))
-    rp2, ci2 = rmat(scale, 2)
+    _, rp2, ci2 = rmat_csr(scale, seed=2)
     A2 = graphs.matrix_from_csr(n, rp2, ci2)
     d = gb.Descriptor()
     cases = []
@@ -219,17 +198,12 @@ def rmat22_extra(n, A2, c_arrays, h_c, rng, s10):
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--iters", type=int, default=10)
-    ap.add_argument("--warmup", type=int, default=2)
-    ap.add_argument("--only", default=None, help="rmat22 or rmat24")
-    args = ap.parse_args()
+    args = parser(iters=10, warmup=2, only="rmat22 or rmat24").parse_args()
     gb.init(0)
     peak = hbm_peak_gbps()
-    print(json.dumps({"card": card(), "torch": torch.__version__,
-                      "peak_GBps": peak}), flush=True)
+    header(peak_GBps=peak)
     rng = np.random.RandomState(7)
-    if args.only in (None, "rmat22"):
+    if selected(args.only, "rmat22"):
         n = 1 << 22
         s10 = np.sort(rng.choice(n, n//10, replace=False)).astype(np.int32)
         sh = rng.permutation(s10).astype(np.int32)
@@ -242,7 +216,7 @@ def main():
             measure(case, args, peak)
         del A2, c_arrays, h_c, cases
         torch.cuda.empty_cache()
-    if args.only in (None, "rmat24"):
+    if selected(args.only, "rmat24"):
         n = 1 << 24
         s50 = np.sort(rng.choice(n, n//2, replace=False)).astype(np.int32)
         _, A2, c_arrays, h_c, cases = workloads(24, rng, [("rmat24_induced50", s50, None)])

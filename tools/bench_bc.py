@@ -12,7 +12,7 @@ Workloads:
                   in-lists of the path-count pull are the CSR rows.
   rmat22_directed the same edges stored one way (self-loops and duplicates removed),
                   adopted with its CSR and CSC: a non-symmetric input.
-  grid27          the 27-point stencil on a 128^3 grid of tools/bench_mxm.py (self-loops
+  grid27          the 27-point stencil on a 128^3 grid of tools/benchlib.py (self-loops
                   included, which BC ignores): one component, up to 127 levels from a
                   source, so a batch runs many grid-wide levels.
 Sources: a numpy RandomState(7) sample without repeats among the vertices with a stored
@@ -33,31 +33,18 @@ highest-degree vertex on the same matrix (the flags of bench.py), and
 BFS traversals, which compute no path counts or dependencies.  "card" is the GPU's name
 and power limit, read in the same run.
 """
-import argparse
 import json
-import os
-import sys
 import time
 import warnings
 
 import numpy as np
 import torch
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, HERE)
-sys.path.insert(0, os.path.join(os.path.dirname(HERE), "tests"))
-
-from bench_mxm import card, grid27                # noqa: E402
-import bc_reference                               # noqa: E402
-import graphblast_b200 as gb                      # noqa: E402
-from graphblast_b200 import algorithm, graphs     # noqa: E402
-
-
-def median_ms(fn, iters, warmup):
-    """Median of the device times fn() returns, after warmup calls."""
-    for _ in range(warmup):
-        fn()
-    return float(np.median([fn() for _ in range(iters)]))
+# benchlib first: it puts the repository root and tests/ on sys.path
+from benchlib import card, device_ms, grid27, header, parser, run
+import bc_reference
+import graphblast_b200 as gb
+from graphblast_b200 import algorithm, graphs
 
 
 def rmat(scale, undirected=True):
@@ -145,7 +132,7 @@ def measure(name, n, rp, ci, cp, ri, symmetric, args):
     bdesc = gb.Descriptor(mxvmode=0, struconly=1, opreuse=1, earlyexit=1)
     lv = gb.Vector(n)
     top = int(np.argmax(deg))
-    bfs_ms = median_ms(lambda: algorithm.bfs(lv, A, top, bdesc, timed=True), args.iters,
+    bfs_ms = device_ms(lambda: algorithm.bfs(lv, A, top, bdesc, timed=True), args.iters,
                        args.warmup)
     del lv
 
@@ -155,7 +142,7 @@ def measure(name, n, rp, ci, cp, ri, symmetric, args):
         rec = {"workload": name, "n": n, "nnz": nnz, "symmetric": symmetric,
                "nsources": count, "batches": (count + 31)//32, "card": card()}
         v = gb.Vector(n)
-        rec["ms"] = median_ms(lambda: algorithm.bc(v, A, desc, sources), args.iters,
+        rec["ms"] = device_ms(lambda: algorithm.bc(v, A, desc, sources), args.iters,
                               args.warmup)
         got = v.extractTuples()
         del v
@@ -186,27 +173,18 @@ def measure(name, n, rp, ci, cp, ri, symmetric, args):
                           "cpu_sources": args.cpu_sources,
                           "cpu": "tests/bc_reference.py, numpy/scipy float64, one host "
                                  "thread, pattern build included"}), flush=True)
-    del A
-    torch.cuda.empty_cache()
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--iters", type=int, default=5)
-    ap.add_argument("--warmup", type=int, default=1)
+    ap = parser(iters=5, warmup=1, only="rmat22, rmat22_directed or grid27")
     ap.add_argument("--sources", type=int, nargs="+", default=[32, 256])
     ap.add_argument("--cpu-sources", type=int, default=1)
-    ap.add_argument("--only", default=None, help="rmat22, rmat22_directed or grid27")
     args = ap.parse_args()
     gb.init(0)
-    print(json.dumps({"card": card(), "torch": torch.__version__}), flush=True)
-    builders = [("rmat22", lambda: rmat(22), True),
-                ("rmat22_directed", lambda: rmat(22, undirected=False), False),
-                ("grid27", grid, True)]
-    for name, build, symmetric in builders:
-        if args.only in (None, name):
-            measure(name, *build(), symmetric, args)
-            torch.cuda.empty_cache()
+    header()
+    run([("rmat22", lambda: rmat(22), True),
+         ("rmat22_directed", lambda: rmat(22, undirected=False), False),
+         ("grid27", grid, True)], args, measure)
 
 
 if __name__ == "__main__":

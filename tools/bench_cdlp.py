@@ -9,9 +9,9 @@ Workloads:
                   symmetric: the kernel reads the CSR alone.
   rmat22_directed R-MAT-22 with each edge stored one way only, CSR and CSC adopted:
                   every list is read twice, once from each side.
-  grid27          the 27-point stencil on a 128^3 grid of tools/bench_mxm.py (self-loops
+  grid27          the 27-point stencil on a 128^3 grid of tools/benchlib.py (self-loops
                   included): lists of 8 to 27 entries, all in the short class.
-  pieces          the 4096 pieces of 1024 vertices of tools/bench_cc.py.
+  pieces          the 4096 pieces of 1024 vertices of tools/benchlib.py's tree_pieces.
 
 Settings: max_iter = 10 (the Graphalytics default), and one run with max_iter = 1000
 that stops at the first iteration that changes nothing ("fix_iterations"; 1000 when no
@@ -29,65 +29,46 @@ CSR, and the CSC when it is held apart) at 3.35 TB/s, the H100 SXM data-sheet HB
 bandwidth: computed from sizes, a bound and not an achieved rate.  "card" is the GPU's
 name and power limit, read in the same run.
 """
-import argparse
 import json
-import os
-import sys
 import time
 
 import numpy as np
-import torch
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, HERE)
-sys.path.insert(0, os.path.join(os.path.dirname(HERE), "tests"))
+# benchlib first: it puts the repository root and tests/ on sys.path
+from benchlib import (adopt_csr_csc, card, device_ms, grid27, header, parser, rmat_csr, run,
+                      stream_bound_ms, tree_pieces)
+import cdlp_reference as R
+import graphblast_b200 as gb
+from graphblast_b200 import algorithm, graphs
 
-from bench_cc import pieces                       # noqa: E402
-from bench_mxm import card, grid27                # noqa: E402
-import cdlp_reference as R                        # noqa: E402
-import graphblast_b200 as gb                      # noqa: E402
-from graphblast_b200 import algorithm, graphs     # noqa: E402
-
-HBM_BYTES_PER_S = 3.35e12
 MAX_ITER = 10
 FIX_ITER = 1000
 FIX_CHECK_MAX = 60
 
 
-def rmat(scale, undirected=True):
-    src, dst = graphs.rmat_edges(scale, seed=0)
-    n = 1 << scale
-    rp, ci = graphs.build_csr(n, src, dst, undirected)
-    if undirected:
-        return n, rp, ci, graphs.matrix_from_csr(n, rp, ci, symmetric=True)
-    cp, ri = graphs.build_csr(n, dst, src, False)
-    A = gb.Matrix(n, n)
-    A.build_device_csr(rp, ci, torch.ones(ci.numel(), dtype=torch.float32, device="cuda"),
-                       ci.numel(), cp, ri,
-                       torch.ones(ri.numel(), dtype=torch.float32, device="cuda"))
-    return n, rp, ci, A
-
-
 def symmetric(build):
     def make():
         n, rp, ci = build()
-        return n, rp, ci, graphs.matrix_from_csr(n, rp, ci, symmetric=True)
+        return n, graphs.matrix_from_csr(n, rp, ci, symmetric=True), rp, ci
     return make
 
 
-def measure(name, n, rp, ci, A, lists, args):
+def directed(scale):
+    n = 1 << scale
+    return (n,) + adopt_csr_csc(n, *graphs.rmat_edges(scale, seed=0), False)
+
+
+def measure(name, n, A, rp, ci, lists, args):
     nnz = int(ci.numel())
     rec = {"workload": name, "n": n, "nnz": nnz, "lists_read": lists, "card": card()}
     desc = gb.Descriptor()
     v = gb.Vector(n)
     out = {}
 
-    def run(max_iter):
+    def run_cdlp(max_iter):
         out["k"], out["it"], ms = algorithm.cdlp(v, A, max_iter, desc)
         return ms
-    for _ in range(args.warmup):
-        run(MAX_ITER)
-    times = [run(MAX_ITER) for _ in range(args.iters)]
+    ms = device_ms(lambda: run_cdlp(MAX_ITER), args.iters, args.warmup)
     got = v.extractTuples().astype(np.int64)
     rec["communities"], rec["iterations"] = out["k"], out["it"]
     s = algorithm.cdlp_stats()
@@ -101,16 +82,16 @@ def measure(name, n, rp, ci, A, lists, args):
         rec["cpu_ms"] = cpu_ms
     rec["equals_checker"] = bool(np.array_equal(got, want) and
                                  (out["k"], out["it"]) == (want_k, want_it))
-    rec["stream_bound_ms"] = lists*(4.0*(n + 1) + 4.0*nnz)/HBM_BYTES_PER_S*1e3
+    rec["stream_bound_ms"] = stream_bound_ms(lists*(4.0*(n + 1) + 4.0*nnz))
     if rec["equals_checker"]:
-        rec["ms"] = float(np.median(times))
+        rec["ms"] = ms
         rec["ms_per_iteration"] = rec["ms"]/max(out["it"], 1)
         rec["over_stream_bound"] = rec["ms_per_iteration"]/rec["stream_bound_ms"]
         if "cpu_ms" in rec:
             rec["cpu_over_cdlp"] = rec["cpu_ms"]/rec["ms"]
 
-    run(FIX_ITER)                                   # warm
-    fix_ms = run(FIX_ITER)
+    run_cdlp(FIX_ITER)                              # warm
+    fix_ms = run_cdlp(FIX_ITER)
     rec["fix_iterations"] = out["it"]
     rec["fix_equals_checker"] = None
     if out["it"] <= FIX_CHECK_MAX:
@@ -123,29 +104,18 @@ def measure(name, n, rp, ci, A, lists, args):
     else:
         rec["fix_ms_per_iteration_unchecked"] = fix_ms/out["it"]
     print(json.dumps(rec), flush=True)
-    del v
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--iters", type=int, default=10)
-    ap.add_argument("--warmup", type=int, default=2)
-    ap.add_argument("--only", default=None,
-                    help="rmat22, rmat24, rmat22_directed, grid27 or pieces")
-    args = ap.parse_args()
+    args = parser(iters=10, warmup=2,
+                  only="rmat22, rmat24, rmat22_directed, grid27 or pieces").parse_args()
     gb.init(0)
-    print(json.dumps({"card": card(), "torch": torch.__version__}), flush=True)
-    builders = [("rmat22", lambda: rmat(22), 1),
-                ("rmat24", lambda: rmat(24), 1),
-                ("rmat22_directed", lambda: rmat(22, undirected=False), 2),
-                ("grid27", symmetric(lambda: grid27(128)), 1),
-                ("pieces", symmetric(pieces), 1)]
-    for name, build, lists in builders:
-        if args.only in (None, name):
-            n, rp, ci, A = build()
-            measure(name, n, rp, ci, A, lists, args)
-            del A, rp, ci
-            torch.cuda.empty_cache()
+    header()
+    run([("rmat22", symmetric(lambda: rmat_csr(22, seed=0)), 1),
+         ("rmat24", symmetric(lambda: rmat_csr(24, seed=0)), 1),
+         ("rmat22_directed", lambda: directed(22), 2),
+         ("grid27", symmetric(lambda: grid27(128)), 1),
+         ("pieces", symmetric(tree_pieces), 1)], args, measure)
 
 
 if __name__ == "__main__":

@@ -22,20 +22,16 @@ row offsets and entries are written once:
 "peak_GBps" is a device-to-device copy measured in the same run (read + write).
 cuSPARSE's result must equal ours entry for entry before its time is quoted.
 """
-import argparse
 import ctypes
 import json
-import os
-import sys
 
 import numpy as np
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-
-from bench_mxm import card, new_matrix, timed     # noqa: E402
-import graphblast_b200 as gb                      # noqa: E402
-from graphblast_b200 import graphs                # noqa: E402
+# benchlib first: it puts the repository root and tests/ on sys.path
+from benchlib import event_ms, hbm_peak_gbps, header, new_matrix, parser, rmat_csr, selected
+import graphblast_b200 as gb
+from graphblast_b200 import graphs
 
 INGEST_DROP_LOOPS, INGEST_DEDUP = 2, 4
 
@@ -44,20 +40,9 @@ def compulsory_bytes(m, nnz_in, nnz_c):
     return 2*(8*(m + 1) + 4*nnz_in) + 4*nnz_in + 4*(m + 1) + 8*nnz_c
 
 
-def hbm_peak_gbps():
-    x = torch.empty(1 << 29, dtype=torch.float32, device="cuda")     # 2 GiB
-    y = torch.empty_like(x)
-    ms = timed(lambda: y.copy_(x), 10, 2)
-    del x, y
-    torch.cuda.empty_cache()
-    return 2*(1 << 31)/ms/1e6
-
-
 def symmetric(scale, seed):
-    src, dst = graphs.rmat_edges(scale, seed=seed)
-    rp, ci = graphs.build_csr(1 << scale, src, dst, True)
-    del src, dst
-    return graphs.matrix_from_csr(1 << scale, rp, ci), rp, ci
+    n, rp, ci = rmat_csr(scale, seed=seed)
+    return graphs.matrix_from_csr(n, rp, ci), rp, ci
 
 
 def directed(scale):
@@ -85,11 +70,11 @@ def measure(name, add, n, A, B, args, peak, desc=None, cusparse=None, with_csc=T
            "nnz_A": A.nvals(), "nnz_B": B.nvals()}
     if with_csc:
         C = gb.Matrix(n, n)
-        rec["ms_with_csc"] = timed(lambda: f(C, None, None, 1, A, B, desc), args.iters,
-                                   args.warmup)
+        rec["ms_with_csc"] = event_ms(lambda: f(C, None, None, 1, A, B, desc), args.iters,
+                                      args.warmup)
         del C
-    C = new_matrix(n, True)
-    rec["ms"] = timed(lambda: f(C, None, None, 1, A, B, desc), args.iters, args.warmup)
+    C = new_matrix(n, n, True)
+    rec["ms"] = event_ms(lambda: f(C, None, None, 1, A, B, desc), args.iters, args.warmup)
     rec["nnz_C"] = C.nvals()
     cb = compulsory_bytes(n, rec["nnz_A"] + rec["nnz_B"], rec["nnz_C"])
     rec["compulsory_GB"] = cb/1e9
@@ -107,7 +92,7 @@ def measure(name, add, n, A, B, args, peak, desc=None, cusparse=None, with_csc=T
             rec["cusparse_agrees"] = bool(agrees)
             del S
             if agrees:
-                rec["cusparse_ms"] = timed(lambda: TA + TB, args.iters, args.warmup)
+                rec["cusparse_ms"] = event_ms(lambda: TA + TB, args.iters, args.warmup)
             del TA, TB
         except torch.cuda.OutOfMemoryError:
             rec["cusparse"] = "out of memory"
@@ -116,16 +101,11 @@ def measure(name, add, n, A, B, args, peak, desc=None, cusparse=None, with_csc=T
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--iters", type=int, default=10)
-    ap.add_argument("--warmup", type=int, default=2)
-    ap.add_argument("--only", default=None, help="rmat22, rmat22_sym or rmat24")
-    args = ap.parse_args()
+    args = parser(iters=10, warmup=2, only="rmat22, rmat22_sym or rmat24").parse_args()
     gb.init(0)
     peak = hbm_peak_gbps()
-    print(json.dumps({"card": card(), "torch": torch.__version__,
-                      "peak_GBps": peak}), flush=True)
-    if args.only in (None, "rmat22"):
+    header(peak_GBps=peak)
+    if selected(args.only, "rmat22"):
         n = 1 << 22
         A, arp, aci = symmetric(22, 1)
         B, brp, bci = symmetric(22, 2)
@@ -135,7 +115,7 @@ def main():
         measure("rmat22_self", True, n, A, A, args, peak)
         del A, B, arp, aci, brp, bci, ts
         torch.cuda.empty_cache()
-    if args.only in (None, "rmat22_sym"):
+    if selected(args.only, "rmat22_sym"):
         n = 1 << 22
         A = directed(22)
         tran1 = gb.Descriptor()
@@ -143,7 +123,7 @@ def main():
         measure("rmat22_sym", True, n, A, A, args, peak, desc=tran1)
         del A
         torch.cuda.empty_cache()
-    if args.only in (None, "rmat24"):
+    if selected(args.only, "rmat24"):
         n = 1 << 24
         A, arp, aci = symmetric(24, 1)
         B, brp, bci = symmetric(24, 2)

@@ -25,21 +25,17 @@ itself built once (8|J| + 4 ncols(A)), and C's row offsets and entries written o
 "peak_GBps" is a device-to-device copy measured in the same run (read + write).
 The device result must equal scipy's entry for entry before either time is quoted.
 """
-import argparse
 import json
-import os
-import sys
 import time
 
 import numpy as np
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-
-from bench_ewise import hbm_peak_gbps             # noqa: E402
-from bench_mxm import card, timed                 # noqa: E402
-import graphblast_b200 as gb                      # noqa: E402
-from graphblast_b200 import graphs                # noqa: E402
+# benchlib first: it puts the repository root and tests/ on sys.path
+from benchlib import (event_ms, hbm_peak_gbps, header, new_matrix, parser, rmat_csr,
+                      selected)
+import graphblast_b200 as gb
+from graphblast_b200 import graphs
 
 
 def compulsory_bytes(n_i, n_j, ncols, sel, nnz_c):
@@ -51,24 +47,14 @@ def compulsory_bytes(n_i, n_j, ncols, sel, nnz_c):
 
 
 def symmetric(scale):
-    src, dst = graphs.rmat_edges(scale, seed=1)
-    rp, ci = graphs.build_csr(1 << scale, src, dst, True)
-    del src, dst
-    return graphs.matrix_from_csr(1 << scale, rp, ci), rp, ci
+    n, rp, ci = rmat_csr(scale, seed=1)
+    return graphs.matrix_from_csr(n, rp, ci), rp, ci
 
 
 def scipy_of(rp, ci, n):
     import scipy.sparse as sp
     rp_h, ci_h = rp.cpu().numpy(), ci.cpu().numpy()
     return sp.csr_matrix((np.ones(len(ci_h), np.float32), ci_h, rp_h), shape=(n, n))
-
-
-def csr_only(nrows, ncols):
-    os.environ["GRB_SPARSE_MATRIX_FORMAT"] = "1"
-    try:
-        return gb.Matrix(nrows, ncols)
-    finally:
-        os.environ.pop("GRB_SPARSE_MATRIX_FORMAT", None)
 
 
 def measure(name, n, A, host, I, J, args, peak, in_place=False):
@@ -85,7 +71,7 @@ def measure(name, n, A, host, I, J, args, peak, in_place=False):
     rec["scipy_ms"] = (time.perf_counter() - t0)*1e3
     # the check runs on a separate C; the in-place workload then permutes A itself
     # on every timed call (the same work each time)
-    C = csr_only(n_i, n_j)
+    C = new_matrix(n_i, n_j, True)
     gb.extract(C, None, None, A, I, n_i, J, n_j, desc)
     rp, ci, val = C.extract_csr()
     agrees = (np.array_equal(rp, want.indptr) and np.array_equal(ci, want.indices) and
@@ -97,13 +83,13 @@ def measure(name, n, A, host, I, J, args, peak, in_place=False):
         print(json.dumps(rec), flush=True)
         raise SystemExit("%s: device result differs from scipy" % name)
     target = A if in_place else C
-    rec["ms"] = timed(lambda: gb.extract(target, None, None, A, I, n_i, J, n_j, desc),
-                      args.iters, args.warmup)
+    rec["ms"] = event_ms(lambda: gb.extract(target, None, None, A, I, n_i, J, n_j, desc),
+                         args.iters, args.warmup)
     if not in_place:
         del C
         C2 = gb.Matrix(n_i, n_j)
-        rec["ms_with_csc"] = timed(lambda: gb.extract(C2, None, None, A, I, n_i, J, n_j,
-                                                      desc), args.iters, args.warmup)
+        rec["ms_with_csc"] = event_ms(lambda: gb.extract(C2, None, None, A, I, n_i, J, n_j,
+                                                         desc), args.iters, args.warmup)
         del C2
     cb = compulsory_bytes(n_i, None if J is None else n_j, n, sel, rec["nnz_C"])
     rec["compulsory_GB"] = cb/1e9
@@ -114,17 +100,12 @@ def measure(name, n, A, host, I, J, args, peak, in_place=False):
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--iters", type=int, default=10)
-    ap.add_argument("--warmup", type=int, default=2)
-    ap.add_argument("--only", default=None, help="rmat22 or rmat24")
-    args = ap.parse_args()
+    args = parser(iters=10, warmup=2, only="rmat22 or rmat24").parse_args()
     gb.init(0)
     peak = hbm_peak_gbps()
-    print(json.dumps({"card": card(), "torch": torch.__version__,
-                      "peak_GBps": peak}), flush=True)
+    header(peak_GBps=peak)
     rng = np.random.RandomState(7)
-    if args.only in (None, "rmat22"):
+    if selected(args.only, "rmat22"):
         n = 1 << 22
         A, rp, ci = symmetric(22)
         host = scipy_of(rp, ci, n)
@@ -139,7 +120,7 @@ def main():
         measure("rmat22_perm", n, A, host, P, P, args, peak, in_place=True)
         del A, rp, ci, host
         torch.cuda.empty_cache()
-    if args.only in (None, "rmat24"):
+    if selected(args.only, "rmat24"):
         n = 1 << 24
         A, rp, ci = symmetric(24)
         host = scipy_of(rp, ci, n)

@@ -5,7 +5,7 @@ csrcolor and against the single-thread CPU oracle.
 
 Workloads: R-MAT (0.57, 0.19, 0.19, 0.05) of scale 22 and 24, edge factor 16,
 symmetrised, self-loops and duplicate edges removed (graphs.rmat_edges /
-build_csr / matrix_from_csr), seed 0.
+build_csr / matrix_from_csr), seed 1.
 
 Each line is one JSON record.  "ms" is the median of the CUDA-event times that gc
 returns for warm calls.  Before any time is quoted, the colouring must equal the
@@ -15,26 +15,20 @@ round count.  cuSPARSE's cusparseScsrcolor (deprecated, still exported by the
 libcusparse.so.12 that ships with torch) runs with fraction = 1.0; its colouring is
 checked as proper before its time and colour count are quoted.  It is not greedy.
 """
-import argparse
 import ctypes as C
 import glob
 import json
 import os
-import sys
 import time
 
 import numpy as np
 import torch
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, HERE)
-sys.path.insert(0, os.path.join(os.path.dirname(HERE), "tests"))
-
-from bench_mxm import card, timed                 # noqa: E402
-import graphblast_b200 as gb                      # noqa: E402
-from graphblast_b200 import algorithm, graphs     # noqa: E402
-import greedy_oracle                              # noqa: E402
-import oracle_binding as orc                      # noqa: E402
+# benchlib first: it puts the repository root and tests/ on sys.path
+from benchlib import card, device_ms, event_ms, header, parser, rmat_csr, selected
+import graphblast_b200 as gb
+from graphblast_b200 import algorithm, graphs
+import greedy_oracle
 
 
 def cusparse_lib():
@@ -88,22 +82,18 @@ def proper(colors, rows, ci):
 
 
 def measure(scale, args):
-    n = 1 << scale
-    src, dst = graphs.rmat_edges(scale)
-    rp, ci = graphs.build_csr(n, src, dst, True)
-    del src, dst
+    n, rp, ci = rmat_csr(scale, seed=1)
     A = graphs.matrix_from_csr(n, rp, ci)
     rec = {"workload": "rmat%d" % scale, "n": n, "nnz": int(ci.numel()), "card": card()}
     v = gb.Vector(n)
     desc = gb.Descriptor()
-    for _ in range(args.warmup):
-        algorithm.gc(v, A, 0, desc)
-    times = []
-    for _ in range(args.iters):
-        ncolors, ms = algorithm.gc(v, A, 0, desc)
-        times.append(ms)
-    rec["ms"] = float(np.median(times))
-    rec["ncolors"] = ncolors
+    count = [0]
+
+    def run_gc():
+        count[0], ms = algorithm.gc(v, A, 0, desc)
+        return ms
+    rec["ms"] = device_ms(run_gc, args.iters, args.warmup)
+    rec["ncolors"] = count[0]
     got = v.extractTuples()
 
     h_rp, h_ci = rp.cpu().numpy(), ci.cpu().numpy()
@@ -113,7 +103,7 @@ def measure(scale, args):
     rec["jp_depth"] = depth
     rec["oracle_ncolors"] = want_n
     rec["equals_oracle"] = bool(np.array_equal(got, want.astype(np.float32)) and
-                                ncolors == want_n)
+                                count[0] == want_n)
     rows = np.repeat(np.arange(n, dtype=np.int32), np.diff(h_rp))
     rec["proper"] = proper(got, rows, h_ci)
     if not rec["equals_oracle"]:
@@ -127,7 +117,7 @@ def measure(scale, args):
         if rec["cusparse_proper"]:
             rec["cusparse_ncolors"] = int(cs.ncolors.value)
             rec["cusparse_distinct_colors"] = int(np.unique(colors).size)
-            rec["cusparse_ms"] = timed(cs, args.iters, args.warmup)
+            rec["cusparse_ms"] = event_ms(cs, args.iters, args.warmup)
         cs.close()
         del cs
     except (OSError, RuntimeError, torch.cuda.OutOfMemoryError) as e:
@@ -138,15 +128,11 @@ def measure(scale, args):
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--iters", type=int, default=10)
-    ap.add_argument("--warmup", type=int, default=2)
-    ap.add_argument("--only", default=None, help="rmat22 or rmat24")
-    args = ap.parse_args()
+    args = parser(iters=10, warmup=2, only="rmat22 or rmat24").parse_args()
     gb.init(0)
-    print(json.dumps({"card": card(), "torch": torch.__version__}), flush=True)
+    header()
     for scale in (22, 24):
-        if args.only in (None, "rmat%d" % scale):
+        if selected(args.only, "rmat%d" % scale):
             measure(scale, args)
 
 

@@ -23,33 +23,20 @@ against "triangles_tril" of tests/golden/tc_golden.json where it has the graph, 
 pattern of each ktruss(k) against {tau >= k} of the trussness result.  "card" is the
 GPU's name and power limit, read in the same run.
 """
-import argparse
 import concurrent.futures
 import json
 import os
-import sys
 
 import numpy as np
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-sys.path.insert(0, HERE)
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-
-from bench_mxm import card                        # noqa: E402
-import truss_reference                            # noqa: E402
-import graphblast_b200 as gb                      # noqa: E402
-from graphblast_b200 import algorithm, graphs     # noqa: E402
+# benchlib first: it puts the repository root and tests/ on sys.path
+from benchlib import ROOT, card, device_ms, parser, rmat_csr
+import truss_reference
+import graphblast_b200 as gb
+from graphblast_b200 import algorithm, graphs
 
 KS = (3, 8, 32)
 ORACLE_MAX_SCALE = 20
-
-
-def median_ms(fn, iters, warmup):
-    for _ in range(warmup):
-        fn()
-    return float(np.median([fn() for _ in range(iters)]))
 
 
 def golden_triangles(scale, nnz):
@@ -65,9 +52,7 @@ def same_csr(M, want):
 
 
 def run(scale, iters, warmup):
-    n = 1 << scale
-    src, dst = graphs.rmat_edges(scale)
-    rp, ci = graphs.build_csr(n, src, dst, True)
+    n, rp, ci = rmat_csr(scale, seed=1)
     A = graphs.matrix_from_csr(n, rp, ci)
     h_rp, h_ci = rp.cpu().numpy(), ci.cpu().numpy()
     nnz = len(h_ci)
@@ -123,28 +108,27 @@ def run(scale, iters, warmup):
         ms = algorithm.ktruss(out, A, 2, desc)[1]
         support.append(algorithm.ktruss_stats()[2])
         return ms
-    rec["k2_ms"] = median_ms(k2, iters, warmup)
+    rec["k2_ms"] = device_ms(k2, iters, warmup)
     rec["support_ms"] = float(np.median(support[warmup:]))
     rec["ktruss"] = []
     for k in KS:
-        ms = median_ms(lambda: algorithm.ktruss(out, A, k, desc)[1], iters, warmup)
+        ms = device_ms(lambda: algorithm.ktruss(out, A, k, desc)[1], iters, warmup)
         rounds, levels, _ = algorithm.ktruss_stats()
         rec["ktruss"].append({"k": k, "ms": ms, "edges": out.nvals()//2, "rounds": rounds})
-    ms = median_ms(lambda: algorithm.trussness(out, A, desc)[1], iters, warmup)
+    ms = device_ms(lambda: algorithm.trussness(out, A, desc)[1], iters, warmup)
     rounds, levels, _ = algorithm.ktruss_stats()
     rec["trussness"] = {"ms": ms, "rounds": rounds, "levels": levels}
     L = graphs.matrix_from_csr(n, rp, ci, dtype=gb.api.INT32, symmetric=True)
     L.tril(desc)
     B = gb.Matrix(n, n, dtype=gb.api.INT32)
-    rec["tc_ms"] = median_ms(lambda: algorithm.tc(L, B, desc)[1], iters, warmup)
+    rec["tc_ms"] = device_ms(lambda: algorithm.tc(L, B, desc)[1], iters, warmup)
     return rec
 
 
 def main():
-    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
+    ap = parser(iters=5, warmup=1)
+    ap.description = __doc__.split("\n\n")[0]
     ap.add_argument("--scales", type=int, nargs="+", default=[18, 20, 22])
-    ap.add_argument("--iters", type=int, default=5)
-    ap.add_argument("--warmup", type=int, default=1)
     args = ap.parse_args()
     gb.init(0)
     for scale in args.scales:

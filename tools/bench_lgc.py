@@ -40,7 +40,6 @@ The two do not compute the same floats (the driver's loop is not the checker's o
 so only lgc's p is checked, against the restatement.  "card" is the GPU's name and power
 limit, read in the same run.
 """
-import argparse
 import json
 import os
 import re
@@ -52,28 +51,13 @@ import time
 import numpy as np
 import torch
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, HERE)
-sys.path.insert(0, os.path.join(os.path.dirname(HERE), "tests"))
-
-from bench_mxm import card                        # noqa: E402
-import graphblast_b200 as gb                      # noqa: E402
-from graphblast_b200 import algorithm, graphs     # noqa: E402
-import lgc_reference as L                         # noqa: E402
+# benchlib first: it puts the repository root and tests/ on sys.path
+from benchlib import ROOT, card, device_ms, header, parser, rmat_csr
+import graphblast_b200 as gb
+from graphblast_b200 import algorithm, graphs
+import lgc_reference as L
 
 ROUTES = (("default", 0), ("push", 1), ("pull", 2))
-
-
-def rmat(scale):
-    src, dst = graphs.rmat_edges(scale, seed=0)
-    rp, ci = graphs.build_csr(1 << scale, src, dst, True)
-    return 1 << scale, rp, ci
-
-
-def median_ms(fn, iters, warmup):
-    for _ in range(warmup):
-        fn()
-    return float(np.median([fn() for _ in range(iters)]))
 
 
 def bits(x):
@@ -113,7 +97,7 @@ def measure(name, A, n, h_rp, h_ci, setting, alpha, eps, cap, s, restate, args):
         rec["ms"] = {}
         for route, mode in ROUTES:
             desc = gb.Descriptor(mxvmode=mode, max_niter=cap)
-            rec["ms"][route] = median_ms(
+            rec["ms"][route] = device_ms(
                 lambda: algorithm.lgc(p, A, s, alpha, eps, desc, residual=r)[1],
                 args.iters, args.warmup)
     algorithm.lgc(p, A, s, alpha, eps, gb.Descriptor(max_niter=cap))
@@ -123,7 +107,7 @@ def measure(name, A, n, h_rp, h_ci, setting, alpha, eps, cap, s, restate, args):
         ok = ok and size == want_size and (phi == want_phi or
                                            (np.isnan(phi) and np.isnan(want_phi)))
     if ok and restate:
-        rec["sweep_ms"] = median_ms(lambda: algorithm.lgc_sweep(cl, p, A, gb.Descriptor())[2],
+        rec["sweep_ms"] = device_ms(lambda: algorithm.lgc_sweep(cl, p, A, gb.Descriptor())[2],
                                     args.iters, args.warmup)
     h_p = got["default"][1]
     rec.update(support=int(np.count_nonzero((h_p > 0) & (np.diff(h_rp) > 0))),
@@ -133,8 +117,7 @@ def measure(name, A, n, h_rp, h_ci, setting, alpha, eps, cap, s, restate, args):
 
 def glgc(scale, args):
     """The unchanged glgc driver against lgc on one R-MAT Matrix Market file."""
-    root = os.path.dirname(HERE)
-    driver = os.path.join(root, "oracle", "_ref", "dropin", "glgc")
+    driver = os.path.join(ROOT, "oracle", "_ref", "dropin", "glgc")
     rec = {"workload": "rmat%d.mtx" % scale, "setting": "driver", "card": card()}
     if not os.path.exists(driver):
         rec["glgc"] = "not built"
@@ -142,7 +125,7 @@ def glgc(scale, args):
         return
     with tempfile.TemporaryDirectory() as tmp:
         mtx = os.path.join(tmp, "rmat%d.mtx" % scale)
-        subprocess.check_call([sys.executable, os.path.join(HERE, "gen_rmat_mtx.py"),
+        subprocess.check_call([sys.executable, os.path.join(ROOT, "tools", "gen_rmat_mtx.py"),
                                str(scale), "16", mtx])
         A = gb.Matrix.from_mtx(mtx, directed=2)
         h_rp, h_ci, _ = A.extract_csr()
@@ -166,17 +149,15 @@ def glgc(scale, args):
     rec["checked"] = bool(k == want_k and np.array_equal(bits(p.extractTuples()),
                                                          bits(want_p)))
     if rec["checked"]:
-        rec["lgc_ms"] = median_ms(lambda: algorithm.lgc(p, A, s, alpha, eps, desc)[1],
+        rec["lgc_ms"] = device_ms(lambda: algorithm.lgc(p, A, s, alpha, eps, desc)[1],
                                   args.iters, args.warmup)
     print(json.dumps(rec), flush=True)
 
 
 def main():
-    ap = argparse.ArgumentParser()
+    ap = parser(iters=5, warmup=1)
     ap.add_argument("--scales", type=int, nargs="+", default=[22, 24])
     ap.add_argument("--sources", type=int, default=2)
-    ap.add_argument("--iters", type=int, default=5)
-    ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--driver-rounds", type=int, default=10)
     ap.add_argument("--restate-max", type=int, default=22,
                     help="largest scale also checked against the numpy restatement")
@@ -184,9 +165,9 @@ def main():
                     help="also time the glgc driver on an R-MAT .mtx of this scale")
     args = ap.parse_args()
     gb.init(0)
-    print(json.dumps({"card": card(), "torch": torch.__version__}), flush=True)
+    header()
     for scale in args.scales:
-        n, rp, ci = rmat(scale)
+        n, rp, ci = rmat_csr(scale, seed=0)
         A = graphs.matrix_from_csr(n, rp, ci, symmetric=True)
         h_rp, h_ci = rp.cpu().numpy(), ci.cpu().numpy()
         deg = np.diff(h_rp)

@@ -14,11 +14,11 @@ adopted as a CSR marked symmetric):
   rmat22_distinct distinct float weights: the floats whose bit patterns are 0x3f800000
                   (1.0) plus a seeded permutation of the stored entries, so no two
                   entries tie.
-  grid27          the 27-point stencil on a 128^3 grid of tools/bench_mxm.py (its
+  grid27          the 27-point stencil on a 128^3 grid of tools/benchlib.py (its
                   self-loops ignored), weights 1..64 from the same stream: a mesh where
                   Boruvka's components grow evenly.
-  pieces          tools/bench_cc.py's 4096 random pieces of 1024 vertices, ids
-                  interleaved, weights 1..64: a forest of 4096 trees.
+  pieces          the 4096 random pieces of 1024 vertices of tools/benchlib.py's
+                  tree_pieces, ids interleaved, weights 1..64: a forest of 4096 trees.
 No weight in these workloads is zero, so scipy, which treats stored zeros as missing
 edges, sees the same graph.
 
@@ -34,39 +34,18 @@ the CSR and its values read once, at 3.35 TB/s (the H100 SXM data-sheet HBM3
 bandwidth): a bound, not an achieved rate.  "card" is the GPU's name and power limit,
 read in the same run.
 """
-import argparse
 import json
-import os
-import sys
 import time
 
 import numpy as np
 import torch
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, HERE)
-sys.path.insert(0, os.path.join(os.path.dirname(HERE), "tests"))
-
-from bench_cc import pieces                       # noqa: E402
-from bench_mxm import card, grid27                # noqa: E402
-import graphblast_b200 as gb                      # noqa: E402
-from graphblast_b200 import algorithm, graphs     # noqa: E402
-from msf_reference import msf as checker          # noqa: E402
-
-HBM_BYTES_PER_S = 3.35e12
-
-
-def median_ms(fn, iters, warmup):
-    """Median of the device times fn() returns, after warmup calls."""
-    for _ in range(warmup):
-        fn()
-    return float(np.median([fn() for _ in range(iters)]))
-
-
-def rmat(scale):
-    src, dst = graphs.rmat_edges(scale, seed=0)
-    rp, ci = graphs.build_csr(1 << scale, src, dst, True)
-    return 1 << scale, rp, ci
+# benchlib first: it puts the repository root and tests/ on sys.path
+from benchlib import (card, device_ms, grid27, header, parser, rmat_csr, run,
+                      stream_bound_ms, tree_pieces)
+import graphblast_b200 as gb
+from graphblast_b200 import algorithm, graphs
+from msf_reference import msf as checker
 
 
 def grid():
@@ -126,42 +105,29 @@ def measure(name, n, rp, ci, weights, args):
         (s_weight == out[1] if integer else abs(s_weight - out[1]) <= 1e-12*abs(s_weight)))
     del got_rp, got_ci, got_val, w_rp, w_ci, w_val
 
-    rec["ms"] = median_ms(run_msf, args.iters, args.warmup)
+    rec["ms"] = device_ms(run_msf, args.iters, args.warmup)
     rec["rounds"], rec["barriers"], rec["canon_ms"] = algorithm.msf_stats()
     cv = gb.Vector(n)
-    rec["cc_ms"] = median_ms(lambda: algorithm.cc(cv, A, desc)[1], args.iters, args.warmup)
-    rec["stream_bound_ms"] = (4.0*(n + 1) + 8.0*nnz)/HBM_BYTES_PER_S*1e3
+    rec["cc_ms"] = device_ms(lambda: algorithm.cc(cv, A, desc)[1], args.iters, args.warmup)
+    rec["stream_bound_ms"] = stream_bound_ms(4.0*(n + 1) + 8.0*nnz)
     if rec["equals_checker"] and rec["weight_equals_scipy"]:
         rec["scipy_over_msf"] = rec["scipy_ms"]/rec["ms"]
     else:
         rec.pop("ms")                 # a wrong forest gets no time
     print(json.dumps(rec), flush=True)
-    del A, F, cv
-    torch.cuda.empty_cache()
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--iters", type=int, default=10)
-    ap.add_argument("--warmup", type=int, default=2)
-    ap.add_argument("--only", default=None,
-                    help="rmat22_ties, rmat24_ties, rmat22_distinct, grid27 or pieces "
-                         "(comma-separated)")
-    args = ap.parse_args()
-    only = None if args.only is None else set(args.only.split(","))
+    args = parser(iters=10, warmup=2,
+                  only="rmat22_ties, rmat24_ties, rmat22_distinct, grid27 or "
+                       "pieces").parse_args()
     gb.init(0)
-    print(json.dumps({"card": card(), "torch": torch.__version__}), flush=True)
-    builders = [("rmat22_ties", lambda: rmat(22), sssp_weights),
-                ("rmat24_ties", lambda: rmat(24), sssp_weights),
-                ("rmat22_distinct", lambda: rmat(22), distinct_weights),
-                ("grid27", grid, sssp_weights),
-                ("pieces", pieces, sssp_weights)]
-    for name, build, weights in builders:
-        if only is None or name in only:
-            n, rp, ci = build()
-            measure(name, n, rp, ci, weights, args)
-            del rp, ci
-            torch.cuda.empty_cache()
+    header()
+    run([("rmat22_ties", lambda: rmat_csr(22, seed=0), sssp_weights),
+         ("rmat24_ties", lambda: rmat_csr(24, seed=0), sssp_weights),
+         ("rmat22_distinct", lambda: rmat_csr(22, seed=0), distinct_weights),
+         ("grid27", grid, sssp_weights),
+         ("pieces", tree_pieces, sssp_weights)], args, measure)
 
 
 if __name__ == "__main__":

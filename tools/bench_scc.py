@@ -32,48 +32,23 @@ algorithm.cc (weak components) on the same matrix.  "trimmed", "pivot_size",
 3.35 TB/s (the H100 SXM data-sheet HBM3 bandwidth): a bound, not an achieved rate.
 "card" is the GPU's name and power limit, read in the same run.
 """
-import argparse
 import json
-import os
-import sys
 import time
 
 import numpy as np
 import torch
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, HERE)
-sys.path.insert(0, os.path.join(os.path.dirname(HERE), "tests"))
-
-from bench_mxm import card                        # noqa: E402
-import graphblast_b200 as gb                      # noqa: E402
-from graphblast_b200 import algorithm, graphs     # noqa: E402
-from scc_reference import scc as checker          # noqa: E402
-
-HBM_BYTES_PER_S = 3.35e12
-
-
-def median_ms(fn, iters, warmup):
-    """Median of the device times fn() returns, after warmup calls."""
-    for _ in range(warmup):
-        fn()
-    return float(np.median([fn() for _ in range(iters)]))
-
-
-def adopt(n, src, dst, undirected=False):
-    """CSR from (src, dst), CSC from the swapped endpoints, both adopted."""
-    rp, ci = graphs.build_csr(n, src, dst, undirected)
-    cp, ri = graphs.build_csr(n, dst, src, undirected)
-    A = gb.Matrix(n, n)
-    A.build_device_csr(rp, ci, torch.ones(ci.numel(), dtype=torch.float32, device="cuda"),
-                       ci.numel(), cp, ri,
-                       torch.ones(ri.numel(), dtype=torch.float32, device="cuda"))
-    return A, rp, ci
+# benchlib first: it puts the repository root and tests/ on sys.path
+from benchlib import (adopt_csr_csc, card, device_ms, header, parser, run,
+                      stream_bound_ms)
+import graphblast_b200 as gb
+from graphblast_b200 import algorithm, graphs
+from scc_reference import scc as checker
 
 
 def rmat(scale, undirected=False):
     src, dst = graphs.rmat_edges(scale, seed=0)
-    return (1 << scale,) + adopt(1 << scale, src, dst, undirected)
+    return (1 << scale,) + adopt_csr_csc(1 << scale, src, dst, undirected)
 
 
 def pieces(count=4096, size=1024, seed=5):
@@ -92,7 +67,7 @@ def pieces(count=4096, size=1024, seed=5):
     perm = rng.permutation(n)
     src = torch.from_numpy(perm[np.concatenate(src)].astype(np.int32)).cuda()
     dst = torch.from_numpy(perm[np.concatenate(dst)].astype(np.int32)).cuda()
-    return (n,) + adopt(n, src, dst)
+    return (n,) + adopt_csr_csc(n, src, dst, False)
 
 
 def cycle(scale):
@@ -100,7 +75,7 @@ def cycle(scale):
     ids = np.random.RandomState(6).permutation(n).astype(np.int32)
     src = torch.from_numpy(ids).cuda()
     dst = torch.from_numpy(np.roll(ids, -1)).cuda()
-    return (n,) + adopt(n, src, dst)
+    return (n,) + adopt_csr_csc(n, src, dst, False)
 
 
 def measure(name, n, A, rp, ci, args):
@@ -113,7 +88,7 @@ def measure(name, n, A, rp, ci, args):
     def run_scc():
         count[0], ms = algorithm.scc(v, A, desc)
         return ms
-    rec["ms"] = median_ms(run_scc, args.iters, args.warmup)
+    rec["ms"] = device_ms(run_scc, args.iters, args.warmup)
     rec["components"] = count[0]
     (rec["trimmed"], rec["pivot_size"], rec["colour_iterations"],
      rec["barriers"]) = algorithm.scc_stats()
@@ -128,39 +103,28 @@ def measure(name, n, A, rp, ci, args):
     rec["largest_component"] = int(np.bincount(want).max())
 
     cv = gb.Vector(n)
-    rec["cc_ms"] = median_ms(lambda: algorithm.cc(cv, A, desc)[1], args.iters, args.warmup)
-    rec["stream_bound_ms"] = (8.0*(n + 1) + 8.0*nnz)/HBM_BYTES_PER_S*1e3
+    rec["cc_ms"] = device_ms(lambda: algorithm.cc(cv, A, desc)[1], args.iters, args.warmup)
+    rec["stream_bound_ms"] = stream_bound_ms(8.0*(n + 1) + 8.0*nnz)
     if rec["equals_checker"]:
         rec["cpu_over_scc"] = rec["cpu_ms"]/rec["ms"]
     else:
         rec.pop("ms")                 # wrong labels get no time
     print(json.dumps(rec), flush=True)
-    del A, v, cv
-    torch.cuda.empty_cache()
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--iters", type=int, default=10)
-    ap.add_argument("--warmup", type=int, default=2)
+    ap = parser(iters=10, warmup=2,
+                only="rmat22_directed, rmat24_directed, rmat22_sym_csc, pieces_directed "
+                     "or cycle")
     ap.add_argument("--cycle-scale", type=int, default=20)
-    ap.add_argument("--only", default=None,
-                    help="rmat22_directed, rmat24_directed, rmat22_sym_csc, "
-                         "pieces_directed or cycle")
     args = ap.parse_args()
     gb.init(0)
-    print(json.dumps({"card": card(), "torch": torch.__version__}), flush=True)
-    builders = [("rmat22_directed", lambda: rmat(22)),
-                ("rmat24_directed", lambda: rmat(24)),
-                ("rmat22_sym_csc", lambda: rmat(22, undirected=True)),
-                ("pieces_directed", pieces),
-                ("cycle", lambda: cycle(args.cycle_scale))]
-    for name, build in builders:
-        if args.only in (None, name):
-            n, A, rp, ci = build()
-            measure(name, n, A, rp, ci, args)
-            del A, rp, ci
-            torch.cuda.empty_cache()
+    header()
+    run([("rmat22_directed", lambda: rmat(22)),
+         ("rmat24_directed", lambda: rmat(24)),
+         ("rmat22_sym_csc", lambda: rmat(22, undirected=True)),
+         ("pieces_directed", pieces),
+         ("cycle", lambda: cycle(args.cycle_scale))], args, measure)
 
 
 if __name__ == "__main__":

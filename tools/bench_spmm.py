@@ -17,19 +17,15 @@ the kernel gathers (mostly from L2).  Plus-times must agree with cuSPARSE within
 MinimumPlus has no cuSPARSE counterpart; its sampled rows (the longest among
 them) must equal a host min-plus exactly.
 """
-import argparse
 import json
-import os
-import sys
 
 import numpy as np
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-
-from bench_mxm import card, grid27, rmat, timed   # noqa: E402
-import graphblast_b200 as gb                      # noqa: E402
-from graphblast_b200 import graphs                # noqa: E402
+# benchlib first: it puts the repository root and tests/ on sys.path
+from benchlib import event_ms, grid27, header, parser, rmat_csr, run
+import graphblast_b200 as gb
+from graphblast_b200 import graphs
 
 
 def compulsory_bytes(m, k, nnz, n):
@@ -56,7 +52,7 @@ def min_plus_agrees(rp, ci, B, got, rows):
     return True
 
 
-def run(name, n, rp, ci, widths, args):
+def measure(name, n, rp, ci, widths, args):
     A = graphs.matrix_from_csr(n, rp, ci)
     nnz = int(ci.numel())
     deg = (rp[1:] - rp[:-1]).float()
@@ -75,15 +71,15 @@ def run(name, n, rp, ci, widths, args):
         rec["compulsory_GB"] = cb/1e9
         rec["gather_GB"] = 4.0*nnz*w/1e9
         for sr in (gb.Semiring.PlusMultiplies, gb.Semiring.MinimumPlus):
-            ms = timed(lambda: gb.mxm(C, None, None, sr, A, Bm, desc), args.iters,
-                       args.warmup)
+            ms = event_ms(lambda: gb.mxm(C, None, None, sr, A, Bm, desc), args.iters,
+                          args.warmup)
             got = torch.from_numpy(C.extract_dense()).cuda()
             key = "plus_times" if sr == gb.Semiring.PlusMultiplies else "min_plus"
             rec[key + "_ms"] = ms
             rec[key + "_GBps"] = cb/ms/1e6
             if sr == gb.Semiring.PlusMultiplies:
-                rec["cusparse_ms"] = timed(lambda: torch.sparse.mm(T, B), args.iters,
-                                           args.warmup)
+                rec["cusparse_ms"] = event_ms(lambda: torch.sparse.mm(T, B), args.iters,
+                                              args.warmup)
                 rec["cusparse_GBps"] = cb/rec["cusparse_ms"]/1e6
                 rec["cusparse_agrees"], _ = plus_times_agrees(T, T, deg, B, got)
             else:
@@ -95,25 +91,12 @@ def run(name, n, rp, ci, widths, args):
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--iters", type=int, default=10)
-    ap.add_argument("--warmup", type=int, default=2)
-    ap.add_argument("--only", default=None, help="rmat22, rmat24 or grid128")
-    args = ap.parse_args()
+    args = parser(iters=10, warmup=2, only="rmat22, rmat24 or grid128").parse_args()
     gb.init(0)
-    print(json.dumps({"card": card(), "torch": torch.__version__}), flush=True)
-    if args.only in (None, "rmat22"):
-        n, rp, ci = rmat(22)
-        run("rmat22", n, rp, ci, [4, 16, 32, 64, 128, 256], args)
-        del rp, ci
-    if args.only in (None, "grid128"):
-        n, rp, ci = grid27(128)
-        run("grid128", n, rp, ci, [32, 128], args)
-        del rp, ci
-    if args.only in (None, "rmat24"):
-        torch.cuda.empty_cache()
-        n, rp, ci = rmat(24)
-        run("rmat24", n, rp, ci, [32, 64], args)
+    header()
+    run([("rmat22", lambda: rmat_csr(22, seed=1), [4, 16, 32, 64, 128, 256]),
+         ("grid128", lambda: grid27(128), [32, 128]),
+         ("rmat24", lambda: rmat_csr(24, seed=1), [32, 64])], args, measure)
 
 
 if __name__ == "__main__":
